@@ -4,6 +4,7 @@
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference]
                     [--gar trmean --nb-workers 25 --nb-byz 10 --dim 1310922] [--no-sweep]
+                    [--dump-outputs DIR]
 
 A "step" is ONE aggregation call over one stack of n worker gradients (fp32, length d per
 GPU).  Default workload = BASELINE.json configs[1]: trimmed mean, n=25, f=10, d=1,310,922
@@ -16,13 +17,18 @@ Per-GPU work is fixed as N grows -> "scaling": "weak"; `value` = N*d / step time
 One JSON line is printed by rank 0 (see the driver contract in the task statement):
   value       params/s with inputs resident in HBM, device-timed (CUDA events, max over ranks)
   roofline    dominant kernel: algorithmic bytes / average per-launch duration vs the measured
-              HBM peak of MEASURED_PEAKS.json
+              HBM peak of MEASURED_PEAKS.json (else the H100 SXM data sheet's 3.35 TB/s)
   e2e         the same metric through the reference-facing call `gars[gar](gradients=<host
               tensors>, f=f)`: pinned host rows -> H2D -> kernel -> D2H of the result, per step
   cpu_baseline  the UNMODIFIED reference's `aggregators.gars[gar].unchecked` on CPU tensors, on the host
-                cores (baseline/_ref; the port oracle/refcost.py only when no reference is present)
+                cores ($BYZ_REFERENCE; the port oracle/refcost.py when no reference is given)
   sweep       (N=1) kernel time / GB/s / roofline fraction of the other rules and sizes
 `--impl reference` times the reference's CPU aggregation alone, on the same workload.
+`--dump-outputs DIR` writes what the timed path returned in its last timed step to
+DIR/aggregate.npy (float32; the inputs are seeded, so runs with the same arguments compare
+output for output).  Above 64 MB it keeps a fixed seeded sample of the coordinates, whose indices
+go to DIR/aggregate_index.npy (float64).  CUDA arm only (the reference arm shrinks d by timing, so
+its inputs are not fixed); with N > 1 it is rank 0's shard of the d axis.
 """
 
 import argparse
@@ -37,8 +43,9 @@ import time
 ROOT = pathlib.Path(__file__).resolve().parent
 sys.path.insert(0, str(ROOT))
 
-L2_BYTES = 126 * 1024 * 1024
-FALLBACK_HBM_GBS = 6650.0   # /opt/skills/guides/B200_PROFILING.md, used only without MEASURED_PEAKS.json
+L2_BYTES = 50 * 1024 * 1024   # H100
+FALLBACK_HBM_GBS = 3350.0     # H100 SXM data sheet, used only without MEASURED_PEAKS.json
+DUMP_BYTES = 64 * 1024 * 1024
 
 # kernels of libbyzagg launched per aggregation call (single device)
 LAUNCHES = dict(average=1, median=1, trmean=1, phocas=1, meamed=1, krum=2, bulyan=2, brute=2, aksel=3, cge=2)
@@ -152,15 +159,7 @@ def peak_hbm():
   try:
     return float(json.loads(path.read_text())["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
   except Exception:
-    return FALLBACK_HBM_GBS, "fallback (B200_PROFILING.md)"
-
-def recorded_traffic(gar, n, f, d):
-  """ dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed ncu capture. """
-  try:
-    table = json.loads((ROOT / "profiles" / "traffic.json").read_text())
-    return table.get(f"{gar}:n{n}:f{f}:d{d}")
-  except Exception:
-    return None
+    return FALLBACK_HBM_GBS, "H100 SXM data sheet (not measured)"
 
 def cpu_info():
   model = "unknown"
@@ -179,8 +178,8 @@ def cpu_info():
 
 def reference_callable(gar):
   """ (fn(rows, f), kind, path): the UNMODIFIED reference's `aggregators.gars[gar].unchecked`
-  (BASELINE.md §4.2; search order $BYZ_REFERENCE, baseline/_ref, /root/reference) — nothing of this
-  repository is on that path — or, only when no reference checkout is present, the port of its
+  (BASELINE.md §4.2; the checkout $BYZ_REFERENCE points at) — nothing of this repository is on
+  that path — or, only when no reference checkout is given, the port of its
   ATen operator sequence (oracle/refcost.py). """
   from oracle import reference
   root, aggregators = reference.load()
@@ -226,7 +225,7 @@ def make_config(gar, n, f, d, world):
   """ The workload description, identical in both arms (the driver compares the dicts). """
   return dict(workload=f"{gar} GAR, n={n} f={f}, d={d} per GPU (BASELINE.json configs[1]: CIFAR-10 empire-cnn shape)",
               gar=gar, n=n, f=f, d=d, parallelism=f"d-sharded x{world}" if world > 1 else "single GPU",
-              l2="GPU arm: inputs rotate over independent [n, d] stacks totalling more than 3x the 126 MB L2; CPU arm: not applicable")
+              l2="GPU arm: inputs rotate over independent [n, d] stacks totalling more than 3x the 50 MB L2; CPU arm: not applicable")
 
 # ---------------------------------------------------------------------------- #
 
@@ -410,8 +409,13 @@ def run_b200(args):
   for k in range(max(args.warmup, 3)):
     step(k)
   barrier()
+  last = {}
+  def timed_step(k):
+    last["out"] = step(k)
   with ClockSampler(local) as clocks:
-    total_ms, _ = time_steps(torch, step, args.steps, pairs=False)     # THE timed region: K steps, two events
+    total_ms, _ = time_steps(torch, timed_step, args.steps, pairs=False)     # THE timed region: K steps, two events
+    if args.dump_outputs and rank == 0:
+      dump_outputs(args.dump_outputs, "aggregate", last["out"].cpu().numpy())   # before any later step rewrites it
     barrier()
     _, per_step = time_steps(torch, step, args.steps, pairs=True)      # second pass: per-launch durations
     barrier()
@@ -441,7 +445,7 @@ def run_b200(args):
   peak, peak_src = peak_hbm()
   alg = algorithmic_bytes(gar, n, f, d)
   achieved = alg / (kernel_ms * 1e-3) / 1e9
-  roofline = dict(bound="hbm", achieved=achieved, peak=peak, unit="GB/s", frac=achieved / peak, traffic=recorded_traffic(gar, n, f, d),
+  roofline = dict(bound="hbm", achieved=achieved, peak=peak, unit="GB/s", frac=achieved / peak,
                   kernel=("k1_sorted" if gar in ("trmean", "phocas", "meamed") else "k1_median" if gar == "median" else "k3_average" if gar == "average" else "k2_pairdist"),
                   algorithmic_bytes=alg, read_only_frac=(n * d * 4) / (kernel_ms * 1e-3) / 1e9 / peak, kernel_ms=kernel_ms,
                   event_pair_ms=event_pair_ms, peak_source=peak_src)
@@ -480,7 +484,7 @@ def run_b200(args):
   probe = h2d_probe(torch, device, n, d)
   e2e = dict(value=world * d / (e2e_ms * 1e-3), unit="params/s", h2d_bytes_per_step=n * d * 4, d2h_bytes_per_step=d * 4,
              h2d_probe=probe, pcie_floor_ms=probe.get("ms"), host_path=bz.engine.host_path_report(device.index), h2d_rate_achieved_gbs=n * d * 4 / (e2e_ms * 1e-3) / 1e9,
-             note="pcie_floor_ms = the faster of one contiguous pinned copy and n pinned row copies of the step's bytes on THIS box, outside the library (PCIe Gen5 x16 nominal: 2.1-2.4 ms); the step adds the kernel (~23 us), the 5 MB result copy and its synchronisation; host_path 'pipeline' = bz_coordinate_host (column chunks: batched H2D of chunk c+1, kernel of chunk c and D2H of chunk c-1 overlap)",
+             note="pcie_floor_ms = the faster of one contiguous pinned copy and n pinned row copies of the step's bytes on THIS box, outside the library; the step adds the kernel, the result copy and its synchronisation; host_path 'pipeline' = bz_coordinate_host (column chunks: batched H2D of chunk c+1, kernel of chunk c and D2H of chunk c-1 overlap)",
              ms_per_step=e2e_ms, ms_per_step_min=min(e2e_each), ms_per_step_median=sorted(e2e_each)[len(e2e_each) // 2], ms_per_step_max=max(e2e_each), steps=e2e_steps, host_buffers="pinned" + (", allocated under the NVML ideal-affinity binding" if numa_local else "") + "; host->device path chosen by measurement (see host_path)", call=f"byzantinemomentum_b200.gars[{gar!r}].unchecked(gradients=<{n} pinned host tensors>, f={f})")
   del host
 
@@ -497,7 +501,7 @@ def run_b200(args):
     line["cpu_baseline"] = dict(value=res["sample_d"] / best, unit="params/s", cores=res["threads"], kind=res["kind"],
                                 sample=f"best of 3 calls ({gar}, n={n}, f={f}) on d={res['sample_d']} of {d} columns", ms_per_call=best * 1e3,
                                 path=res["path"], cpu_model=res["cpu_model"], cpus_allowed=res["cpus_allowed"], torch=res["torch"])
-    # the same operator sequence on CUDA tensors ("PyTorch on B200" incumbent, BASELINE.md §4.5)
+    # the same operator sequence on CUDA tensors ("PyTorch on the GPU" incumbent, BASELINE.md §4.5)
     try:
       from oracle import refcost
       for _ in range(2):
@@ -521,6 +525,20 @@ def run_b200(args):
     print(json.dumps(line), flush=True)
   if dist is not None:
     dist.destroy_process_group()
+
+def dump_outputs(directory, name, values):
+  """ `values` (one output of the timed path) as <directory>/<name>.npy in float32; above DUMP_BYTES, a
+  fixed seeded sample of its coordinates, their indices in <name>_index.npy (float64). """
+  import numpy as np
+  directory = pathlib.Path(directory)
+  directory.mkdir(parents=True, exist_ok=True)
+  values = np.asarray(values, dtype=np.float32).ravel()
+  if values.nbytes > DUMP_BYTES:
+    keep = DUMP_BYTES // (4 + 8)
+    index = np.sort(np.random.default_rng(0).choice(values.size, size=keep, replace=False))
+    np.save(directory / f"{name}_index.npy", index.astype(np.float64))
+    values = values[index]
+  np.save(directory / f"{name}.npy", values)
 
 def sweep(torch, bz, device, peak):
   """ Kernel-level numbers for the other rules / sizes (single GPU; not part of `value`). """
@@ -608,9 +626,16 @@ def main():
   ap.add_argument("--dim", dest="d", type=int, default=1_310_922)
   ap.add_argument("--no-sweep", action="store_true")
   ap.add_argument("--no-sharded", action="store_true", help="skip the `sharded` block (collective path at C3 per GPU + C4 strong scaling; at N = 1 it is the reference line of the series)")
+  ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                  help="write the output of the last timed step to DIR/aggregate.npy (float32, at most 64 MB; "
+                       "CUDA arm only, with N > 1 rank 0's shard)")
   ap.add_argument("--exchange", choices=("auto", "nccl", "p2p"), default="auto",
                   help="N > 1, distance-based rules: all-gather (NCCL) or blocks read in place over NVLink peer memory")
   args = ap.parse_args()
+  if args.steps < 1 or args.warmup < 0:
+    ap.error("--steps must be at least 1 and --warmup at least 0")
+  if args.dump_outputs and args.impl == "reference":
+    ap.error("--dump-outputs applies to the CUDA arm: the reference arm times a d shrunk to its time budget")
   global EXCHANGE
   EXCHANGE = args.exchange
   if args.impl == "reference":

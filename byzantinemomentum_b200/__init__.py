@@ -1,5 +1,5 @@
 # coding: utf-8
-"""byzantinemomentum_b200 — B200-native (sm_100a) Byzantine-robust gradient aggregation.
+"""byzantinemomentum_b200 — H100-native (sm_90a) Byzantine-robust gradient aggregation.
 
 A drop-in for the aggregation hot path of LPD-EPFL/ByzantineMomentum (`aggregators/*.py` as
 called from `attack.py:821-822`): same plugin interface, hand-written CUDA underneath.
@@ -7,7 +7,7 @@ called from `attack.py:821-822`): same plugin interface, hand-written CUDA under
     from byzantinemomentum_b200 import gars
     aggregated = gars["krum"](gradients=list_of_flat_fp32_cuda_tensors, f=5)
 
-    plan = byzantinemomentum_b200.Plan("krum", gradients, f=5)   # prepared call: plan() is ~3 us of host time
+    plan = byzantinemomentum_b200.Plan("krum", gradients, f=5)   # prepared call: plan() is one C call, no sync
 
     import aggregators                              # the unmodified reference
     byzantinemomentum_b200.plugin.install(aggregators)   # registers "b200-<name>" rules

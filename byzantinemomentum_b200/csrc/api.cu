@@ -26,7 +26,7 @@ int sm_count() {
   cudaGetDevice(&dev);
   int& c = cached[dev & 63];
   if (c == 0) cudaDeviceGetAttribute(&c, cudaDevAttrMultiProcessorCount, dev);
-  return c > 0 ? c : 148;
+  return c > 0 ? c : 132;
 }
 
 int check_launch(const char* what) {

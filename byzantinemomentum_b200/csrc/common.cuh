@@ -1,4 +1,4 @@
-// common.cuh — shared device/host helpers of libbyzagg (sm_100a only).
+// common.cuh — shared device/host helpers of libbyzagg (sm_90a only).
 #pragma once
 
 #include <cuda_runtime.h>
@@ -7,8 +7,8 @@
 
 #include "../../include/byzagg.h"
 
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 1000)
-#error "libbyzagg is written for sm_100a (B200) only"
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ != 900)
+#error "libbyzagg is written for sm_90a (H100) only"
 #endif
 
 namespace bz {
@@ -166,8 +166,7 @@ struct OpsFast {
 // is instead computed on the bit patterns as a + b - min (exact: min is bitwise one of the two
 // inputs, so the other one comes out) with two IMADs, which issue on the FMA pipe at the same
 // rate.  `one` / `mone` are 1 and -1 passed as kernel parameters so that ptxas cannot fold
-// the multiply-adds back into an ALU-pipe IADD3.  At the balanced mix (about 2/3 of the full
-// comparators) the comparator throughput is 1.48x that of FMNMX pairs (tools/ub/ce_pipes.cu).
+// the multiply-adds back into an ALU-pipe IADD3 (tools/ub/ce_pipes.cu compares the mixes).
 // NOT valid with NaN inputs (FMNMX then returns neither input) nor under flush-to-zero.
 template <class Mask>
 struct OpsMix {

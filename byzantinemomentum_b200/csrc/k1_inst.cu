@@ -32,7 +32,7 @@ static unsigned persistent_grid(K kernel, size_t smem, int64_t nv, int (&cache)[
     int per_sm = 0, sms = 0;
     cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kK1Threads, smem);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    resident = (per_sm > 0 ? per_sm : 1) * (sms > 0 ? sms : 148);
+    resident = (per_sm > 0 ? per_sm : 1) * (sms > 0 ? sms : 132);
   }
   const int64_t tiles = (nv + kK1Threads - 1) / kK1Threads;
 #if BZ_K1_VARIANT == 2

@@ -37,8 +37,7 @@ constexpr int kK1Threads = BZ_K1_THREADS;
 
 // How a thread walks the coordinates (A/B builds: `make VARIANT=v0 EXTRA=-DBZ_K1_VARIANT=0`):
 //   2 (default)  one logical vector per thread, direct register loads, grid = all tiles.  The
-//                hardware CTA scheduler balances the tail; measured fastest on B200
-//                (profiles/README.md, "K1 walk variants").
+//                hardware CTA scheduler balances the tail.
 //   1            persistent grid-stride loop, direct loads.
 //   0            persistent loop with cp.async staging of the next tile in a per-thread
 //                shared-memory column while the current one is sorted.

@@ -7,8 +7,8 @@
 // is staged in shared memory with cp.async (zero-filled past d), double buffered.  Rows are
 // grouped by 5; a warp owns one group pair (A, B) — a 5x5 block of row pairs (10 pairs on
 // the diagonal) — and sweeps the tile: each lane reads 4 adjacent coordinates of the 10 rows
-// (LDS.128, conflict free) and feeds 25 packed accumulators with FADD2/FFMA2 (sub.f32x2 /
-// fma.rn.f32x2: two coordinates per instruction).  No Gram trick: (a-b)^2 is formed
+// (LDS.128, conflict free) and feeds 25 accumulators, each a pair of coordinates updated with
+// one FADD and one FFMA per coordinate (reduce.cuh).  No Gram trick: (a-b)^2 is formed
 // directly, so aliased rows give an exact 0 and nothing cancels (SURVEY.md §7.2).
 // Every tile (<= 1024 coordinates, i.e. <= 16 terms per fp32 accumulator half) the 25 lane
 // partials are transposed-reduced over the warp (lane p ends with pair p) and added to a

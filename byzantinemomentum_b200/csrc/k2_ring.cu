@@ -2,31 +2,29 @@
 // the rows, every input byte fetched from HBM/L2 exactly once for any n <= 64
 // (krum.py:44-48, bulyan.py:49-54, brute.py:44-45: one pass PER PAIR plus a host sync each).
 //
-// What changed against k2_pairdist.cu (kept for unaligned rows), each point from an ncu finding
-// of round 1 (profiles/README.md):
+// What changed against k2_pairdist.cu (kept for unaligned rows):
 //  * Balanced tasks.  Pairs are cut in tasks of 25 accumulator slots: the 5x5 block of two row
 //    groups (OFF), or a composite of diagonal blocks (COMP: two whole 5-row blocks, 10 pairs each,
 //    plus one 5-cycle of a third block; K5 = two edge-disjoint 5-cycles, so a block split over
 //    two composites costs no extra slot).  n = 25: 10 OFF + 2 COMP = 12 equal warps, 3 per SM
-//    sub-partition (was 10 heavy + 5 light warps: the busiest sub-partition carried 85 of 300
-//    pair slots, now 75).
-//  * Distributed bulk-copy issue.  One thread issuing the n copies of a tile needed ~100 cycles
-//    per copy (dependent constant-bank pointer load, 64-bit add, UBLKCP) = a serial 2500-cycle
-//    loop per 2400-cycle tile: 22 % of the stall samples sat on the `full` barrier.  Now row r
+//    sub-partition (was 10 heavy + 5 light warps).
+//  * Distributed bulk-copy issue.  One thread issuing the n copies of a tile serialises them
+//    (dependent constant-bank pointer load, 64-bit add, UBLKCP per copy).  Now row r
 //    belongs to one warp which keeps its pointer in a register and issues <= 3 copies per tile,
 //    one tile late (the stage freed in the PREVIOUS iteration), so that the `empty` wait before
 //    the refill never blocks in steady state.
 //  * Thread-block clusters + TMA multicast for n > 25.  12 warps hold 12 tasks of accumulators;
 //    n = 51 has 60 tasks.  Instead of several independent CTAs each staging the whole tile
-//    (round 1: 1.92x DRAM traffic, 5x L2->SM traffic), C = ceil(tasks / 12) CTAs of one cluster
+//    (every row read once per CTA), C = ceil(tasks / 12) CTAs of one cluster
 //    work on the SAME tile: every row is fetched once per cluster by one CTA and written into the
 //    shared memory of all C CTAs by the copy itself (cp.async.bulk ... .multicast::cluster); a
 //    consumer releases a stage by arriving on the `empty` barrier of every CTA of the cluster.
 //  * Alias flags instead of self pairs: the distance of an aliased row to itself is 0 or NaN
 //    (x.sub(x).norm() of a row holding NaN/inf); fma(x, 0, acc) over the row gives the same
 //    0 / NaN for 1 operation per coordinate, only for the rows that ARE aliased.
-// Arithmetic is unchanged: (a-b)^2 formed directly (no Gram trick), packed fp32 (FADD2/FFMA2),
-// <= 16 terms per fp32 accumulator half, then a transposed warp reduction into fp64.
+// Arithmetic is unchanged: (a-b)^2 formed directly (no Gram trick), coordinate pairs updated with
+// one FADD and one FFMA per coordinate (reduce.cuh), a bounded number of fp32 terms per accumulator
+// half, then a transposed warp reduction into fp64.
 #include <cstdlib>
 
 #include "dist.cuh"
@@ -43,7 +41,7 @@ constexpr int kRWarpsSmall = 6;         // ... or 6, two CTAs per SM, when all t
                                         // task takes the same time per tile whatever n, so small n is bound by tiles per
                                         // SM per unit time, and two resident CTAs walk two tile streams at once
 constexpr int kRWarpsWide = 16;         // ... or 16 (four per scheduler, 128 registers) in the clusters of n > 35: the same 60 tasks of
-                                        // n = 51 then need 4 CTAs instead of 5, and 4-CTA clusters fill 144 of the 148 SMs (5-CTA: 130)
+                                        // n = 51 then need 4 CTAs instead of 5
 constexpr int kRThreads = kRWarps * 32;
 constexpr int kRSlots = kG * kG;
 constexpr size_t kRSmemBudget = 226 * 1024;
@@ -451,8 +449,8 @@ k2_ring(const __grid_constant__ RowTable rows, const __grid_constant__ SelfList 
     __syncwarp();
     if (lane == 0) {
       // the values read from the stage have been consumed by the arithmetic above: a plain
-      // (relaxed) arrive is enough to hand the stage back; `.release.cluster` here compiled to
-      // MEMBAR + ERRBAR per arrive and took 37 % of the stall samples at n = 51
+      // (relaxed) arrive is enough to hand the stage back; `.release.cluster` here would add a
+      // fence (MEMBAR) per arrive
       if (!CLUSTER) mbar_arrive(&empty[s]);
       else
         for (int r = 0; r < C; ++r) mbar_arrive_remote(&empty[s], (unsigned)r);
@@ -528,8 +526,8 @@ k2_ring(const __grid_constant__ RowTable rows, const __grid_constant__ SelfList 
   }
   if (tail.kind != 0) {
     // Two-level, fixed-order reduction of the per-cluster blocks followed by the scoring step, all
-    // inside this launch.  One CTA pulling 148 blocks alone is bandwidth-starved (a single SM:
-    // ~10 us for 740 KB at n = 25), so the blocks are first summed by groups of kTailGroup clusters
+    // inside this launch.  One CTA pulling one block per cluster alone is bandwidth-starved
+    // (a single SM pulls ~740 KB at n = 25), so the blocks are first summed by groups of kTailGroup clusters
     // — by whichever CTA of the group finishes last, but always in index order: deterministic —
     // and the last group to finish sums the <= 10 group blocks and runs the selection in the
     // shared memory the ring no longer needs (every other CTA is past its ring by then).

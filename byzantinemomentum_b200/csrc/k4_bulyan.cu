@@ -102,8 +102,8 @@ k4_bulyan_static(const __grid_constant__ RowTable rows, const Geom g, const int3
   // Stage 1 (bulyan.py:66-70, scores never updated): selected[i] = (0 + v[i] + ... + v[M_MAX-1]) / (M_MAX - i).
   // The THETA chains start at different rows, so no partial sum can be shared without changing the
   // rounding: sum(M_MAX - i) additions per coordinate (156 for n = 25, 625 for n = 51) and THETA
-  // divisions make this kernel instruction bound.  With two coordinates per thread both go through
-  // packed fp32 instructions (add.rn.f32x2: the same IEEE addition per lane) and the divisions by the
+  // divisions make this kernel instruction bound.  With two coordinates per thread the additions go
+  // through the pair helpers (`add2`: one IEEE addition per lane) and the divisions by the
   // compile-time row counts through `div_small2` (exact, reduce.cuh).
   float sel[VEC][THETA];
   if (VEC == 2) {

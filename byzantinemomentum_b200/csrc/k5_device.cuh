@@ -32,8 +32,8 @@ struct PeerParts {
 // entries t, t + T, ... and adds its class in ascending p; the classes are then added in
 // ascending order.  The order depends only on (nparts, slices): bitwise reproducible, and the
 // same on every rank of the sharded path.  All loads of a thread are independent across
-// entries, so a thread keeps several in flight (the naive per-entry loop over 148 parts cost
-// ~20 us of pure latency).
+// entries, so a thread keeps several in flight (a naive per-entry loop over one part per SM
+// is pure latency).
 template <class Parts>
 __device__ void block_sum_parts(const Parts& parts, int nparts, int len, int slices,
                                 double* __restrict__ scratch, double* __restrict__ out) {

@@ -187,8 +187,9 @@ static void launch_bucket(const RowTable& rows, int n, const Geom& g, float* avg
 
 void launch_study(const RowTable& rows, int n, const float* const* host_rows, int64_t d, float* avg,
                   double* stats, double* parts, unsigned* bits, cudaStream_t st) {
-  // widest vector that keeps the n x VEC values plus the accumulators in registers
-  const int want = n <= 16 ? 4 : n <= 32 ? 2 : 1;
+  // widest vector that keeps the n x VEC values plus the accumulators in registers (on sm_90,
+  // 8 < n <= 16 with VEC = 4 spills under the two-CTAs-per-SM bound)
+  const int want = n <= 8 ? 4 : n <= 32 ? 2 : 1;
   const Geom g = make_geom(host_rows, n, avg, nullptr, d, want);
   int64_t grid = (g.nv + kStThreads - 1) / kStThreads;
   const int64_t cap = (int64_t)sm_count() * 2;
@@ -200,7 +201,7 @@ void launch_study(const RowTable& rows, int n, const float* const* host_rows, in
   cudaMemsetAsync(bits, 0, 2 * sizeof(unsigned), st);      // max |avg| pattern, ticket counter
   const unsigned gr = (unsigned)grid;
   if (n <= 8)       launch_bucket<8, 4>(rows, n, g, avg, parts, bits, stats, gr, st);
-  else if (n <= 16) launch_bucket<16, 4>(rows, n, g, avg, parts, bits, stats, gr, st);
+  else if (n <= 16) launch_bucket<16, 2>(rows, n, g, avg, parts, bits, stats, gr, st);
   else if (n <= 24) launch_bucket<24, 2>(rows, n, g, avg, parts, bits, stats, gr, st);
   else if (n <= 32) launch_bucket<32, 2>(rows, n, g, avg, parts, bits, stats, gr, st);
   else if (n <= 48) launch_bucket<48, 1>(rows, n, g, avg, parts, bits, stats, gr, st);

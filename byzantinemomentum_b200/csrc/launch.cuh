@@ -15,8 +15,7 @@ namespace bz {
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 // In the PRIMARY kernel, at its start: dependents launched with `launch_after` may be scheduled as soon as
 // SM resources free up (they still block in pdl_wait() until this whole grid has completed and flushed).
-// Used by K1 (back-to-back calls of the coordinate-wise rules: +8 %); measured HARMFUL in the distance pass
-// (profiles/README.md), which therefore does not trigger early.
+// Used by K1 (back-to-back calls of the coordinate-wise rules); the distance pass does not trigger early.
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 #endif
 template <class... Params, class... Args>

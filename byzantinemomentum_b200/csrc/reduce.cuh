@@ -7,34 +7,35 @@ namespace bz {
 
 typedef unsigned long long u64;
 
-// Packed fp32 pairs (two coordinates per instruction: SASS FADD2 / FFMA2)
-__device__ __forceinline__ u64 sub2(u64 a, u64 b) {
-  u64 d;
-  asm("sub.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-__device__ __forceinline__ u64 fma2(u64 a, u64 b, u64 c) {
-  u64 d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
-}
-__device__ __forceinline__ u64 add2(u64 a, u64 b) {
-  u64 d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-__device__ __forceinline__ u64 mul2(u64 a, u64 b) {
-  u64 d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
+// fp32 pairs: two coordinates in one 64-bit register pair.  sm_90 has no packed fp32 arithmetic
+// (f32x2), so each helper issues one IEEE-rounded scalar FADD / FMUL / FFMA per lane; the scalar
+// pipe already retires 128 fp32 lanes per clock per SM, so nothing is lost against the pair form.
 __device__ __forceinline__ u64 pack2(float lo, float hi) {
-  u64 d;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(d) : "f"(lo), "f"(hi));
-  return d;
+  return (u64)__float_as_uint(lo) | ((u64)__float_as_uint(hi) << 32);
 }
 __device__ __forceinline__ void unpack2(u64 v, float& lo, float& hi) {
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
+  lo = __uint_as_float((unsigned)v);
+  hi = __uint_as_float((unsigned)(v >> 32));
+}
+__device__ __forceinline__ u64 sub2(u64 a, u64 b) {
+  float a0, a1, b0, b1;
+  unpack2(a, a0, a1); unpack2(b, b0, b1);
+  return pack2(__fsub_rn(a0, b0), __fsub_rn(a1, b1));
+}
+__device__ __forceinline__ u64 fma2(u64 a, u64 b, u64 c) {
+  float a0, a1, b0, b1, c0, c1;
+  unpack2(a, a0, a1); unpack2(b, b0, b1); unpack2(c, c0, c1);
+  return pack2(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
+}
+__device__ __forceinline__ u64 add2(u64 a, u64 b) {
+  float a0, a1, b0, b1;
+  unpack2(a, a0, a1); unpack2(b, b0, b1);
+  return pack2(__fadd_rn(a0, b0), __fadd_rn(a1, b1));
+}
+__device__ __forceinline__ u64 mul2(u64 a, u64 b) {
+  float a0, a1, b0, b1;
+  unpack2(a, a0, a1); unpack2(b, b0, b1);
+  return pack2(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
 }
 
 // IEEE division of two lanes by a small positive integer m known at compile time (after unrolling),
@@ -72,17 +73,22 @@ __device__ __forceinline__ float half_sum(u64 v) {
 
 
 // Transposed warp reduction: on return, lane L holds sum over lanes of v[L] (v has 32 slots).
-__device__ __forceinline__ float transpose_reduce(float (&v)[32], int lane) {
+// The halving step is a template parameter so that every loop below has a constant trip count
+// and unrolls fully: a `for (h = 16; h >= 1; h >>= 1)` loop is not always unrolled for sm_90,
+// and v[] then lives in local memory.
+template <int H>
+__device__ __forceinline__ void transpose_step(float (&v)[32], int lane) {
+  const bool up = (lane & H) != 0;
 #pragma unroll
-  for (int h = 16; h >= 1; h >>= 1) {
-    const bool up = (lane & h) != 0;
-#pragma unroll
-    for (int j = 0; j < h; ++j) {
-      const float send = up ? v[j] : v[j + h];
-      const float keep = up ? v[j + h] : v[j];
-      v[j] = __fadd_rn(keep, __shfl_xor_sync(0xffffffffu, send, h));
-    }
+  for (int j = 0; j < H; ++j) {
+    const float send = up ? v[j] : v[j + H];
+    const float keep = up ? v[j + H] : v[j];
+    v[j] = __fadd_rn(keep, __shfl_xor_sync(0xffffffffu, send, H));
   }
+  if constexpr (H > 1) transpose_step<H / 2>(v, lane);
+}
+__device__ __forceinline__ float transpose_reduce(float (&v)[32], int lane) {
+  transpose_step<16>(v, lane);
   return v[0];
 }
 

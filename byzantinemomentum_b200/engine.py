@@ -73,8 +73,8 @@ _copy_lanes = {}
 
 class _HostPath:
   """ How host rows reach the GPU is decided by MEASUREMENT, per device: the right answer differs between
-  boxes of the same model (profiles/README.md: pinned rows on the far socket copy at 8.5 GB/s on one
-  stream and at 53 GB/s on four; on other boxes four streams are the slow ones).  Candidates:
+  boxes of the same model (pinned rows on the far socket can copy several times faster over four streams
+  than over one; on other boxes four streams are the slow ones).  Candidates:
     "lanes"     the row copies spread over 4 streams,
     "lane"      the row copies on the current stream,
     "batch"     `bz_stage_rows`: the row copies as ONE cudaMemcpyBatchAsync on a copy stream (a separate
@@ -110,7 +110,7 @@ class _HostPath:
 
 _host_paths = {}
 forced_host_path = None      # tests / A-B runs: pin the host path ("lanes", "lane", "pipeline") instead of measuring
-_PIPELINE_CHUNKS = 4       # measured (profiles/r02_e2e_pipeline_ab.txt): 2 .. 8 within 1 %, 1 and 16+ slower
+_PIPELINE_CHUNKS = 4       # column chunks of the host pipeline: H2D, kernel and D2H of three chunks overlap
 _RULE_CODES = dict(average=0, median=1, trmean=2, phocas=3, meamed=4)      # BZ_RULE_*
 
 def host_path_report(device_index=None):
@@ -192,7 +192,7 @@ def _prepare(gradients, single_pass=False):
     return prep
   first, contiguous = _validate(gradients)
   if not torch.cuda.is_available():
-    raise _lib.LibraryError("no CUDA device available: byzantinemomentum_b200 runs on B200 GPUs only (no CPU fallback)")
+    raise _lib.LibraryError("no CUDA device available: byzantinemomentum_b200 runs on H100 (sm_90a) GPUs only (no CPU fallback)")
   _lib.lib()
   prep = _Prepared()
   prep.host_mode = None

@@ -1,4 +1,4 @@
-/* byzagg.h — C ABI of libbyzagg (B200 / sm_100a Byzantine-robust gradient aggregation).
+/* byzagg.h — C ABI of libbyzagg (H100 / sm_90a Byzantine-robust gradient aggregation).
  *
  * Drop-in boundary for the aggregation rules (GARs) of LPD-EPFL/ByzantineMomentum.
  * Each entry point replaces one Python/ATen implementation in the reference (citations

@@ -2,8 +2,8 @@
 """CPU cost model of the reference: the same ATen operator sequence, on CPU tensors.
 
 TEST / BENCH INFRASTRUCTURE ONLY (see `oracle/byzoracle.py` for the rules on who may import
-`oracle/`).  The reference cannot travel to the GPU box (`/root/reference` does not exist
-there), so `bench.py --impl reference` and `bench.py`'s `cpu_baseline` time THIS module on the
+`oracle/`).  The reference is not part of this repository, so where $BYZ_REFERENCE does not point at a
+checkout `bench.py --impl reference` and `bench.py`'s `cpu_baseline` time THIS module on the
 box's host cores: each function issues the ATen calls the reference's rule issues
 (`stack`, `sort`, `median`, `topk`, per-pair `sub`/`norm`/`.item()`, Python-level scoring),
 so its run time is the reference's run time on that host.  Its results are checked against

@@ -4,10 +4,10 @@
 Only `tests/`, `__graft_entry__.smoke()` and `bench.py`'s CPU legs (`--impl reference`,
 `cpu_baseline`) may import this module; nothing under `byzantinemomentum_b200/` does.
 
-Search order (BASELINE.md §4.2): `$BYZ_REFERENCE`, `<repo>/baseline/_ref` (a verbatim copy made by
-`tools/install_ref.sh`; git-ignored, but it travels to the GPU box with the gpurun snapshot),
-`/root/reference` (build container only).  A candidate counts when it holds
-`aggregators/__init__.py` and `attack.py`.
+The reference is never copied into this repository: it is found through `$BYZ_REFERENCE`, the
+root of a ByzantineMomentum checkout, which counts when it holds `aggregators/__init__.py` and
+`attack.py`.  Without it the callers use what the repository records instead (the goldens under
+`tests/golden/`, the operator-sequence port `oracle/refcost.py`).
 
 Importing the reference's `tools` package rewires `sys.stdout`, `sys.stderr` and `sys.excepthook`
 (tools/__init__.py:215-216,246); `load()` restores them, so a test or the bench keeps its own
@@ -27,8 +27,6 @@ def candidates():
   out = []
   if env:
     out.append(pathlib.Path(env))
-  out.append(ROOT / "baseline" / "_ref")
-  out.append(pathlib.Path("/root/reference"))
   return out
 
 def find_root():

@@ -14,15 +14,8 @@ if str(ROOT) not in sys.path:
 
 GOLDEN_DIR = ROOT / "tests" / "golden"
 
-def reference_root():
-  """ Root of the unmodified reference ($BYZ_REFERENCE, baseline/_ref, /root/reference) or None. """
-  from oracle import reference
-  return reference.find_root()
-
-needs_reference = pytest.mark.skipif(reference_root() is None, reason="no reference checkout on this box (tools/install_ref.sh)")
-
 def pytest_configure(config):
-  config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with `-m gpu`)")
+  config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with `-m gpu`)")
 
 class Golden:
   """One golden fixture: input rows + the reference's recorded outputs."""

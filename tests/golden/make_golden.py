@@ -1,11 +1,9 @@
 #!/usr/bin/env python3
 # coding: utf-8
 """Generate the golden fixtures `tests/golden/golden_*.npz` by running the UNMODIFIED
-reference (`/root/reference`, or $BYZ_REFERENCE) on seeded inputs.
+reference ($BYZ_REFERENCE: the root of a ByzantineMomentum checkout) on seeded inputs:
 
-Run in the build container only (the reference does not exist on the GPU box):
-
-    python tests/golden/make_golden.py
+    BYZ_REFERENCE=<reference checkout> python tests/golden/make_golden.py
 
 Each fixture holds, per case: the [n, d] fp32 input rows (Byzantine rows last; in the
 reference call they are ONE tensor object repeated, as `attacks/identical.py:86` produces),
@@ -24,7 +22,7 @@ import sys
 import numpy as np
 import torch
 
-REF = os.environ.get("BYZ_REFERENCE", "/root/reference")
+REF = os.environ["BYZ_REFERENCE"]
 sys.path.insert(0, REF)
 _stdout, _stderr, _hook = sys.stdout, sys.stderr, sys.excepthook
 import aggregators  # noqa: E402  (wraps stdout/stderr at import: tools/__init__.py:215-216,246)
@@ -97,6 +95,19 @@ CASES = [
   ("empire_n33_d777", "empire", 33, 7, 777, 120, [7, 16]),
   ("iid_n19_d100", "iid", 19, 0, 100, 121, [1, 4, 9]),
 ]
+
+# Further stacks with other shapes and seeds than CASES, three seeds each -> `live/golden_live_*.npz`
+# (`tests/test_oracle_live_reference.py`; kept apart so that the GPU golden tests do not pick them up)
+LIVE_CASES = [
+  ("live_iid_n13", "iid", 13, 3, 211, 9001, [1, 2, 3, 5]),
+  ("live_empire_n17", "empire", 17, 4, 333, 9002, [2, 3, 4, 7]),
+  ("live_little_n10", "little", 10, 2, 97, 9003, [1, 2, 3]),
+  ("live_nan_n9", "nan", 9, 2, 65, 9004, [1, 2, 3]),
+  ("live_inf_n15", "inf", 15, 3, 130, 9005, [1, 3, 5]),
+  ("live_quant_n21", "quant", 21, 4, 96, 9006, [2, 4, 9]),
+  ("live_iid_n40", "iid", 40, 9, 75, 9007, [3, 9, 18]),
+]
+LIVE_CASES = [(f"{name}_s{k}", kind, n, nb, d + 7 * k, seed + 100 * k, fs) for (name, kind, n, nb, d, seed, fs) in LIVE_CASES for k in range(3)]
 
 def module(name):
   return sys.modules["aggregators." + name]
@@ -182,9 +193,10 @@ def run_case(name, kind, n, nb, d, seed, fs):
 def main():
   torch.set_num_threads(1)  # thread-count independent results where ATen's order depends on it
   total = 0
-  for case in CASES:
+  (HERE / "live").mkdir(exist_ok=True)
+  for case in CASES + LIVE_CASES:
     data = run_case(*case)
-    path = HERE / f"golden_{case[0]}.npz"
+    path = HERE / ("live" if case in LIVE_CASES else ".") / f"golden_{case[0]}.npz"
     np.savez_compressed(path, **data)
     total += path.stat().st_size
     man = json.loads(str(data["manifest"]))

@@ -5,7 +5,7 @@
 `golden_*.npz` fixture, split the way attack.py:846-848 calls it: all rows ("sampled"),
 the honest rows, the Byzantine rows (which may be an empty list).
 
-Run in the build container only (the reference does not exist on the GPU box):
+Run with $BYZ_REFERENCE set to the root of a ByzantineMomentum checkout:
 
     python tests/golden/make_study_golden.py
 """
@@ -18,7 +18,7 @@ import sys
 import numpy as np
 import torch
 
-REF = os.environ.get("BYZ_REFERENCE", "/root/reference")
+REF = os.environ["BYZ_REFERENCE"]
 sys.path.insert(0, REF)
 _stdout, _stderr, _hook = sys.stdout, sys.stderr, sys.excepthook
 import tools  # noqa: E402  (wraps stdout/stderr at import: tools/__init__.py:215-216,246)

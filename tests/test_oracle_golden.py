@@ -1,6 +1,6 @@
 # coding: utf-8
 """Pin the NumPy oracle (`oracle/byzoracle.py`) against outputs of the reference itself
-(`tests/golden/*.npz`, produced by `tests/golden/make_golden.py` from /root/reference).
+(`tests/golden/*.npz`, produced by `tests/golden/make_golden.py` from the reference).
 CPU-only; part of the `-m "not gpu"` suite."""
 
 import math

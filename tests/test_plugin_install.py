@@ -1,8 +1,7 @@
 # coding: utf-8
 """`plugin.install` against a stand-in with the reference registry's interface (`gars`,
-`register`, `make_gar`: aggregators/__init__.py:42-86), so that the registration logic is also
-covered on boxes without the reference (the GPU box); `tests/test_reference_integration.py` runs
-the same against the real package in the build container."""
+`register`, `make_gar`: aggregators/__init__.py:42-86), so that the registration logic is
+covered without the reference's code."""
 
 import types
 

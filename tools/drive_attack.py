@@ -135,9 +135,9 @@ def run_attack(path, fuse, helper, fuse_study=False):
   return scope
 
 def find_reference(root):
-  """ $BYZ_REFERENCE, <repo>/baseline/_ref (tools/install_ref.sh), /root/reference: the first that holds attack.py. """
+  """ $BYZ_REFERENCE when it holds attack.py. """
   import os
-  places = ([pathlib.Path(os.environ["BYZ_REFERENCE"])] if os.environ.get("BYZ_REFERENCE") else []) + [root / "baseline" / "_ref", pathlib.Path("/root/reference")]
+  places = ([pathlib.Path(os.environ["BYZ_REFERENCE"])] if os.environ.get("BYZ_REFERENCE") else [])
   for path in places:
     if (path / "aggregators" / "__init__.py").exists() and (path / "attack.py").exists():
       return path.resolve()
@@ -145,7 +145,7 @@ def find_reference(root):
 
 def main():
   parser = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
-  parser.add_argument("--reference", default=None, help="root of the ByzantineMomentum checkout (default: $BYZ_REFERENCE, baseline/_ref, /root/reference)")
+  parser.add_argument("--reference", default=None, help="root of the ByzantineMomentum checkout (default: $BYZ_REFERENCE)")
   parser.add_argument("--count-calls", action="store_true", help="count the calls of every registered rule and its influence(); print `gar-calls <tag> <name> <calls> <influence calls>` lines after each run")
   parser.add_argument("--shape", default="mnist", choices=sorted(SHAPES), help="shape of the synthetic samples")
   parser.add_argument("--override", action="store_true", help="replace the stock rules instead of adding b200-<name>")
@@ -163,7 +163,7 @@ def main():
   if args.reference is None:
     ref = find_reference(root)
     if ref is None:
-      raise SystemExit("no reference found (run tools/install_ref.sh or pass --reference)")
+      raise SystemExit("no reference found (set $BYZ_REFERENCE or pass --reference)")
   else:
     ref = pathlib.Path(args.reference).resolve()
   sys.path.insert(0, str(ref))

@@ -47,11 +47,8 @@ def main():
   ap.add_argument("--no-alias", action="store_true")
   ap.add_argument("--only", default=None, choices=("legacy", "ring"))
   args = ap.parse_args()
-  peak = 6572.2
-  try:
-    peak = json.load(open(pathlib.Path(__file__).resolve().parent.parent / "MEASURED_PEAKS.json"))["hbm_gbs"]
-  except Exception:
-    pass
+  from bench import peak_hbm
+  peak = peak_hbm()[0]          # MEASURED_PEAKS.json, else the H100 SXM data sheet
   if args.cases:
     cases = [tuple(int(v) for v in c.split(":")) for c in args.cases.split(",")]
   elif args.quick:
@@ -78,8 +75,8 @@ def main():
       reps = 50 if n * d < 2e8 else 10
       rec[mode + "_us"] = timed(lambda k: block(stacks[k]), sets, reps)
       rec[mode + "_hbm_frac"] = n * d * 4 / (rec[mode + "_us"] * 1e-6) / 1e9 / peak
-    # FP32 pipe floor: n(n-1) lane-ops per coordinate at 128 lanes/clk/SM, 148 SMs, 1.9 GHz
-    rec["fp_floor_us"] = n * (n - 1) * d / (148 * 128 * 1.9e9) * 1e6
+    # FP32 pipe floor: n(n-1) lane-ops per coordinate at 128 lanes/clk/SM, 132 SMs, 1.98 GHz (H100 SXM)
+    rec["fp_floor_us"] = n * (n - 1) * d / (132 * 128 * 1.98e9) * 1e6
     rec["hbm_floor_us"] = n * d * 4 / (peak * 1e9) * 1e6
     results.append(rec)
     print(json.dumps(rec), flush=True)

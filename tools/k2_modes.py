@@ -6,7 +6,7 @@ TMA K2 of tools/experiments/k2_producer_warp_and_row_blocks.patch under its issu
 issues every copy, bit 2 = the producer is warp 0 (the oldest warp, scheduler priority) instead of
 the last warp.  2 and 4 tiles per CTA need no `empty` wait at all (4 stages), so the step from
 4 to 5 tiles isolates that wait.  Apply the patch, rebuild, then:
-    gpurun --timeout 200 -- 'timeout 150 python tools/k2_modes.py'
+    python tools/k2_modes.py
 """
 import os, sys, pathlib, time
 sys.path.insert(0, str(pathlib.Path(__file__).resolve().parent.parent))
@@ -14,8 +14,9 @@ import torch
 import byzantinemomentum_b200 as bz
 dev = torch.device("cuda", 0)
 n = 25
+sms = torch.cuda.get_device_properties(dev).multi_processor_count
 for tiles in (2, 4, 5, 8, 16):
-  d = 148 * 512 * tiles
+  d = sms * 512 * tiles
   rows = [torch.randn(d, device=dev) for _ in range(n)]
   for mode in (0, 1, 2, 3, 4, 5):
     os.environ["BYZAGG_K2_MODE"] = str(mode)

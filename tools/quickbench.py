@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
 # coding: utf-8
 """Quick kernel timing on one GPU (development aid; bench.py is the contract)."""
-import json, sys, time, pathlib
+import sys, time, pathlib
 sys.path.insert(0, str(pathlib.Path(__file__).resolve().parent.parent))
 import torch
 import byzantinemomentum_b200 as bz
@@ -18,10 +18,8 @@ def timeit(fn, iters=20, warmup=3):
   return ts[len(ts) // 2], ts[0]
 
 def main():
-  peak = 6572.2
-  try:
-    peak = json.load(open(pathlib.Path(__file__).resolve().parent.parent / "MEASURED_PEAKS.json"))["hbm_gbs"]
-  except Exception: pass
+  from bench import peak_hbm
+  peak = peak_hbm()[0]          # MEASURED_PEAKS.json, else the H100 SXM data sheet
   dev = torch.device("cuda", 0)
   bz.config.strict_status = "--nostrict" not in sys.argv
   cases = []

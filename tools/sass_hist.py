@@ -1,9 +1,9 @@
 #!/usr/bin/env python3
 # coding: utf-8
 """Opcode histogram of the hot kernels in libbyzagg.so (cuobjdump -sass), the tracked evidence that
-the kernels are sm_100a code using TMA bulk copies (UBLKCP), mbarriers (SYNCS), packed fp32
-(FADD2 / FFMA2), dual-pipe comparators (FMNMX + IMAD) and no tensor-core instruction.
-    python tools/sass_hist.py > profiles/r02_sass_opcodes.txt"""
+the kernels are sm_90a code using TMA bulk copies (UBLKCP), mbarriers (SYNCS), fp32 FADD / FFMA,
+dual-pipe comparators (FMNMX + IMAD) and no tensor-core instruction.
+    python tools/sass_hist.py"""
 import collections, pathlib, re, subprocess, sys
 ROOT = pathlib.Path(__file__).resolve().parent.parent
 lib = ROOT / "byzantinemomentum_b200" / "libbyzagg.so"
@@ -23,6 +23,6 @@ for pat in WANT:
       total = sum(ops.values())
       demangled = subprocess.run(["c++filt", name], capture_output=True, text=True).stdout.strip()
       print(f"\n## {demangled[:150]}\n   {total} SASS instructions; top opcodes: " + ", ".join(f"{o} {c}" for o, c in ops.most_common(14)))
-      flags = {k: ops.get(k, 0) for k in ("UBLKCP", "SYNCS", "FADD2", "FFMA2", "FMNMX", "IMAD", "LDS", "LDG", "LDGSTS", "ATOM", "ATOMG", "RED", "HMMA", "UTCHMMA", "UTCQMMA", "LDTM")}
-      print("   markers: " + ", ".join(f"{k} {v}" for k, v in flags.items() if v or k in ("HMMA", "UTCHMMA")))
+      flags = {k: ops.get(k, 0) for k in ("UBLKCP", "SYNCS", "FADD", "FFMA", "FMNMX", "IMAD", "LDS", "LDG", "LDGSTS", "ATOM", "ATOMG", "RED", "HMMA", "HGMMA")}
+      print("   markers: " + ", ".join(f"{k} {v}" for k, v in flags.items() if v or k in ("HMMA", "HGMMA")))
       break

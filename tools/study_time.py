@@ -55,7 +55,7 @@ def main():
   stock = library_avg_dev_max
   try:
     import os
-    places = ([pathlib.Path(os.environ["BYZ_REFERENCE"])] if os.environ.get("BYZ_REFERENCE") else []) + [ROOT / "baseline" / "_ref", pathlib.Path("/root/reference")]
+    places = ([pathlib.Path(os.environ["BYZ_REFERENCE"])] if os.environ.get("BYZ_REFERENCE") else [])
     ref = next((q.resolve() for q in places if (q / "tools" / "__init__.py").exists() and (q / "attack.py").exists()), None)
     if ref is not None:
       sys.path.insert(0, str(ref))

@@ -1,7 +1,7 @@
-// Microbenchmark: compare-exchange throughput on B200 when the max half of a comparator is
+// Microbenchmark: compare-exchange throughput on H100 when the max half of a comparator is
 // (a) FMNMX (ALU pipe, like the min), or (b) computed as a + b - min with two IMADs whose
 // multipliers live in registers (FMA pipe), for different mixing ratios.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o ce_pipes ce_pipes.cu && ./ce_pipes
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o ce_pipes ce_pipes.cu && ./ce_pipes
 #include <cstdio>
 #include <cuda_runtime.h>
 
@@ -44,10 +44,10 @@ template <int MODE>
 float run(const float* in, float* out, int iters) {
   cudaEvent_t a, b;
   cudaEventCreate(&a); cudaEventCreate(&b);
-  bench<MODE><<<148 * 8, 128>>>(in, out, 10, 1, -1);
+  bench<MODE><<<132 * 8, 128>>>(in, out, 10, 1, -1);
   cudaDeviceSynchronize();
   cudaEventRecord(a);
-  bench<MODE><<<148 * 8, 128>>>(in, out, iters, 1, -1);
+  bench<MODE><<<132 * 8, 128>>>(in, out, iters, 1, -1);
   cudaEventRecord(b);
   cudaEventSynchronize(b);
   float ms;
@@ -56,12 +56,12 @@ float run(const float* in, float* out, int iters) {
 }
 
 int main() {
-  const size_t n = (size_t)148 * 8 * 128 * 16;
+  const size_t n = (size_t)132 * 8 * 128 * 16;
   float *in, *out;
   cudaMalloc(&in, n * 4); cudaMalloc(&out, n * 4);
   cudaMemset(in, 0, n * 4);
   const int iters = 2000;
-  const double ces = (double)148 * 8 * 128 * iters * 8 * 15;
+  const double ces = (double)132 * 8 * 128 * iters * 8 * 15;
   const float t0 = run<0>(in, out, iters), t1 = run<1>(in, out, iters), t2 = run<2>(in, out, iters), t3 = run<3>(in, out, iters);
   printf("all FMNMX      : %.3f ms  %.1f G CE/s\n", t0, ces / t0 / 1e6);
   printf("all IMAD max   : %.3f ms  %.1f G CE/s\n", t1, ces / t1 / 1e6);
