@@ -101,6 +101,9 @@ __device__ __forceinline__ void load_rows(const RowTable& rows, int64_t e0, int6
   }
 }
 
+// Bring the line holding p into L2 (no register result, no effect on what later loads return).
+__device__ __forceinline__ void prefetch_l2(const float* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
+
 // Single-row variant (K3): same semantics.
 template <int VEC>
 __device__ __forceinline__ void load_vec(const float* row, int64_t e0, int64_t d, bool full, float (&o)[VEC]) {

@@ -20,26 +20,18 @@
 
 namespace bz {
 
-// Persistent grid: as many CTAs as are resident at once (occupancy x SMs), or fewer when the
-// launch has fewer tiles.  The occupancy query is cached per kernel instantiation and device.
+// One CTA per tile of kK1Threads vectors.  The closest modes' sorted columns may need more than
+// 48 KB of shared memory: opted in once per kernel instantiation and device.
 template <class K>
-static unsigned persistent_grid(K kernel, size_t smem, int64_t nv, int (&cache)[64]) {
+static unsigned tile_grid(K kernel, size_t smem, int64_t nv, unsigned long long& opted) {
   int dev = 0;
   cudaGetDevice(&dev);
-  int& resident = cache[dev & 63];
-  if (resident == 0) {
-    if (smem > 48 * 1024) cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    int per_sm = 0, sms = 0;
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kK1Threads, smem);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    resident = (per_sm > 0 ? per_sm : 1) * (sms > 0 ? sms : 132);
+  const unsigned long long bit = 1ull << (dev & 63);
+  if (smem > 48 * 1024 && !(opted & bit)) {
+    cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    opted |= bit;
   }
-  const int64_t tiles = (nv + kK1Threads - 1) / kK1Threads;
-#if BZ_K1_VARIANT == 2
-  return (unsigned)tiles;
-#else
-  return (unsigned)(tiles < resident ? tiles : resident);
-#endif
+  return (unsigned)((nv + kK1Threads - 1) / kK1Threads);
 }
 
 #if BZ_PART < 4
@@ -47,15 +39,11 @@ static unsigned persistent_grid(K kernel, size_t smem, int64_t nv, int (&cache)[
 template <int N>
 static void launch_median_n(const RowTable& rows, const Geom& g, float* out, cudaStream_t st) {
   if (g.nv <= 0) return;
-  if (g.vec == 1) {
-    static int cache[64] = {0};
-    const size_t smem = Stage<N, 1>::kFloats * sizeof(float);
-    launch_after(k1_median<N, 1>, persistent_grid(k1_median<N, 1>, smem, g.nv, cache), kK1Threads, smem, st, rows, g, out);
-  } else {
-    static int cache[64] = {0};
-    const size_t smem = Stage<N, body_vec(N)>::kFloats * sizeof(float);
-    launch_after(k1_median<N, body_vec(N)>, persistent_grid(k1_median<N, body_vec(N)>, smem, g.nv, cache), kK1Threads, smem, st, rows, g, out);
-  }
+  static unsigned long long opted = 0;
+  if (g.vec == 1)
+    launch_after(k1_median<N, 1>, tile_grid(k1_median<N, 1>, 0, g.nv, opted), kK1Threads, 0, st, rows, g, out);
+  else
+    launch_after(k1_median<N, body_vec(N)>, tile_grid(k1_median<N, body_vec(N)>, 0, g.nv, opted), kK1Threads, 0, st, rows, g, out);
 }
 
 #define BZ_FN2(p) launch_median_part##p
@@ -74,14 +62,10 @@ bool BZ_FN(BZ_PART)(int n, const RowTable& rows, const Geom& g, float* out, cuda
 template <int N, int VEC>
 static void launch_sorted_nv(const RowTable& rows, const Geom& g, int mode, int f, float* out, cudaStream_t st) {
   if (g.nv <= 0) return;
-  // stage, plus the sorted columns for the closest modes (two occupancy classes: cached apart)
-  static int cache_plain[64] = {0}, cache_closest[64] = {0};
-  const size_t stage = Stage<N, VEC>::kFloats * sizeof(float);
-  const size_t both = stage + Stage<N, VEC>::kColumnFloats * sizeof(float);
-  if (mode == kModeTrmean)
-    launch_after(k1_sorted<N, VEC, -1, -1>, persistent_grid(k1_sorted<N, VEC, -1, -1>, stage, g.nv, cache_plain), kK1Threads, stage, st, rows, g, mode, f, out);
-  else
-    launch_after(k1_sorted<N, VEC, -1, -1>, persistent_grid(k1_sorted<N, VEC, -1, -1>, both, g.nv, cache_closest), kK1Threads, both, st, rows, g, mode, f, out);
+  // the closest modes stage the sorted columns in shared memory
+  static unsigned long long opted = 0;
+  const size_t smem = (mode == kModeTrmean) ? 0 : Stage<N, VEC>::kColumnFloats * sizeof(float);
+  launch_after(k1_sorted<N, VEC, -1, -1>, tile_grid(k1_sorted<N, VEC, -1, -1>, smem, g.nv, opted), kK1Threads, smem, st, rows, g, mode, f, out);
 }
 
 template <int N>
@@ -125,9 +109,8 @@ bool BZ_FN(BZ_PART)(int n, const RowTable& rows, const Geom& g, int mode, int f,
 template <int N, int F>
 static void launch_special_nf(const RowTable& rows, const Geom& g, float* out, cudaStream_t st) {
   if (g.nv <= 0) return;
-  static int cache[64] = {0};
-  const size_t smem = Stage<N, body_vec(N)>::kFloats * sizeof(float);
-  launch_after(k1_sorted<N, body_vec(N), F, BZ_SPECIAL_MODE>, persistent_grid(k1_sorted<N, body_vec(N), F, BZ_SPECIAL_MODE>, smem, g.nv, cache), kK1Threads, smem, st, rows, g, BZ_SPECIAL_MODE, F, out);
+  static unsigned long long opted = 0;
+  launch_after(k1_sorted<N, body_vec(N), F, BZ_SPECIAL_MODE>, tile_grid(k1_sorted<N, body_vec(N), F, BZ_SPECIAL_MODE>, 0, g.nv, opted), kK1Threads, 0, st, rows, g, BZ_SPECIAL_MODE, F, out);
 }
 
 bool BZ_SPECIAL_FN(int n, int f, const RowTable& rows, const Geom& g, float* out, cudaStream_t st) {

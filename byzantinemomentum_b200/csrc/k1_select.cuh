@@ -6,8 +6,8 @@
 // n rows (the `torch.stack` of median.py:39 / trmean.py:79 is gone), no shared memory on the
 // default path, no block-level barrier.  Tiles of 128·VEC coordinates map one to one onto
 // CTAs; ~4 CTAs are resident per SM, so while some warps sort others have their loads in
-// flight (two alternative walks — persistent, and persistent with cp.async prefetch — are kept
-// as build variants; they measured slower, see BZ_K1_VARIANT below).
+// flight.  (Persistent walks — grid-stride, with cp.async prefetch, and a per-SM TMA ring —
+// measured slower: DESIGN.md §4.1.)
 //
 //   k1_median<N, VEC>            median.py:31-39        FMNMX.NAN network, pruned to one rank
 //   k1_sorted<N, VEC, F, MODE>   trmean.py:24-50,69-109 sort, then trmean / phocas / meamed
@@ -35,43 +35,28 @@ namespace bz {
 #endif
 constexpr int kK1Threads = BZ_K1_THREADS;
 
-// How a thread walks the coordinates (A/B builds: `make VARIANT=v0 EXTRA=-DBZ_K1_VARIANT=0`):
-//   2 (default)  one logical vector per thread, direct register loads, grid = all tiles.  The
-//                hardware CTA scheduler balances the tail.
-//   1            persistent grid-stride loop, direct loads.
-//   0            persistent loop with cp.async staging of the next tile in a per-thread
-//                shared-memory column while the current one is sorted.
-#ifndef BZ_K1_VARIANT
-#define BZ_K1_VARIANT 2
-#endif
-
-// Shared-memory staging of one tile: column of thread t = N slots of VEC floats,
-// slot r at stage[(r * kK1Threads + t) * VEC] (a warp's slots of one row are contiguous).
+// Shared-memory sorted columns of the closest modes (run-time f): rank k of thread t's column c at
+// [k * VEC * kK1Threads + c * kK1Threads + t] (a warp's slots of one rank are contiguous).
 template <int N, int VEC>
 struct Stage {
-  static constexpr int kFloats = (BZ_K1_VARIANT == 0) ? N * kK1Threads * VEC : 0;   // experiment variants stage nothing
   static constexpr int kColumnFloats = N * kK1Threads * VEC;
-  static __device__ __forceinline__ void issue(const RowTable& rows, int64_t e0, float* col) {
-#pragma unroll
-    for (int r = 0; r < N; ++r) cp_async_vec<VEC>(col + r * kK1Threads * VEC, rows.p[r] + e0);
-    cp_async_commit();
-  }
-  static __device__ __forceinline__ void fetch(const float* col, float (&x)[VEC][N]) {
-    cp_async_wait<0>();
-#pragma unroll
-    for (int r = 0; r < N; ++r) {
-      float t[VEC];
-      lds_vec<VEC>(col + r * kK1Threads * VEC, t);
-#pragma unroll
-      for (int c = 0; c < VEC; ++c) x[c][r] = t[c];
-    }
-  }
 };
 
-// Walk this thread's tiles: `body(x, e0, full)` consumes the N x VEC values of one logical
-// vector (sorting them in place is fine) and stores its result.
+// CTAs per SM whose first vectors are prefetched into L2 before the PDL wait (k1_walk): the
+// resident CTAs of the wide kernels (128 registers, 4 per SM).
+constexpr unsigned kK1PrefetchWave = 4;
+constexpr unsigned kK1PrefetchMaxWaves = 16;   // ... in grids of at most this many such waves
+__device__ __forceinline__ unsigned nsm() {
+  unsigned r;
+  asm("mov.u32 %0, %%nsmid;" : "=r"(r));
+  return r;
+}
+
+// Walk this thread's logical vectors (the launcher sizes the grid to one per thread):
+// `body(x, e0, full)` consumes the N x VEC values of one logical vector (sorting them in place is
+// fine) and stores its result.
 template <int N, int VEC, class Body>
-__device__ __forceinline__ void k1_walk(const RowTable& rows, const Geom& g, float* stage, Body body) {
+__device__ __forceinline__ void k1_walk(const RowTable& rows, const Geom& g, Body body) {
   const int64_t stride = (int64_t)gridDim.x * kK1Threads;
   int64_t v = (int64_t)blockIdx.x * kK1Threads + threadIdx.x;
   // Programmatic dependent launch on both sides: the NEXT kernel of the stream may be scheduled while this
@@ -80,30 +65,23 @@ __device__ __forceinline__ void k1_walk(const RowTable& rows, const Geom& g, flo
   // calls lose the launch gap (~1.5 us of a 24 us pass at d = 1.3M).
   pdl_trigger();
   if (v >= g.nv) return;
-  pdl_wait();
-#if BZ_K1_VARIANT == 0
-  float* col = stage + threadIdx.x * VEC;
-  int64_t e0 = v * VEC - g.shift;
-  bool full = e0 >= 0 && e0 + VEC <= g.d;
-  if (full) Stage<N, VEC>::issue(rows, e0, col);
-  while (true) {
-    float x[VEC][N];
-    if (full) Stage<N, VEC>::fetch(col, x);
-    else      load_rows<N, VEC>(rows, e0, g.d, false, x);      // first / last partial vector only
-    // Prefetch the next tile into the (now free) column before the ALU phase
-    const int64_t vn = v + stride;
-    const bool more = vn < g.nv;
-    const int64_t en = vn * VEC - g.shift;
-    const bool fulln = more && en >= 0 && en + VEC <= g.d;
-    if (fulln) Stage<N, VEC>::issue(rows, en, col);
-    body(x, e0, full);
-    if (!more) break;
-    v = vn; e0 = en; full = fulln;
+  const unsigned wave = kK1PrefetchWave * nsm();
+  if (blockIdx.x < wave && gridDim.x <= kK1PrefetchMaxWaves * wave) {
+    // A CTA scheduled while its predecessor drains would otherwise leave HBM idle until the wait below
+    // returns (back to back, the predecessor's last wave is sorting with no loads in flight).  Pull this
+    // thread's first vector into L2 meanwhile.  A prefetch is only a hint, and L2 is the GPU's point of
+    // coherence: the loads after the wait still see every write the predecessor made to these rows.
+    // Only the first wave can be scheduled that early; for later CTAs the prefetch would only
+    // duplicate the loads' requests (measured: +1 % at d = 36.5M, +6 % at n = 51, d = 4.57M).  And only a
+    // short grid gains: over dozens of waves the predecessor's drain is a sliver of the pass, and the
+    // first-wave prefetch still measured ~1 % slower there.
+    const int64_t e0 = v * VEC - g.shift;
+    if (e0 >= 0 && e0 + VEC <= g.d) {
+#pragma unroll
+      for (int r = 0; r < N; ++r) prefetch_l2(rows.p[r] + e0);
+    }
   }
-#else
-  // Experiment variants (A/B builds, `make VARIANT=...`): direct register loads, no prefetch;
-  // 1 = persistent grid-stride loop, 2 = one tile per thread (the launcher sizes the grid).
-  (void)stage;
+  pdl_wait();
   for (; v < g.nv; v += stride) {
     const int64_t e0 = v * VEC - g.shift;
     const bool full = e0 >= 0 && e0 + VEC <= g.d;
@@ -111,7 +89,6 @@ __device__ __forceinline__ void k1_walk(const RowTable& rows, const Geom& g, flo
     load_rows<N, VEC>(rows, e0, g.d, full, x);
     body(x, e0, full);
   }
-#endif
 }
 
 // ---- median ---------------------------------------------------------------------------
@@ -125,8 +102,7 @@ __host__ __device__ constexpr int k1_min_blocks(int n, int vec) { return (n * ve
 template <int N, int VEC>
 __global__ void __launch_bounds__(kK1Threads, k1_min_blocks(N, VEC))
 k1_median(const __grid_constant__ RowTable rows, const Geom g, float* __restrict__ out) {
-  extern __shared__ __align__(16) float smem[];
-  k1_walk<N, VEC>(rows, g, smem, [&](float (&x)[VEC][N], int64_t e0, bool full) {
+  k1_walk<N, VEC>(rows, g, [&](float (&x)[VEC][N], int64_t e0, bool full) {
     float chk = 0.f;
 #pragma unroll
     for (int r = 0; r < N; ++r)
@@ -224,11 +200,11 @@ template <int N, int VEC, int F, int MODE>
 __global__ void __launch_bounds__(kK1Threads, k1_min_blocks(N, VEC))
 k1_sorted(const __grid_constant__ RowTable rows, const Geom g, const int mode_rt, const int f_rt,
           float* __restrict__ out) {
-  extern __shared__ __align__(16) float smem[];   // [stage][+ sorted columns for the closest modes]
+  extern __shared__ __align__(16) float smem[];   // sorted columns for the closest modes
   const int mode = (MODE >= 0) ? MODE : mode_rt;
   const int f = (F >= 0) ? F : f_rt;
-  float* sorted_cols = smem + Stage<N, VEC>::kFloats;
-  k1_walk<N, VEC>(rows, g, smem, [&](float (&x)[VEC][N], int64_t e0, bool full) {
+  float* sorted_cols = smem;
+  k1_walk<N, VEC>(rows, g, [&](float (&x)[VEC][N], int64_t e0, bool full) {
     float chk = 0.f;
 #pragma unroll
     for (int r = 0; r < N; ++r)
