@@ -575,17 +575,28 @@ k2_ring(const __grid_constant__ RowTable rows, const __grid_constant__ SelfList 
           // bits whether it comes out of a full pass, a star pass or the cache), assembled where the
           // scoring code expects it; diagonal entries (alias flags) always come from this pass.
           const int N = tail.n;
-          double* table = sm + (n == N ? 0 : (size_t)N * N);
-          if (tail.nranks > 0) {
+          const bool exchange = tail.nranks > 0;
+          double* table = sm + (n == N || exchange ? 0 : (size_t)N * N);
+          RowMap map = tail.map;
+          if (exchange) {
             // ---- exchange over peer memory, inside this launch ----
+            // The block is published in the N x N layout of the original rows: entry (i, j), i < j, is the
+            // pair of their distinct rows (the alias flag when both are one tensor), every other entry 0.
+            // That layout is the same on every rank whatever its rows alias — a rank with an empty shard
+            // cannot tell, an empty tensor has no address — and holds nothing the workspace left behind.
+            const int NN = N * N;
             double* mine = tail.peer_block[tail.rank];
-            for (int e = threadIdx.x; e < len; e += kThreads) {
-              const int i = e / n, j = e - i * n;
+            for (int e = threadIdx.x; e < NN; e += kThreads) {
+              const int i = e / N, j = e - i * N;
               double v = 0.;
-              if (i <= j)
-                for (int g = 0; g < ngroups; ++g) v += __ldcg(gblocks + (size_t)g * len + e);
+              if (i < j) {
+                const int a = map.to_unique[i], b = map.to_unique[j];
+                const size_t k = (size_t)min(a, b) * n + max(a, b);
+                for (int g = 0; g < ngroups; ++g) v += __ldcg(gblocks + (size_t)g * len + k);
+              }
               mine[e] = v;
             }
+            map.u = N;                          // the summed table below is N x N already
             __threadfence_system();
             __syncthreads();
             if ((int)threadIdx.x < tail.nranks) {
@@ -600,7 +611,7 @@ k2_ring(const __grid_constant__ RowTable rows, const __grid_constant__ SelfList 
             }
             __syncthreads();
             asm volatile("" ::: "memory");      // the block loads below stay below the flag wait
-            for (int e = threadIdx.x; e < len; e += kThreads) {
+            for (int e = threadIdx.x; e < NN; e += kThreads) {
               double part[BZ_MAX_PEERS];
 #pragma unroll
               for (int r = 0; r < BZ_MAX_PEERS; ++r) part[r] = (r < tail.nranks) ? ld_relaxed_sys_f64(tail.peer_block[r] + e) : 0.;
@@ -626,8 +637,8 @@ k2_ring(const __grid_constant__ RowTable rows, const __grid_constant__ SelfList 
             if (tail.cache_out != nullptr) tail.cache_out[e] = v;
           }
           __syncthreads();
-          if (tail.kind == 3) brute_from_table(tail.map, N, tail.f, tail.total, tail.order, tail.status, sm);
-          else                score_from_table(tail.map, N, tail.count, tail.order, tail.kind == 2 ? tail.status : nullptr,
+          if (tail.kind == 3) brute_from_table(map, N, tail.f, tail.total, tail.order, tail.status, sm);
+          else                score_from_table(map, N, tail.count, tail.order, tail.kind == 2 ? tail.status : nullptr,
                                                tail.f, tail.m, tail.kind == 2 ? 1 : 0, sm);
           __syncthreads();
           if (threadIdx.x == 0 && peer_timeout && tail.status != nullptr) *tail.status = BZ_STATUS_PEER_TIMEOUT;
@@ -729,7 +740,7 @@ int launch_pairdist_ring(const RowTable& rows, int n, int64_t d, double* parts, 
   if (!ring_shape(n, W, C)) return -1;
   if (force_cluster > C && force_cluster <= kRMaxCluster) C = force_cluster;   // experiments: more CTAs per tile than needed
   if (nself > W * C * kSelfPerWarp) return -1;
-  for (int r = 0; r < n; ++r)
+  for (int r = 0; r < n && d > 0; ++r)           // an empty shard reads nothing: any address will do
     if ((((uintptr_t)rows.p[r]) & 15) != 0) return -1;
   SelfList self;
   self.count = nself;

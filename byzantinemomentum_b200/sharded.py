@@ -27,9 +27,10 @@ import math
 import torch
 import torch.distributed as dist
 
+from . import _lib
 from . import engine as _engine
 
-__all__ = ["aggregate", "aggregate_p2p", "compute_avg_dev_max", "replicate", "apply_update", "shard_bounds", "PeerExchange", "FusedExchange", "ShardedPlan", "COORDINATE_WISE", "DISTANCE_BASED"]
+__all__ = ["aggregate", "aggregate_p2p", "compute_avg_dev_max", "replicate", "apply_update", "shard_bounds", "rows_aligned", "choose_exchange", "PeerExchange", "FusedExchange", "ShardedPlan", "COORDINATE_WISE", "DISTANCE_BASED"]
 
 COORDINATE_WISE = ("average", "median", "trmean", "phocas", "meamed")
 DISTANCE_BASED = ("krum", "bulyan", "brute", "aksel", "cge")
@@ -124,6 +125,48 @@ def fused_exchange(n, device, group=None):
     ex = _fused[key] = FusedExchange(n, device, group)
   return ex
 
+def rows_aligned(rows):
+  """ Whether the ring kernel takes these rows: every non-empty row 16-byte aligned (an empty shard
+  reads nothing). """
+  return all(g.numel() == 0 or g.data_ptr() % 16 == 0 for g in rows)
+
+def _symmetric_memory_importable():
+  try:
+    import torch.distributed._symmetric_memory  # noqa: F401
+  except Exception:
+    return False
+  return True
+
+EXCHANGES = ("auto", "fused", "p2p", "nccl")
+
+def choose_exchange(gar, exchange, aligned, symmetric, group=None):
+  """ The exchange of `ShardedPlan`, the same on every rank of `group`.  The two ranks' protocols do
+  not mix (different symmetric buffers, flags nobody raises), so the local facts — `aligned`: this
+  rank's rows are 16-byte aligned; `symmetric`: symmetric memory can be set up here — are agreed on
+  with one all-reduce (MIN) before the choice: a shard that starts mid-vector on one rank moves every
+  rank to "p2p".  An explicit request that some rank cannot serve raises on every rank.
+  Returns "fused", "p2p" or "nccl". """
+  if exchange not in EXCHANGES:
+    raise ValueError(f"unknown exchange {exchange!r}")
+  world = dist.get_world_size(group) if dist.is_initialized() else 1
+  facts = [int(bool(aligned)), int(bool(symmetric))]
+  if world > 1:
+    device = torch.device("cuda", torch.cuda.current_device()) if dist.get_backend(group) == "nccl" else torch.device("cpu")
+    agreed = torch.tensor(facts, dtype=torch.int32, device=device)
+    dist.all_reduce(agreed, op=dist.ReduceOp.MIN, group=group)
+    facts = agreed.tolist()
+  aligned, symmetric = bool(facts[0]), bool(facts[1])
+  fusable = gar in ("krum", "bulyan") and aligned
+  if exchange == "auto":
+    if world == 1 or world > _lib.MAX_PEERS or not symmetric:
+      return "nccl"
+    return "fused" if fusable else "p2p"
+  if exchange == "fused" and not (fusable and symmetric and world <= _lib.MAX_PEERS):
+    raise ValueError(f"the fused exchange serves krum / bulyan on 16-byte aligned rows, with symmetric memory, on every one of at most {_lib.MAX_PEERS} ranks")
+  if exchange == "p2p" and not symmetric:
+    raise ValueError("the p2p exchange needs symmetric memory on every rank")
+  return exchange
+
 def aggregate_p2p(gar, gradients, f=None, m=None, mode="mid", group=None, return_selection=False):
   """ `aggregate` for the distance-based rules with the exchange fused into the selection kernel
   (peer memory over NVLink, see PeerExchange).  CUDA engine only. """
@@ -182,8 +225,9 @@ class ShardedPlan:
             "fused" (krum, bulyan) the exchange runs INSIDE the distance pass: its last CTA publishes the
                     block in the symmetric buffer, flags the peers, waits for theirs and scores — a step
                     is the single-GPU rule's two launches, nothing else (`bz_krum_peers`);
-            "auto"  "fused" where it applies, else "p2p", when symmetric memory can be set up for the
-                    group; else "nccl".
+            "auto"  "fused" where it applies on every rank, else "p2p", when every rank of the group
+                    has symmetric memory; else "nccl".  The ranks agree on the choice
+                    (`choose_exchange`); a failing symmetric-memory setup raises.
   Both exchanges use the same fixed summation order: bitwise identical selections on every rank.
   Coordinate-wise rules need no exchange and simply wrap `engine.Plan`. """
   def __init__(self, gar, gradients, f=None, m=None, mode="mid", group=None, exchange="auto"):
@@ -220,28 +264,12 @@ class ShardedPlan:
     o = self.out.data_ptr()
     pair = gar in ("krum", "bulyan", "brute")
     width = n * n if pair else n
-    # ---- exchange -------------------------------------------------------------------------------
-    fusable = gar in ("krum", "bulyan") and all(g.data_ptr() % 16 == 0 for g in self.rows)
-    if exchange == "auto":
-      exchange = "nccl"
-      if self.world > 1 and self.world <= _lib.MAX_PEERS:
-        try:
-          if fusable:
-            self._fx = fused_exchange(n, device, group)
-            exchange = "fused"
-          else:
-            self._ex = peer_exchange(n, device, group)
-            exchange = "p2p"
-        except Exception:
-          exchange = "nccl"
-    elif exchange == "fused":
-      if not fusable or self.world < 1:
-        raise ValueError("the fused exchange serves krum / bulyan on 16-byte aligned rows")
+    # ---- exchange: one choice for the whole group ------------------------------------------------
+    exchange = choose_exchange(gar, exchange, rows_aligned(self.rows), _symmetric_memory_importable(), group)
+    if exchange == "fused":
       self._fx = fused_exchange(n, device, group)
     elif exchange == "p2p":
       self._ex = peer_exchange(n, device, group)
-    elif exchange != "nccl":
-      raise ValueError(f"unknown exchange {exchange!r}")
     self.exchange = exchange
     if exchange == "fused":
       fx = self._fx

@@ -165,7 +165,12 @@ BZ_API int bz_brute_reuse(const float* const* rows, int n, int f, int64_t d, flo
  *                  slot on every rank; zero before the first step
  *   epoch          step number: strictly increasing, the same on every rank for the same step
  *   status         DEVICE int32, required: BZ_STATUS_PEER_TIMEOUT when a peer did not show up
- * Rows must be 16-byte aligned (the ring kernel); otherwise BZ_EUNSUPPORTED: use the phases below. */
+ * Rows must be 16-byte aligned (the ring kernel); otherwise BZ_EUNSUPPORTED: use the phases below.
+ * The published block is n x n: entry (i, j), i < j, is this shard's sum of squared differences of
+ * rows i and j (the same layout on every rank, whichever rows alias), every other entry 0.
+ * d == 0 (an empty shard, e.g. the last ranks when d < nranks) is a full participant: the rank
+ * publishes a zero block, signals, waits, and writes `order` and `status` like every other rank; only
+ * the reduce pass is skipped.  Its rows are not read: neither their addresses nor their aliasing matter. */
 BZ_API int bz_krum_peers(const float* const* rows, int n, int f, int m, int64_t d, float* out, int32_t* order,
                          int32_t* status, int rank, int nranks, double* const* peer_blocks,
                          unsigned* const* peer_flags, unsigned epoch, void* ws, size_t ws_bytes, void* stream);

@@ -68,6 +68,36 @@ def test_c_abi_rejects_bad_arguments_without_a_gpu():
   assert lib.bz_avg_dev_max(_rows(7), 7, 16, out, None, ctypes.c_void_p(0xB000), need, None) == -1 and "stats" in message()
   assert lib.bz_aksel(_rows(7), 7, 2, 9, 16, out, order, ctypes.c_void_p(0xB000), need, None) == -1 and "mode" in message()
 
+@pytest.mark.parametrize("name", ["bz_krum_peers", "bz_bulyan_peers"])
+def test_fused_peer_calls_reject_bad_exchange_arguments_without_a_gpu(name):
+  """ `bz_*_peers` check rank, nranks, status and the peer tables before any CUDA call (fake,
+  never dereferenced addresses). """
+  lib = _lib.lib()
+  fn = getattr(lib, name)
+  n, f, m, d = 11, 2, 3, 64
+  need = lib.bz_workspace_bytes(n)
+  table = lambda addrs: (ctypes.c_void_p * len(addrs))(*addrs)
+  ok = dict(rank=1, nranks=3, status=0x9100, blocks=[0x10000 + 0x1000 * r for r in range(3)],
+            flags=[0x20000 + 0x40 * r for r in range(3)])
+  def call(**kw):
+    a = dict(ok, **kw)
+    status = None if a["status"] is None else ctypes.c_void_p(a["status"])
+    blocks = None if a["blocks"] is None else table(a["blocks"])
+    flags = None if a["flags"] is None else table(a["flags"])
+    return fn(_rows(n), n, f, m, d, ctypes.c_void_p(0x9000), ctypes.c_void_p(0x9200), status, a["rank"], a["nranks"],
+              blocks, flags, 7, ctypes.c_void_p(0xB000), need, None)
+  message = lambda: lib.bz_last_error().decode()
+  assert call(rank=3) == -1 and "rank 3 of 3" in message()
+  assert call(rank=-1) == -1
+  assert call(nranks=0, rank=0) == -1
+  assert call(nranks=17, rank=0, blocks=ok["blocks"] * 6, flags=ok["flags"] * 6) == -1 and "of 17" in message()
+  assert call(status=None) == -1 and "status" in message()
+  assert call(blocks=None) == -1 and call(flags=None) == -1
+  for bad in (0, 0x10004):                                        # NULL, not 8-byte aligned
+    assert call(blocks=[ok["blocks"][0], bad, ok["blocks"][2]]) == -1 and "peer 1" in message()
+  for bad in (0, 0x20002):                                        # NULL, not 4-byte aligned
+    assert call(flags=[ok["flags"][0], ok["flags"][1], bad]) == -1 and "peer 2" in message()
+
 def test_check_maps_codes_to_exceptions():
   lib = _lib.lib()
   code = lib.bz_median(None, 3, 16, None, None)

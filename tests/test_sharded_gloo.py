@@ -71,6 +71,59 @@ def _worker(rank, world, port, queue):
   finally:
     dist.destroy_process_group()
 
+def _exchange_worker(rank, world, port, queue):
+  """ Rank 0 holds aligned rows, rank 1 views that start one float in (as `shard_bounds` gives an odd
+  shard start); symmetric memory counts as available on both. """
+  import sys, pathlib
+  root = pathlib.Path(__file__).resolve().parent.parent
+  sys.path.insert(0, str(root))
+  import torch.distributed as dist
+  from byzantinemomentum_b200 import sharded
+  os.environ["MASTER_ADDR"] = "127.0.0.1"
+  os.environ["MASTER_PORT"] = str(port)
+  dist.init_process_group("gloo", rank=rank, world_size=world)
+  try:
+    base = [torch.zeros(65) for _ in range(7)]
+    rows = [b[:64] for b in base] if rank == 0 else [b[1:] for b in base]
+    aligned = sharded.rows_aligned(rows)
+    got = {"aligned": aligned}
+    for gar in ("krum", "bulyan", "cge"):
+      for request in ("auto", "fused", "p2p", "nccl"):
+        try:
+          got[(gar, request)] = sharded.choose_exchange(gar, request, aligned, True)
+        except ValueError:
+          got[(gar, request)] = "refused"
+    got["no symmetric memory"] = sharded.choose_exchange("krum", "auto", True, rank == 0)
+    got["both aligned"] = sharded.choose_exchange("krum", "auto", True, True)
+    queue.put((rank, got))
+  finally:
+    dist.destroy_process_group()
+
+def test_ranks_agree_on_the_exchange():
+  """ Each rank's own rows would pick "fused" on rank 0 and "p2p" on rank 1: two protocols that never
+  meet.  The choice is agreed across the group, and an infeasible explicit request fails everywhere. """
+  import torch.multiprocessing as mp
+  with socket.socket() as s:
+    s.bind(("127.0.0.1", 0))
+    port = s.getsockname()[1]
+  ctx = mp.get_context("spawn")
+  queue = ctx.Queue()
+  procs = [ctx.Process(target=_exchange_worker, args=(r, 2, port, queue)) for r in range(2)]
+  for p in procs:
+    p.start()
+  got = dict(queue.get(timeout=180) for _ in procs)
+  for p in procs:
+    p.join(timeout=60)
+    assert p.exitcode == 0
+  assert got[0]["aligned"] and not got[1]["aligned"]
+  assert got[0] == dict(got[1], aligned=True), "the ranks chose different exchanges"
+  for gar in ("krum", "bulyan", "cge"):
+    assert got[0][(gar, "auto")] == "p2p"
+    assert got[0][(gar, "fused")] == "refused"
+    assert got[0][(gar, "p2p")] == "p2p" and got[0][(gar, "nccl")] == "nccl"
+  assert got[0]["no symmetric memory"] == "nccl"
+  assert got[0]["both aligned"] == "fused"
+
 def test_two_rank_sharding_matches_single_process():
   import torch.multiprocessing as mp
   from oracle import byzoracle as orc
