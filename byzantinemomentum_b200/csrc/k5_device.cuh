@@ -27,44 +27,23 @@ struct PeerParts {
   __device__ __forceinline__ const double* block(int p) const { return ptr[p]; }
 };
 
-// Block-wide, deterministic sum of `nparts` partial blocks of `len` doubles into smem `out`.
-// The parts are split in `slices` interleaved classes (p mod slices); thread (slice, t) walks
-// entries t, t + T, ... and adds its class in ascending p; the classes are then added in
-// ascending order.  The order depends only on (nparts, slices): bitwise reproducible, and the
-// same on every rank of the sharded path.  All loads of a thread are independent across
-// entries, so a thread keeps several in flight (a naive per-entry loop over one part per SM
-// is pure latency).
+// Block-wide sum of `nparts` partial blocks of `len` doubles into smem `out`, in rank order:
+// out[e] = ((p0[e] + p1[e]) + p2[e]) + ..., the table the fused exchange of k2_ring.cu sums, so the
+// gathered, the peer-memory and the fused paths of the sharded rules select the same rows.  One
+// thread per entry; the loads do not wait on the adds, so a batch of B parts is in flight at once.
 template <class Parts>
-__device__ void block_sum_parts(const Parts& parts, int nparts, int len, int slices,
-                                double* __restrict__ scratch, double* __restrict__ out) {
-  const int T = blockDim.x / slices;            // threads per slice
-  const int slice = threadIdx.x / T, t = threadIdx.x - slice * T;
-  constexpr int E = 8;                          // entries per thread in flight together
-  if (slice < slices) {
-    for (int e0 = t; e0 < len; e0 += T * E) {
-      double s[E];
-#pragma unroll
-      for (int q = 0; q < E; ++q) s[q] = 0.;
-#pragma unroll 4
-      for (int p = slice; p < nparts; p += slices) {
-        const double* __restrict__ row = parts.block(p);
-#pragma unroll
-        for (int q = 0; q < E; ++q) {
-          const int e = e0 + q * T;
-          if (e < len) s[q] += __ldcg(row + e);
-        }
-      }
-#pragma unroll
-      for (int q = 0; q < E; ++q) {
-        const int e = e0 + q * T;
-        if (e < len) scratch[slice * len + e] = s[q];
-      }
-    }
-  }
-  __syncthreads();
+__device__ void block_sum_parts(const Parts& parts, int nparts, int len, double* __restrict__ out) {
+  constexpr int B = 8;
   for (int e = threadIdx.x; e < len; e += blockDim.x) {
-    double s = 0.;
-    for (int k = 0; k < slices; ++k) s += scratch[k * len + e];
+    double s = __ldcg(parts.block(0) + e);
+    for (int p0 = 1; p0 < nparts; p0 += B) {
+      double v[B];
+#pragma unroll
+      for (int q = 0; q < B; ++q) v[q] = (p0 + q < nparts) ? __ldcg(parts.block(p0 + q) + e) : 0.;
+#pragma unroll
+      for (int q = 0; q < B; ++q)
+        if (p0 + q < nparts) s += v[q];
+    }
     out[e] = s;
   }
   __syncthreads();
@@ -173,7 +152,6 @@ __device__ inline void stable_order(const double* key, int n, int32_t* __restric
 // krum.py:52-62 (count = n-f-1, diagonal excluded) and bulyan.py:56-62 (count = m over the
 // row INCLUDING its +inf diagonal).  Putting +inf on the diagonal serves both: the extra +inf
 // can only be reached after every finite distance, where the sum is +inf either way.
-// Block-wide, any blockDim.x that `slices` divides; `sm`: (2 n^2 + n + slices n^2) doubles of shared memory.
 // Scoring from an already summed table of squared distances, left by the caller in shared memory:
 // at `sm` (n x n) when map.u == n, else the u x u table at `sm + n*n`.  `sm`: (2 n^2 + n) doubles.
 __device__ inline void score_from_table(const RowMap& map, int n, int count, int32_t* __restrict__ order, int32_t* __restrict__ status,
@@ -207,11 +185,10 @@ __device__ inline void score_from_table(const RowMap& map, int n, int count, int
 
 template <class Parts>
 __device__ void score_select_body(const Parts& parts, const RowMap& map, int nparts, int n, int count,
-                                  int32_t* __restrict__ order, int32_t* __restrict__ status, int f, int m, int bulyan, int slices,
+                                  int32_t* __restrict__ order, int32_t* __restrict__ status, int f, int m, int bulyan,
                                   double* sm) {
-  double* scratch = sm + 2 * n * n + n;
-  if (map.u == n) block_sum_parts(parts, nparts, n * n, slices, scratch, sm);
-  else            block_sum_parts(parts, nparts, map.u * map.u, slices, scratch, sm + n * n);   // u x u table, parked in `sorted`
+  if (map.u == n) block_sum_parts(parts, nparts, n * n, sm);
+  else            block_sum_parts(parts, nparts, map.u * map.u, sm + n * n);   // u x u table, parked in `sorted`
   score_from_table(map, n, count, order, status, f, m, bulyan, sm);
 }
 
@@ -328,26 +305,14 @@ __device__ inline void brute_from_table(const RowMap& map, int n, int f, unsigne
 }
 
 
-// Block-wide, any blockDim.x <= 1024 that `slices` divides; `sm`: n^2 + (n+1)^2 + 64 + slices n^2 doubles.
+// Block-wide, any blockDim.x <= 1024; `sm`: n^2 + (n+1)^2 + 64 doubles.
 template <class Parts>
 __device__ void brute_select_body(const Parts& parts, const RowMap& map, int nparts, int n, int f,
-                                  unsigned long long total, int32_t* __restrict__ sel, int32_t* __restrict__ status, int slices,
+                                  unsigned long long total, int32_t* __restrict__ sel, int32_t* __restrict__ status,
                                   double* sm) {
-  double* scratch = sm + n * n + (n + 1) * (n + 1) + 64;
-  if (map.u == n) block_sum_parts(parts, nparts, n * n, slices, scratch, sm);
-  else            block_sum_parts(parts, nparts, map.u * map.u, slices, scratch, sm + n * n);
+  if (map.u == n) block_sum_parts(parts, nparts, n * n, sm);
+  else            block_sum_parts(parts, nparts, map.u * map.u, sm + n * n);
   brute_from_table(map, n, f, total, sel, status, sm);
-}
-
-// Interleaved part classes for block_sum_parts: as many as fit `budget` bytes of scratch, at most 8,
-// dividing `threads`.
-inline int pick_slices(int n, int nparts, int threads, size_t budget = 48 * 1024) {
-  int slices = (int)(budget / ((size_t)n * n * sizeof(double)));
-  if (slices > 8) slices = 8;
-  if (slices > nparts) slices = nparts;
-  if (slices < 1) slices = 1;
-  while (threads % slices) --slices;
-  return slices;
 }
 
 inline RowMap identity_map(int n) {

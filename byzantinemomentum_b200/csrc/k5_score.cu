@@ -14,19 +14,18 @@ constexpr int kK5Threads = 1024;
 template <class Parts>
 __global__ void __launch_bounds__(kK5Threads)
 k5_score_select(const __grid_constant__ Parts parts, const __grid_constant__ RowMap map, int nparts, int n, int count,
-                int32_t* __restrict__ order, int32_t* __restrict__ status, int f, int m, int bulyan, int slices) {
+                int32_t* __restrict__ order, int32_t* __restrict__ status, int f, int m, int bulyan) {
   extern __shared__ double sm[];
-  score_select_body(parts, map, nparts, n, count, order, status, f, m, bulyan, slices, sm);
+  score_select_body(parts, map, nparts, n, count, order, status, f, m, bulyan, sm);
 }
 
 // aksel.py:39-49 / cge.py:28-38: stable order of n keys.
-constexpr int kRowSelThreads = 1024, kRowSelSlices = 16;   // 64 threads per slice: one per row
+constexpr int kRowSelThreads = kMaxN;   // one per row
 template <class Parts>
 __global__ void __launch_bounds__(kRowSelThreads)
 k5_rowdist_select(const __grid_constant__ Parts parts, int nparts, int n, int sqrt_norm, int32_t* __restrict__ order) {
   __shared__ double key[kMaxN];
-  __shared__ double scratch[kRowSelSlices * kMaxN];
-  block_sum_parts(parts, nparts, n, kRowSelSlices, scratch, key);
+  block_sum_parts(parts, nparts, n, key);
   for (int i = threadIdx.x; i < n; i += blockDim.x) {
     const double s = key[i];
     double v;
@@ -45,9 +44,9 @@ k5_rowdist_select(const __grid_constant__ Parts parts, int nparts, int n, int sq
 template <class Parts>
 __global__ void __launch_bounds__(kK5Threads)
 k5_brute_select(const __grid_constant__ Parts parts, const __grid_constant__ RowMap map, int nparts, int n, int f,
-                unsigned long long total, int32_t* __restrict__ sel, int32_t* __restrict__ status, int slices) {
+                unsigned long long total, int32_t* __restrict__ sel, int32_t* __restrict__ status) {
   extern __shared__ double sm[];
-  brute_select_body(parts, map, nparts, n, f, total, sel, status, slices, sm);
+  brute_select_body(parts, map, nparts, n, f, total, sel, status, sm);
 }
 
 // ---- host side ---------------------------------------------------------------------------
@@ -63,29 +62,26 @@ static void opt_in_once(K kernel, size_t bytes, unsigned long long& mask) {
   }
 }
 
-constexpr size_t kScoreSmemMax = (size_t)(2 * kMaxN * kMaxN + kMaxN) * sizeof(double) + 48 * 1024;
-constexpr size_t kBruteSmemMax = (size_t)kMaxN * kMaxN * sizeof(double) + (size_t)(kMaxN + 1) * (kMaxN + 1) * sizeof(unsigned long long) + 48 * 1024 + 512;
+constexpr size_t kScoreSmemMax = (size_t)(2 * kMaxN * kMaxN + kMaxN) * sizeof(double);
+constexpr size_t kBruteSmemMax = (size_t)kMaxN * kMaxN * sizeof(double) + (size_t)(kMaxN + 1) * (kMaxN + 1) * sizeof(unsigned long long) + 512;
 
 template <class Parts>
 static void score_select(const Parts& parts, const RowMap& map, int nparts, int n, int count, int32_t* order, int32_t* status, int f, int m,
                          int bulyan, cudaStream_t st) {
-  const int slices = pick_slices(n, nparts, kK5Threads);
-  const size_t smem = (size_t)(2 * n * n + n + slices * n * n) * sizeof(double);
+  const size_t smem = (size_t)(2 * n * n + n) * sizeof(double);
   static unsigned long long opted = 0;
   opt_in_once(k5_score_select<Parts>, kScoreSmemMax, opted);
-  k5_score_select<Parts><<<1, kK5Threads, smem, st>>>(parts, map, nparts, n, count, order, status, f, m, bulyan, slices);
+  k5_score_select<Parts><<<1, kK5Threads, smem, st>>>(parts, map, nparts, n, count, order, status, f, m, bulyan);
 }
 
 template <class Parts>
 static int brute_select(const Parts& parts, const RowMap& map, int nparts, int n, int f, int32_t* sel, int32_t* status, cudaStream_t st) {
   const unsigned long long total = brute_total(n, f);
   if (total > (1ull << 31)) return -1;
-  const int slices = pick_slices(n, nparts, kK5Threads);
-  const size_t smem = (size_t)n * n * sizeof(double) + (size_t)(n + 1) * (n + 1) * sizeof(unsigned long long) +
-                      (size_t)(slices * n * n + 64) * sizeof(double);
+  const size_t smem = (size_t)n * n * sizeof(double) + (size_t)(n + 1) * (n + 1) * sizeof(unsigned long long) + 64 * sizeof(double);
   static unsigned long long opted = 0;
   opt_in_once(k5_brute_select<Parts>, kBruteSmemMax, opted);
-  k5_brute_select<Parts><<<1, kK5Threads, smem, st>>>(parts, map, nparts, n, f, total, sel, status, slices);
+  k5_brute_select<Parts><<<1, kK5Threads, smem, st>>>(parts, map, nparts, n, f, total, sel, status);
   return 0;
 }
 

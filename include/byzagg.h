@@ -192,7 +192,9 @@ BZ_API int bz_pairdist_partial(const float* const* rows, int n, int64_t d, doubl
  *    origin: squared norms).  part: device double[n]. */
 BZ_API int bz_rowdist_partial(const float* const* rows, int n, const float* center, int64_t d,
                        double* part, void* ws, size_t ws_bytes, void* stream);
-/* B: selections from `nparts` gathered blocks (parts: device double[nparts][n*n] or [nparts][n]). */
+/* B: selections from `nparts` gathered blocks (parts: device double[nparts][n*n] or [nparts][n]).
+ *    The blocks are added in rank order, ((p0 + p1) + p2) + ..., for any nparts: the same table, bit
+ *    for bit, as the exchange fused into bz_krum_peers / bz_bulyan_peers, hence the same selection. */
 BZ_API int bz_krum_select(const double* parts, int nparts, int n, int f, int32_t* order, void* stream);
 BZ_API int bz_bulyan_select(const double* parts, int nparts, int n, int f, int m, int32_t* order,
                      int32_t* status, void* stream);
@@ -202,7 +204,7 @@ BZ_API int bz_brute_select(const double* parts, int nparts, int n, int f, int32_
  * sqrt_norm == 0: keys are fl32(sum) (aksel.py:41).  Stable ascending order of the n keys. */
 BZ_API int bz_rowdist_select(const double* parts, int nparts, int n, int sqrt_norm, int32_t* order,
                       void* stream);
-/* B over PEER MEMORY: same selections, but block p is read in place from peers[p], a device
+/* B over PEER MEMORY: same selections (same rank-order sum), but block p is read in place from peers[p], a device
  *    pointer into rank p's memory mapped over NVLink (e.g. torch symmetric memory): the exchange
  *    step is fused into the selection kernel, no all-gather.  peers: HOST array of npeers device
  *    pointers (double[n*n] or double[n] each), npeers <= BZ_MAX_PEERS; the caller orders the

@@ -47,10 +47,7 @@ class OracleBackend:
   # phase B: blocks are summed in rank order
   @staticmethod
   def _sum_parts(parts):
-    acc = np.zeros(parts.shape[1:], dtype=np.float64)
-    for r in range(parts.shape[0]):
-      acc = acc + parts[r].numpy()
-    return acc
+    return orc.sum_parts(parts.numpy())
   def _distances(self, parts, n, map_nonfinite):
     sq = self._sum_parts(parts)
     D = np.triu(orc.fp32_norm(sq), 1)
