@@ -33,16 +33,14 @@ struct Workspace {
 bool carve_workspace(void* ws, size_t bytes, int n, Workspace& out);
 
 // ---- K2: partial squared pairwise distances -------------------------------------------------
-// parts[x*n*n + i*n + j] (i < j) = this CTA's share of sum_k (rows[i][k] - rows[j][k])^2.
-// Returns the number of partial blocks written (grid size along x), <= kMaxParts.
-// self_pairs: also write the diagonal entries i == j (sum of (x_i - x_i)^2: 0 or NaN), needed by
-// the alias map of K5.
-int launch_pairdist(const RowTable& rows, int n, int64_t d, double* parts, cudaStream_t st, int self_pairs = 0);
-
-// K2, second generation (k2_ring.cu): balanced tasks, distributed TMA issue, clusters + multicast for
-// n > 25.  Returns the number of blocks written or -1 when it cannot run (unaligned rows, ...).
+// parts[x*n*n + i*n + j] (i < j) = the share of block x of sum_k (rows[i][k] - rows[j][k])^2, and
+// the diagonal entries i == j (sum of (x_i - x_i)^2: 0 or NaN) of the rows the alias map of K5 reads.
+// The ring kernel (k2_ring.cu): balanced tasks, distributed TMA issue, clusters + multicast for
+// n > 25.  Returns the number of blocks written, <= kMaxParts, or -1 when it cannot run (rows not
+// 16-byte aligned, or a launch / occupancy failure).
 // Optional scoring / selection step to run inside the distance pass (its last CTA): what the
-// caller would otherwise launch as K5.  `fused` is set when the pass did run it.
+// caller would otherwise launch as K5.  `fused` is set when the pass did run it; it does not when
+// the step's tables do not fit the ring's shared memory.
 struct SelectTail {
   int kind;                 // 1 = Multi-Krum order, 2 = Bulyan order + status, 3 = brute subset,
                             // 4 = the reduced block only (phase A of the sharded path): `order` is a double[n*n]
@@ -71,6 +69,7 @@ int launch_pairdist_ring(const RowTable& rows, int n, int64_t d, double* parts, 
                          const unsigned char* self_rows, int nself, SelectTail* select = nullptr);
 // Dispatcher used by the rules: `rows` are the u unique rows, `to_unique` (or NULL) maps the n_orig
 // original rows to them; the self distance is produced for the unique rows that are aliased.
+// Runs the ring, or the cp.async kernel of k2_pairdist.cu when the ring returns -1.
 int launch_pairdist_auto(const RowTable& rows, int u, int64_t d, double* parts, cudaStream_t st,
                          const int* to_unique, int n_orig, SelectTail* select = nullptr);
 

@@ -2,7 +2,8 @@
 // the rows, every input byte fetched from HBM/L2 exactly once for any n <= 64
 // (krum.py:44-48, bulyan.py:49-54, brute.py:44-45: one pass PER PAIR plus a host sync each).
 //
-// What changed against k2_pairdist.cu (kept for unaligned rows):
+// What changed against the round-1 kernel (k2_pairdist.cu's layout with one thread issuing every
+// bulk copy; that file now holds only the cp.async variant, for rows that are not 16-byte aligned):
 //  * Balanced tasks.  Pairs are cut in tasks of 25 accumulator slots: the 5x5 block of two row
 //    groups (OFF), or a composite of diagonal blocks (COMP: two whole 5-row blocks, 10 pairs each,
 //    plus one 5-cycle of a third block; K5 = two edge-disjoint 5-cycles, so a block split over
@@ -25,8 +26,6 @@
 // Arithmetic is unchanged: (a-b)^2 formed directly (no Gram trick), coordinate pairs updated with
 // one FADD and one FFMA per coordinate (reduce.cuh), a bounded number of fp32 terms per accumulator
 // half, then a transposed warp reduction into fp64.
-#include <cstdlib>
-
 #include "dist.cuh"
 #include "k5_device.cuh"
 #include "launch.cuh"
@@ -50,11 +49,10 @@ constexpr int kSelfPerWarp = 3;
 constexpr int kTailGroup = 16;           // clusters per first-level group of the fused reduction
 constexpr int kTailTickets = 32;         // words of ticket scratch (1 + number of groups)
 // fp32 terms per accumulator half between two flushes into fp64.  32: worst-case relative error
-// 32 * 2^-24 = 1.9e-6 on one lane partial if every rounding went the same way; measured against
-// fp64 (tools/k2_ab.py) the summed distance is within 1e-8.
-#ifndef BZ_K2_FLUSH_TERMS
-#define BZ_K2_FLUSH_TERMS 32
-#endif
+// 32 * 2^-24 = 1.9e-6 on one lane partial if every rounding went the same way; the distance tests
+// hold the summed distance to rtol = 5e-7 against fp64 (test_cuda_abi.py, test_cuda_depth.py).
+// It decides the bits of every distance, which the reuse cache relies on: not a tuning knob.
+constexpr int kFlushTerms = 32;
 
 // Unique rows whose distance to themselves is needed (multiplicity > 1), spread over the warps.
 struct SelfList {
@@ -428,8 +426,8 @@ k2_ring(const __grid_constant__ RowTable rows, const __grid_constant__ SelfList 
   const int star_valid = task.kind == 3 ? min(star.slots, n - task.g1) : 0;
   const int o2 = (task.g2 >= 0 ? task.g2 : 0) * kG * T;
   // fp32 terms per accumulator half between two flushes into fp64 (a tile adds T / 64 of them)
-  constexpr int kFlushTiles = (BZ_K2_FLUSH_TERMS * 64) / T;
-  static_assert(kFlushTiles >= 1, "BZ_K2_FLUSH_TERMS");
+  constexpr int kFlushTiles = (kFlushTerms * 64) / T;
+  static_assert(kFlushTiles >= 1, "kFlushTerms");
 
   int pending = 0;
   int s = 0, sp = 0;
@@ -652,9 +650,45 @@ k2_ring(const __grid_constant__ RowTable rows, const __grid_constant__ SelfList 
 
 // ---- host side -------------------------------------------------------------------------------
 
-template <int T, int STAGES, bool SELF, bool CLUSTER, int W = kRWarps>
-static int launch_ring_cfg(const RowTable& rows, const SelfList& self, RingTail& tail, const StarList& star, int n, int C, int64_t d,
-                           double* parts, cudaStream_t st) {
+// The launch shapes: warps per CTA, tile width, ring depth, and whether C > 1 CTAs of a cluster share
+// each tile (multicast).
+struct RingShape { int W, T, stages; bool cluster; };
+enum { kShapeSmall, kShapeOne, kShapeCluster, kShapeWide };
+constexpr RingShape kShapes[] = {
+    {kRWarpsSmall, 512, 3, false},   // n <= 15 (all tasks fit 6 warps): two CTAs per SM
+    {kRWarps, 512, 4, false},        // n <= 25: one CTA per tile
+    {kRWarps, 512, 3, true},         // n <= 35: clusters of 12-warp CTAs
+    {kRWarpsWide, 256, 3, true},     // n >  35: clusters of 16-warp CTAs (512-column tiles with 2 stages
+                                     // measured 20 % slower at n = 40...51)
+};
+
+// The shape for n rows and its cluster size C (1 when all tasks fit one CTA).  Returns false when
+// the kernel does not support n.
+static bool ring_shape(int n, int& shape, int& C) {
+  const int ng = (n + kG - 1) / kG, tasks = ring_ntasks(ng);
+  if (tasks <= kRWarpsSmall && n <= 3 * kRWarpsSmall) shape = kShapeSmall;
+  else if (ng * kG > 35)                              shape = kShapeWide;
+  else                                                shape = tasks <= kRWarps ? kShapeOne : kShapeCluster;
+  const int W = kShapes[shape].W;
+  C = (tasks + W - 1) / W;
+  return C <= kRMaxCluster;
+}
+
+// Whether the scoring step's tables fit the ring's stage area, where it works once the ring is drained
+// (the barriers behind the stages stay untouched).  Kind 4 writes its block to global memory only.
+static bool tail_fits(const SelectTail& sel, size_t stage_area) {
+  if (sel.kind == 4) return true;
+  const size_t nn = (size_t)sel.n * sel.n * sizeof(double);
+  const size_t need = sel.kind == 3 ? nn + (size_t)(sel.n + 1) * (sel.n + 1) * sizeof(unsigned long long) + 64 * sizeof(double)
+                                    : 2 * nn + (size_t)sel.n * sizeof(double);
+  return stage_area >= need;
+}
+
+template <int S, bool SELF>
+static int launch_ring_cfg(const RowTable& rows, const SelfList& self, const RingTail& tail, const StarList& star, int n, int C,
+                           int64_t d, double* parts, cudaStream_t st) {
+  constexpr int T = kShapes[S].T, STAGES = kShapes[S].stages, W = kShapes[S].W;
+  constexpr bool CLUSTER = kShapes[S].cluster;
   const int ng = (n + kG - 1) / kG;
   const size_t smem = (size_t)STAGES * ng * kG * T * sizeof(float) + 2 * STAGES * sizeof(unsigned long long);
   auto kernel = k2_ring<T, STAGES, SELF, CLUSTER, W>;
@@ -695,50 +729,29 @@ static int launch_ring_cfg(const RowTable& rows, const SelfList& self, RingTail&
   if ((int64_t)nclusters > ntiles) nclusters = (int)(ntiles > 0 ? ntiles : 1);
   if (nclusters < 1) nclusters = 1;
   cfg.gridDim = dim3((unsigned)(nclusters * C));
-  if (tail.kind != 0) {
-    // the tail works in the ring's stage area (the barriers behind it stay untouched)
-    const size_t avail = (size_t)STAGES * ng * kG * T * sizeof(float);
-    const size_t nn = (size_t)tail.n * tail.n * sizeof(double);
-    const size_t fixed = tail.kind == 3 ? nn + (size_t)(tail.n + 1) * (tail.n + 1) * sizeof(unsigned long long) + 64 * sizeof(double)
-                                        : 2 * nn + (size_t)tail.n * sizeof(double);
-    if (tail.kind != 4 && avail < fixed) tail.kind = 0;          // does not fit: the caller launches K5 itself
-    else cudaMemsetAsync(tail.ticket, 0, kTailTickets * sizeof(unsigned), st);
-  }
-  if (tail.kind == 0 && star.count > 0) return -1;               // a star pass is only meaningful with the fused tail
+  if (tail.kind != 0) cudaMemsetAsync(tail.ticket, 0, kTailTickets * sizeof(unsigned), st);
   if (cudaLaunchKernelEx(&cfg, kernel, rows, self, tail, star, n, C, d, nfull, parts) != cudaSuccess) return -1;
   return nclusters;
 }
 
-// Launch shape for n rows: warps per CTA and CTAs per cluster (1 when all tasks fit one CTA).
-//   n <= 15 (all tasks fit 6 warps): 6 warps, two CTAs per SM       (BYZAGG_K2_W12=1: 12, for A/B runs)
-//   n <= 25: 12 warps;   n <= 35: clusters of 12-warp CTAs
-//   n >  35: clusters of 16-warp CTAs                                (BYZAGG_K2_W16=0: 12, for A/B runs)
-// Returns false when the kernel does not support n.
-static bool ring_shape(int n, int& W, int& C) {
-  static const bool w12 = [] { const char* e = getenv("BYZAGG_K2_W12"); return e && e[0] == '1'; }();
-  static const bool w16 = [] { const char* e = getenv("BYZAGG_K2_W16"); return !(e && e[0] == '0'); }();
-  const int ng = (n + kG - 1) / kG, tasks = ring_ntasks(ng);
-  W = kRWarps;
-  if (tasks <= kRWarpsSmall && n <= 3 * kRWarpsSmall && !w12) W = kRWarpsSmall;
-  else if (ng * kG > 35 && w16) W = kRWarpsWide;
-  C = (tasks + W - 1) / W;
-  if (C < 1) C = 1;
-  return C <= kRMaxCluster;
-}
-int ring_cluster_size(int n) {
-  int W, C;
-  return ring_shape(n, W, C) ? C : 0;
+template <bool SELF>
+static int launch_ring(int shape, const RowTable& rows, const SelfList& self, const RingTail& tail, const StarList& star, int n, int C,
+                       int64_t d, double* parts, cudaStream_t st) {
+  switch (shape) {
+    case kShapeSmall:   return launch_ring_cfg<kShapeSmall, SELF>(rows, self, tail, star, n, C, d, parts, st);
+    case kShapeOne:     return launch_ring_cfg<kShapeOne, SELF>(rows, self, tail, star, n, C, d, parts, st);
+    case kShapeCluster: return launch_ring_cfg<kShapeCluster, SELF>(rows, self, tail, star, n, C, d, parts, st);
+    default:            return launch_ring_cfg<kShapeWide, SELF>(rows, self, tail, star, n, C, d, parts, st);
+  }
 }
 
-// Returns the number of partial blocks written, or -1 when the configuration cannot run here
-// (the caller falls back to k2_pairdist).  `self_rows`: unique rows whose self distance K5 reads.
+// Returns the number of partial blocks written, or -1 when the rows are not 16-byte aligned or the
+// launch fails (the caller falls back to k2_pairdist).  `self_rows`: unique rows whose self distance K5 reads.
 int launch_pairdist_ring(const RowTable& rows, int n, int64_t d, double* parts, cudaStream_t st,
                          const unsigned char* self_rows, int nself, SelectTail* select) {
-  const char* env = getenv("BYZAGG_K2_CLUSTER");
-  const int force_cluster = env ? atoi(env) : 0;
-  int W, C;
-  if (!ring_shape(n, W, C)) return -1;
-  if (force_cluster > C && force_cluster <= kRMaxCluster) C = force_cluster;   // experiments: more CTAs per tile than needed
+  int shape, C;
+  if (!ring_shape(n, shape, C)) return -1;
+  const int W = kShapes[shape].W;
   if (nself > W * C * kSelfPerWarp) return -1;
   for (int r = 0; r < n && d > 0; ++r)           // an empty shard reads nothing: any address will do
     if ((((uintptr_t)rows.p[r]) & 15) != 0) return -1;
@@ -746,13 +759,13 @@ int launch_pairdist_ring(const RowTable& rows, int n, int64_t d, double* parts, 
   self.count = nself;
   for (int q = 0; q < nself; ++q) self.row[q] = self_rows[q];
   const int ng = (n + kG - 1) / kG;
-  const int rows_alloc = ng * kG;
-  const bool selfk = nself > 0;
+  const size_t stage_area = (size_t)kShapes[shape].stages * ng * kG * kShapes[shape].T * sizeof(float);
   RingTail tail = {};
   StarList star = {};
   for (int k = 0; k < kMaxN; ++k) tail.old_index[k] = -1;
-  const char* nofuse = getenv("BYZAGG_K2_NOFUSE");
-  if (select != nullptr && select->kind != 0 && !(nofuse && nofuse[0] == '1')) {
+  // The scoring step is fused only when it fits; otherwise the caller launches K5, and no star pass is
+  // prepared, so that a reuse call runs exactly the pass of the plain call.
+  if (select != nullptr && select->kind != 0 && tail_fits(*select, stage_area)) {
     tail.kind = select->kind; tail.n = select->n; tail.f = select->f; tail.m = select->m; tail.count = select->count;
     tail.total = select->total; tail.order = select->order; tail.status = select->status; tail.ticket = select->ticket;
     tail.map = make_map(select->to_unique, select->n, n);
@@ -768,9 +781,9 @@ int launch_pairdist_ring(const RowTable& rows, int n, int64_t d, double* parts, 
     }
     // Distance reuse: unique row k was row old_index[k] of the table in `cache_in`.  A star pass is
     // taken when 1..kStarMax unique rows are new, every other one is in the table, and that table
-    // came out of the same launch geometry (tile width, cluster size: functions of the row count) —
-    // then every pair has the bits the full pass would give it.
-    if (select->cache_in != nullptr && select->old_index != nullptr && select->u_old >= 1 && select->kind != 4 && force_cluster == 0) {
+    // came out of the same launch shape and cluster size (functions of the row count) — then every
+    // pair has the bits the full pass would give it.
+    if (select->cache_in != nullptr && select->old_index != nullptr && select->u_old >= 1 && select->kind != 4) {
       int fresh[kMaxN], nfresh = 0;
       bool ok = true;
       for (int k = 0; k < n; ++k) {
@@ -781,16 +794,13 @@ int launch_pairdist_ring(const RowTable& rows, int n, int64_t d, double* parts, 
         tail.old_index[k] = (signed char)oi;
         if (oi < 0) fresh[nfresh++] = k;
       }
-      const int old_ng = (select->u_old + kG - 1) / kG, old_alloc = old_ng * kG;
-      const auto geometry = [](int alloc, int c) { return c == 1 ? 0 : alloc <= 35 ? 1 : 2; };
       // 3 rows per star task when the cluster has the warps for it, else 25
       int slots = 3;
       if (nfresh * ((n + slots - 1) / slots) > W * C) slots = kRSlots;
       const int chunks = (n + slots - 1) / slots;
-      int old_W = 0, old_C = 0;
+      int old_shape = 0, old_C = 0;
       ok = ok && nfresh >= 1 && nfresh <= kStarMax && nfresh * chunks <= W * C && nfresh < n
-              && ring_shape(select->u_old, old_W, old_C) && old_C == C && old_W == W
-              && geometry(old_alloc, C) == geometry(rows_alloc, C);
+              && ring_shape(select->u_old, old_shape, old_C) && old_shape == shape && old_C == C;
       if (ok) {
         star.count = nfresh;
         star.slots = slots;
@@ -802,18 +812,8 @@ int launch_pairdist_ring(const RowTable& rows, int n, int64_t d, double* parts, 
       }
     }
   }
-#define BZ_RING(T, S, CL) (selfk ? launch_ring_cfg<T, S, true, CL>(rows, self, tail, star, n, C, d, parts, st) : launch_ring_cfg<T, S, false, CL>(rows, self, tail, star, n, C, d, parts, st))
-  int nparts;
-  if (C == 1) {
-    if (rows_alloc > 25) return -1;
-    if (W == kRWarpsSmall) nparts = selfk ? launch_ring_cfg<512, 3, true, false, kRWarpsSmall>(rows, self, tail, star, n, C, d, parts, st)
-                                          : launch_ring_cfg<512, 3, false, false, kRWarpsSmall>(rows, self, tail, star, n, C, d, parts, st);
-    else                   nparts = BZ_RING(512, 4, false);
-  } else if (rows_alloc <= 35) nparts = BZ_RING(512, 3, true);
-  else if (W == kRWarpsWide)   nparts = selfk ? launch_ring_cfg<256, 3, true, true, kRWarpsWide>(rows, self, tail, star, n, C, d, parts, st)
-                                              : launch_ring_cfg<256, 3, false, true, kRWarpsWide>(rows, self, tail, star, n, C, d, parts, st);
-  else                         nparts = BZ_RING(256, 3, true);   // (512-column tiles with 2 stages measured 20 % slower at n = 40...51)
-#undef BZ_RING
+  const int nparts = nself > 0 ? launch_ring<true>(shape, rows, self, tail, star, n, C, d, parts, st)
+                               : launch_ring<false>(shape, rows, self, tail, star, n, C, d, parts, st);
   if (select != nullptr) {
     select->fused = (nparts > 0 && tail.kind != 0) ? 1 : 0;
     if (!select->fused) select->reused = 0;

@@ -1,4 +1,4 @@
-// tma.cuh — mbarrier and bulk-copy (TMA, SASS UBLKCP) helpers shared by the K2 kernels.
+// tma.cuh — mbarrier and bulk-copy (TMA, SASS UBLKCP) helpers of the K2 ring (k2_ring.cu).
 #pragma once
 
 #include "common.cuh"
@@ -11,9 +11,6 @@ __device__ __forceinline__ void mbar_init(unsigned long long* bar, int count) {
 }
 __device__ __forceinline__ void mbar_arrive(unsigned long long* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(unsigned long long* bar, unsigned bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
 // BZ_MBAR_HINT_NS (A/B builds): suspend-time hint of try_wait.  Without it the hardware wait is
 // short and a waiting warp re-issues the probe ~28 times per tile (ncu, n = 25: SYNCS + BRA + YIELD
@@ -39,10 +36,5 @@ __device__ __forceinline__ void mbar_wait(unsigned long long* bar, unsigned pari
       ::"r"(smem_u32(bar)), "r"(parity) : "memory");
 #endif
 }
-__device__ __forceinline__ void tma_load_1d(float* dst, const float* src, unsigned bytes, unsigned long long* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-               ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
-
 
 }  // namespace bz

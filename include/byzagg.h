@@ -138,7 +138,7 @@ BZ_API int bz_cge(const float* const* rows, int n, int f, int64_t d, float* out,
  *              u x u table over the unique rows (pointer equality, first-appearance order)
  *   mode_out   HOST int: 1 = only the pairs of the new rows were computed (1..4 new unique rows
  *              and the launch geometry of the cached call), 0 = full pass, table written,
- *              -1 = full pass and NO table written (unaligned rows: the round-1 kernel ran)
+ *              -1 = full pass and NO table written (unaligned rows, or the fused tail does not fit)
  * Results are bit-identical to the plain calls: a reused pair has exactly the bits the full pass
  * gives it (same coordinate-to-lane mapping, same summation order). */
 BZ_API int bz_krum_reuse(const float* const* rows, int n, int f, int m, int64_t d, float* out, int32_t* order,

@@ -116,3 +116,38 @@ def test_reuse_with_non_finite_attack_rows_and_other_streams():
   assert engine.pair_cache_stats()["star"] == s0["star"]
   want, _ = _plain(bz, "krum", rows, f=f)
   assert torch.equal(got, want)
+
+def test_reuse_takes_the_plain_pass_when_the_fused_tail_does_not_fit():
+  """ 64 row entries over few distinct tensors: the fused scoring step works on a 64 x 64 table in the
+  ring's shared memory.  Over 15 distinct rows (6-warp shape, 3 stages of 15 x 512 floats) it fits;
+  over 10 (61,440 < 66,048 bytes) it does not, so the call with 1 new row among 10 takes no star pass:
+  it must run the very kernels of the plain call, give its bits and write no table ("off"). """
+  import byzantinemomentum_b200 as bz
+  from byzantinemomentum_b200 import engine
+  from torch.profiler import ProfilerActivity, profile
+  n, f, d = 64, 5, 30_011
+  distinct = _honest(15, d, 9)
+  before = engine.pair_cache_stats()
+  bz.gars["krum"](gradients=(distinct * 5)[:n], f=f)
+  s0 = engine.pair_cache_stats()
+  assert s0["full"] - before["full"] == 1, (before, s0)      # the table of the 15 rows is there to reuse
+  rows = ((distinct[:9] + [_attack(distinct, 0.8)]) * 7)[:n]
+
+  def run(reuse):
+    engine.config.reuse_distances = reuse
+    try:
+      with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        out = bz.gars["krum"](gradients=rows, f=f)
+        torch.cuda.synchronize()
+      sel = bz.last_selection()
+    finally:
+      engine.config.reuse_distances = True
+    return out, sel, sorted({e.name for e in prof.events() if "bz::" in e.name})
+
+  got, sel, got_kernels = run(True)
+  s1 = engine.pair_cache_stats()
+  want, want_sel, want_kernels = run(False)
+  assert torch.equal(got, want) and sel == want_sel
+  assert (s1["off"] - s0["off"], s1["star"] - s0["star"], s1["full"] - s0["full"]) == (1, 0, 0), (s0, s1)
+  assert any("k2_ring" in k for k in want_kernels), want_kernels
+  assert got_kernels == want_kernels, (got_kernels, want_kernels)
