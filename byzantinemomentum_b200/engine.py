@@ -13,6 +13,7 @@ compiled library every entry point raises; there is no CPU fallback.
 """
 
 import ctypes
+import functools
 import math
 import time
 import weakref
@@ -22,7 +23,7 @@ import torch
 from . import _lib, hostmem
 
 __all__ = ["average", "median", "trmean", "phocas", "meamed", "krum", "bulyan", "brute", "aksel", "cge",
-           "pairdist_partial", "rowdist_partial", "krum_select", "bulyan_select", "brute_select",
+           "pairdist_partial", "rowdist_partial", "select", "krum_select", "bulyan_select", "brute_select",
            "rowdist_select", "average_selected", "bulyan_reduce", "avg_dev_max_async", "compute_avg_dev_max", "rowdots_async", "study_step",
            "config", "Plan", "pair_cache_stats", "GradientStack", "host_path_report"]
 
@@ -65,6 +66,19 @@ def _workspace(device, stream):
       _workspaces.pop(next(iter(_workspaces)))
   _workspaces[key] = ws          # most recently used last
   return ws
+
+def _row_buffer(rows, d, device):
+  """ [rows, pitch] fp32 device buffer whose rows start 256-byte aligned (vector loads, TMA bulk copies). """
+  return torch.empty((rows, (d + 63) // 64 * 64), dtype=torch.float32, device=device)
+
+def _staging_buffer(device, rows, d):
+  """ The device buffer host rows are staged into; one shape is kept at a time. """
+  key = (device.index, rows, d)
+  buf = _staging.get(key)
+  if buf is None:
+    _staging.clear()
+    buf = _staging[key] = _row_buffer(rows, d, device)
+  return buf
 
 _F32 = torch.float32
 
@@ -109,6 +123,13 @@ class _HostPath:
       self.times.setdefault(key, {}).setdefault(mode, []).append(seconds)
 
 _host_paths = {}
+
+def _host_path(device):
+  path = _host_paths.get(device.index)
+  if path is None:
+    path = _host_paths[device.index] = _HostPath()
+  return path
+
 forced_host_path = None      # tests / A-B runs: pin the host path ("lanes", "lane", "pipeline") instead of measuring
 _PIPELINE_CHUNKS = 4       # column chunks of the host pipeline: H2D, kernel and D2H of three chunks overlap
 _RULE_CODES = dict(average=0, median=1, trmean=2, phocas=3, meamed=4)      # BZ_RULE_*
@@ -209,20 +230,11 @@ def _prepare(gradients, single_pass=False):
     for g in gradients:
       uniq.setdefault(id(g), g)
     pinned = False          # never asked: Tensor.is_pinned() is a slow driver query on some boxes
-    path = _host_paths.get(device.index)
-    if path is None:
-      path = _host_paths[device.index] = _HostPath()
-    mode = path.choose(single_pass, pinned)
+    mode = _host_path(device).choose(single_pass, pinned)
     prep.host_mode = (single_pass, pinned, mode)
     torch.cuda.current_stream(device).synchronize()        # the clock below times this call only
     prep.host_t0 = time.perf_counter()
-    key = (device.index, len(uniq), d)
-    buf = _staging.get(key)
-    if buf is None:
-      _staging.clear()
-      pitch = (d + 63) // 64 * 64       # rows 256-byte aligned: keeps the vector-load path
-      buf = torch.empty((len(uniq), pitch), dtype=torch.float32, device=device)
-      _staging[key] = buf
+    buf = _staging_buffer(device, len(uniq), d)
     # The row copies go out on several streams.  Measured (tools/h2d_probe2.py, two-socket host):
     # pinned rows that live on the OTHER socket's memory copy at 8.5 GB/s on one stream and at
     # 53 GB/s on two or more — with one stream the e2e step took 12.5 ms, 2.5x the box's own PCIe
@@ -237,9 +249,7 @@ def _prepare(gradients, single_pass=False):
     slot = {}
     if mode == "batch":
       hosts = (ctypes.c_void_p * len(uniq))(*[g.data_ptr() for g in uniq.values()])
-      with _on(device):
-        code = _lib.lib().bz_stage_rows(hosts, len(uniq), d, buf.data_ptr(), buf.stride(0), lanes[0].cuda_stream)
-      _lib.check(code, "bz_stage_rows")
+      _run(device, _lib.lib().bz_stage_rows, (hosts, len(uniq), d, buf.data_ptr(), buf.stride(0), lanes[0].cuda_stream))
       for k, ident in enumerate(uniq):
         slot[ident] = buf[k, :d]
     else:
@@ -280,7 +290,20 @@ class _on:
     if self.prev is not None:
       torch.cuda.set_device(self.prev)
 
-_host_out = {}
+def _call(fn, args):
+  """ One C-ABI call; raises on a non-zero return code. """
+  code = fn(*args)
+  if code != 0:
+    _lib.check(code, fn.__name__)
+
+def _run(device, fn, args):
+  """ `_call` with `device` current. """
+  with _on(device):
+    _call(fn, args)
+
+def _check_like_rows(vector, prep, what):
+  if vector.dtype != torch.float32 or vector.shape != (prep.d,) or vector.device != prep.device or not vector.is_contiguous():
+    raise ValueError(f"{what} must be a contiguous float32 vector like the rows")
 
 def _finish(prep, out):
   """ Device result for device inputs; for staged host inputs, a NEW host tensor (the copy goes
@@ -312,46 +335,36 @@ def _coordinate_pipeline(name, gradients, f, path, device):
   t0 = time.perf_counter()
   n, d = len(gradients), gradients[0].shape[0]
   rows = [g if g.is_contiguous() else g.contiguous() for g in gradients]
-  pitch = (d + 63) // 64 * 64
-  key = (device.index, n, d)
-  buf = _staging.get(key)
-  if buf is None or buf.shape[0] < n:
-    _staging.clear()
-    buf = _staging[key] = torch.empty((n, pitch), dtype=torch.float32, device=device)
+  buf = _staging_buffer(device, n, d)
   out = torch.empty(d, dtype=torch.float32, device=device)
   result = torch.empty(d, dtype=torch.float32, pin_memory=True)
   current = torch.cuda.current_stream(device)
   lanes = _copy_streams(device)
   ptrs = (ctypes.c_void_p * n)(*[g.data_ptr() for g in rows])
-  with _on(device):
-    code = _lib.lib().bz_coordinate_host(_RULE_CODES[name], ptrs, n, 0 if f is None else int(f), d, result.data_ptr(),
-                                         buf.data_ptr(), pitch, out.data_ptr(), _PIPELINE_CHUNKS,
-                                         current.cuda_stream, lanes[0].cuda_stream, lanes[1].cuda_stream)
-  _lib.check(code, "bz_coordinate_host")
+  _run(device, _lib.lib().bz_coordinate_host, (_RULE_CODES[name], ptrs, n, 0 if f is None else int(f), d, result.data_ptr(),
+                                               buf.data_ptr(), buf.stride(0), out.data_ptr(), _PIPELINE_CHUNKS,
+                                               current.cuda_stream, lanes[0].cuda_stream, lanes[1].cuda_stream))
   current.synchronize()           # the host rows, `out` and the staging rows stay alive until here
   path.record(True, False, "pipeline", time.perf_counter() - t0)
   return result
+
+def _coordinate_call(name, prep, f, out):
+  """ (fn, args) of the coordinate-wise rule `name` writing to the address `out`. """
+  head = (prep.ptrs, prep.n, int(f)) if name in ("trmean", "phocas", "meamed") else (prep.ptrs, prep.n)
+  return getattr(_lib.lib(), "bz_" + name), head + (prep.d, out, prep.stream)
 
 def _coordinate(name, gradients, f=None):
   if type(gradients) in (list, tuple) and len(gradients) > 0 and isinstance(gradients[0], torch.Tensor) and gradients[0].device.type == "cpu" and torch.cuda.is_available():
     _validate(gradients)
     _lib.lib()
     device = torch.device("cuda", torch.cuda.current_device())
-    path = _host_paths.get(device.index)
-    if path is None:
-      path = _host_paths[device.index] = _HostPath()
+    path = _host_path(device)
     if path.choose(True, False) == "pipeline":
       torch.cuda.current_stream(device).synchronize()        # the clock times this call only
       return _coordinate_pipeline(name, gradients, f, path, device)
   prep = _prepare(gradients, single_pass=True)
   out = torch.empty(prep.d, dtype=torch.float32, device=prep.device)
-  fn = getattr(_lib.lib(), "bz_" + name)
-  with _on(prep.device):
-    if f is None:
-      code = fn(prep.ptrs, prep.n, prep.d, out.data_ptr(), prep.stream)
-    else:
-      code = fn(prep.ptrs, prep.n, int(f), prep.d, out.data_ptr(), prep.stream)
-  _lib.check(code, "bz_" + name)
+  _run(prep.device, *_coordinate_call(name, prep, f, out.data_ptr()))
   return _finish(prep, out)
 
 def average(gradients):
@@ -451,95 +464,87 @@ def pair_cache_stats(device_index=None):
   return dict(cache.stats) if cache is not None else dict(full=0, star=0, off=0)
 
 # ---------------------------------------------------------------------------- #
-# Distance-based rules (single device).  Each returns (out, selection) where `selection` is a
-# DEVICE int32 tensor (all n indices by increasing score/distance; brute: the n-f subset).
+# Distance-based rules: what each one runs, resolved once for the plain call, `Plan` and the
+# phases of the d-sharded path
 
-def _aux(prep):
+DISTANCE_BASED = ("krum", "bulyan", "brute", "aksel", "cge")
+
+class _Rule:
+  """ The facts of a distance-based rule for (gar, n, f, m, mode):
+    m              Multi-Krum selection size (krum, bulyan; default n - f - 2)
+    params         its arguments after (rows, n) in `bz_<gar>`
+    pair           the distances are pairwise (else from every row to `center`)
+    center         the distances are to the coordinate-wise median (aksel; else cge: to the origin)
+    select, select_params   phase B: `bz_<select>_select[_peers]`, its arguments after (blocks, R, n)
+                            (those of `<select>_select[_peers]` after (blocks, n))
+    status         the rule reports a status word, after the n-entry order (bulyan, brute)
+    count, zero_init        phase C of all but bulyan: average of the first `count` selected rows
+    length         length of the selection returned """
+  __slots__ = ("gar", "n", "f", "m", "params", "pair", "center", "select", "select_params", "status", "count", "zero_init", "length")
+  def __init__(self, gar, n, f, m, mode):
+    if gar not in DISTANCE_BASED:
+      raise KeyError(f"unknown aggregation rule {gar!r}")
+    f = int(f)
+    m = n - f - 2 if m is None else int(m)
+    self.gar, self.n, self.f, self.m = gar, n, f, m
+    self.pair = gar in ("krum", "bulyan", "brute")
+    self.center = gar == "aksel"
+    self.status = gar in ("bulyan", "brute")
+    self.zero_init = gar != "cge"
+    self.length = n - f if gar == "brute" else n
+    if gar == "aksel":
+      if mode not in _lib.AKSEL_MODES:
+        raise NotImplementedError(mode)      # aksel.py:47-48
+      self.params = (f, _lib.AKSEL_MODES[mode])
+      self.count = (n + 1) // 2 if mode == "mid" else n - f
+    else:
+      self.params = (f, m) if gar in ("krum", "bulyan") else (f,)
+      self.count = m if gar == "krum" else n - f
+    self.select = gar if self.pair else "rowdist"
+    self.select_params = (f, m) if gar == "bulyan" else (f,) if self.pair else (int(gar == "cge"),)
+  def entry(self, ptrs, d, out, meta, ws, stream, reuse=()):
+    """ (fn, args) of the single-GPU call `bz_<gar>` writing to the addresses `out` and `meta`
+    (order[n] + status), or of `bz_<gar>_reuse` given the distance cache's `reuse` arguments. """
+    status = (meta + 4 * self.n,) if self.status else ()
+    fn = getattr(_lib.lib(), "bz_" + self.gar + ("_reuse" if reuse else ""))
+    return fn, (ptrs, self.n) + self.params + (d, out, meta) + status + reuse + (ws.data_ptr(), ws.numel(), stream)
+
+@functools.lru_cache(maxsize=256)
+def _rule(gar, n, f, m=None, mode="mid"):
+  """ The `_Rule` of these arguments; KeyError for an unknown rule, NotImplementedError for an unknown aksel mode. """
+  return _Rule(gar, n, f, m, mode)
+
+def _distance(gar, gradients, f, m=None, mode="mid"):
+  """ The single-device call: (out, selection) where `selection` is a DEVICE int32 tensor (all n
+  indices by increasing score/distance; brute: the n-f subset). """
+  rule = _rule(gar, len(gradients) if isinstance(gradients, (list, tuple)) else 0, f, m, mode)    # before the device is touched
+  prep = _prepare(gradients)
+  out = torch.empty(prep.d, dtype=torch.float32, device=prep.device)
   ws = _workspace(prep.device, prep.stream)
   meta = torch.empty(prep.n + 1, dtype=torch.int32, device=prep.device)   # order[n] + status
-  return ws, meta
-
-def krum(gradients, f, m):
-  prep = _prepare(gradients)
-  out = torch.empty(prep.d, dtype=torch.float32, device=prep.device)
-  ws, meta = _aux(prep)
-  cache = _pair_cache(prep, gradients)
-  with _on(prep.device):
-    if cache is None:
-      code = _lib.lib().bz_krum(prep.ptrs, prep.n, int(f), int(m), prep.d, out.data_ptr(), meta.data_ptr(),
-                                ws.data_ptr(), ws.numel(), prep.stream)
-    else:
-      old, cache_in, u_old = cache.old_index(gradients, prep.d, prep.stream)
-      code = _lib.lib().bz_krum_reuse(prep.ptrs, prep.n, int(f), int(m), prep.d, out.data_ptr(), meta.data_ptr(), old, cache_in, u_old,
-                                      cache.out_buffer(), ctypes.byref(cache.mode), ws.data_ptr(), ws.numel(), prep.stream)
-  _lib.check(code, "bz_krum")
+  cache = _pair_cache(prep, gradients) if rule.pair else None
+  reuse = () if cache is None else cache.old_index(gradients, prep.d, prep.stream) + (cache.out_buffer(), ctypes.byref(cache.mode))
+  _run(prep.device, *rule.entry(prep.ptrs, prep.d, out.data_ptr(), meta.data_ptr(), ws, prep.stream, reuse))
   if cache is not None:
     cache.update(gradients, prep.d, prep.stream)
-  return _finish(prep, out), meta[:prep.n]
+  if rule.status and config.strict_status:
+    _raise_status(int(meta[prep.n].item()))
+  return _finish(prep, out), meta[:rule.length]
 
-def bulyan(gradients, f, m):
-  prep = _prepare(gradients)
-  out = torch.empty(prep.d, dtype=torch.float32, device=prep.device)
-  ws, meta = _aux(prep)
-  status = meta[prep.n:]
-  cache = _pair_cache(prep, gradients)
-  with _on(prep.device):
-    if cache is None:
-      code = _lib.lib().bz_bulyan(prep.ptrs, prep.n, int(f), int(m), prep.d, out.data_ptr(), meta.data_ptr(),
-                                  status.data_ptr(), ws.data_ptr(), ws.numel(), prep.stream)
-    else:
-      old, cache_in, u_old = cache.old_index(gradients, prep.d, prep.stream)
-      code = _lib.lib().bz_bulyan_reuse(prep.ptrs, prep.n, int(f), int(m), prep.d, out.data_ptr(), meta.data_ptr(), status.data_ptr(),
-                                        old, cache_in, u_old, cache.out_buffer(), ctypes.byref(cache.mode), ws.data_ptr(), ws.numel(), prep.stream)
-  _lib.check(code, "bz_bulyan")
-  if cache is not None:
-    cache.update(gradients, prep.d, prep.stream)
-  if config.strict_status:
-    _raise_status(int(status.item()))
-  return _finish(prep, out), meta[:prep.n]
+def krum(gradients, f, m=None):
+  return _distance("krum", gradients, f, m)
+
+def bulyan(gradients, f, m=None):
+  return _distance("bulyan", gradients, f, m)
 
 def brute(gradients, f):
-  prep = _prepare(gradients)
-  out = torch.empty(prep.d, dtype=torch.float32, device=prep.device)
-  ws, meta = _aux(prep)
-  status = meta[prep.n:]
-  cache = _pair_cache(prep, gradients)
-  with _on(prep.device):
-    if cache is None:
-      code = _lib.lib().bz_brute(prep.ptrs, prep.n, int(f), prep.d, out.data_ptr(), meta.data_ptr(),
-                                 status.data_ptr(), ws.data_ptr(), ws.numel(), prep.stream)
-    else:
-      old, cache_in, u_old = cache.old_index(gradients, prep.d, prep.stream)
-      code = _lib.lib().bz_brute_reuse(prep.ptrs, prep.n, int(f), prep.d, out.data_ptr(), meta.data_ptr(), status.data_ptr(),
-                                       old, cache_in, u_old, cache.out_buffer(), ctypes.byref(cache.mode), ws.data_ptr(), ws.numel(), prep.stream)
-  _lib.check(code, "bz_brute")
-  if cache is not None:
-    cache.update(gradients, prep.d, prep.stream)
-  if config.strict_status:
-    _raise_status(int(status.item()))
-  return _finish(prep, out), meta[:prep.n - int(f)]
+  return _distance("brute", gradients, f)
 
 def aksel(gradients, f, mode="mid"):
-  if mode not in _lib.AKSEL_MODES:
-    raise NotImplementedError(mode)      # aksel.py:47-48
-  prep = _prepare(gradients)
-  out = torch.empty(prep.d, dtype=torch.float32, device=prep.device)
-  ws, meta = _aux(prep)
-  with _on(prep.device):
-    code = _lib.lib().bz_aksel(prep.ptrs, prep.n, int(f), _lib.AKSEL_MODES[mode], prep.d, out.data_ptr(),
-                               meta.data_ptr(), ws.data_ptr(), ws.numel(), prep.stream)
-  _lib.check(code, "bz_aksel")
-  return _finish(prep, out), meta[:prep.n]
+  return _distance("aksel", gradients, f, mode=mode)
 
 def cge(gradients, f):
-  prep = _prepare(gradients)
-  out = torch.empty(prep.d, dtype=torch.float32, device=prep.device)
-  ws, meta = _aux(prep)
-  with _on(prep.device):
-    code = _lib.lib().bz_cge(prep.ptrs, prep.n, int(f), prep.d, out.data_ptr(), meta.data_ptr(),
-                             ws.data_ptr(), ws.numel(), prep.stream)
-  _lib.check(code, "bz_cge")
-  return _finish(prep, out), meta[:prep.n]
+  return _distance("cge", gradients, f)
 
 # ---------------------------------------------------------------------------- #
 # Study metrics on the same stack (tools/pytorch.py:97-125, attack.py:846-848)
@@ -551,40 +556,44 @@ def avg_dev_max_async(samples):
   avg = torch.empty(prep.d, dtype=torch.float32, device=prep.device)
   stats = torch.empty(2 + prep.n, dtype=torch.float64, device=prep.device)
   ws = _workspace(prep.device, prep.stream)
-  with _on(prep.device):
-    code = _lib.lib().bz_avg_dev_max(prep.ptrs, prep.n, prep.d, avg.data_ptr(), stats.data_ptr(),
-                                     ws.data_ptr(), ws.numel(), prep.stream)
-  _lib.check(code, "bz_avg_dev_max")
+  _run(prep.device, _lib.lib().bz_avg_dev_max, (prep.ptrs, prep.n, prep.d, avg.data_ptr(), stats.data_ptr(), ws.data_ptr(), ws.numel(), prep.stream))
   return avg, stats
 
-class _StudyMemo:
-  """ Last `compute_avg_dev_max` result, valid for the very same tensor objects at the same
-  addresses and in-place versions (weak references: a dead or different tensor never matches).
-  attack.py:846-847 asks for the sampled and for the honest gradients; without worker/server-side
-  momentum and with nb_for_study = nb_honests those are the SAME tensors (`grad_honests =
-  grad_sampleds[:nb_honests]`, attack.py:808): the second pass over n x d is saved. """
+class _Memo:
+  """ One result of a computation `what` with parameters `params`, valid only for the very tensor
+  OBJECTS it was computed on (held through weak references, compared with `is`, like `_CallCache`),
+  at the same addresses and in-place versions: a freed list whose ids / addresses are reused by new
+  tensors can never match, and a dead reference drops the entry. """
   def __init__(self):
-    self.refs = self.state = self.result = None
-  def lookup(self, samples):
-    if self.refs is None or len(self.refs) != len(samples):
-      return None
-    for ref, g in zip(self.refs, samples):
-      if ref() is not g:
-        return None
-    if tuple((g.data_ptr(), g._version) for g in samples) != self.state:
-      return None
-    avg, a, b, c = self.result
-    return avg.clone(), a, b, c                               # callers own the average they get (grad_pasts keeps it)
-  def store(self, samples, result):
+    self.clear()
+  def clear(self):
+    self.what = self.params = self.refs = self.state = self.value = None
+  @staticmethod
+  def _state(tensors):
+    return tuple((g.data_ptr(), g._version) for g in tensors)
+  def store(self, what, params, tensors, value):
     try:
-      self.refs = tuple(weakref.ref(g) for g in samples)
+      refs = tuple(weakref.ref(g) for g in tensors)
     except TypeError:
-      self.refs = None
+      self.clear()
       return
-    self.state = tuple((g.data_ptr(), g._version) for g in samples)
-    self.result = result
+    self.what, self.params, self.refs, self.state, self.value = what, params, refs, self._state(tensors), value
+  def lookup(self, what, params, tensors):
+    if self.refs is None or self.what != what or self.params != params or len(self.refs) != len(tensors):
+      return None
+    for ref, g in zip(self.refs, tensors):
+      if ref() is not g:
+        if ref() is None:
+          self.clear()
+        return None
+    if self._state(tensors) != self.state:
+      return None
+    return self.value
 
-_study_memo = _StudyMemo()
+# attack.py:846-847 asks for the sampled and for the honest gradients; without worker/server-side
+# momentum and with nb_for_study = nb_honests those are the SAME tensors (`grad_honests =
+# grad_sampleds[:nb_honests]`, attack.py:808): the second pass over n x d is saved.
+_study_memo = _Memo()
 
 def compute_avg_dev_max(samples):
   """ Drop-in for `tools.compute_avg_dev_max(samples)` (tools/pytorch.py:97-125): returns
@@ -593,11 +602,12 @@ def compute_avg_dev_max(samples):
   n = len(samples)
   if n == 0:
     return None, math.nan, math.nan, math.nan                 # :105-106
-  hit = _study_memo.lookup(samples)
+  hit = _study_memo.lookup("avg_dev_max", (), samples)
   if hit is not None:
-    return hit
+    avg, a, b, c = hit
+    return avg.clone(), a, b, c                               # callers own the average they get (grad_pasts keeps it)
   result = _compute_avg_dev_max(samples, n)
-  _study_memo.store(samples, (result[0].clone(),) + result[1:])
+  _study_memo.store("avg_dev_max", (), samples, (result[0].clone(),) + result[1:])
   return result
 
 def _compute_avg_dev_max(samples, n):
@@ -631,13 +641,10 @@ def rowdots_async(center, rows):
   if len(rows) > _lib.MAX_N:
     return torch.cat([rowdots_async(center, rows[k:k + _lib.MAX_N]) for k in range(0, len(rows), _lib.MAX_N)])
   prep = _prepare_device(rows, "the study dot products take CUDA tensors")
-  if center.dtype != torch.float32 or center.shape != (prep.d,) or center.device != prep.device or not center.is_contiguous():
-    raise ValueError("center must be a contiguous float32 vector like the rows")
+  _check_like_rows(center, prep, "center")
   out = torch.empty(prep.n, dtype=torch.float64, device=prep.device)
   ws = _workspace(prep.device, prep.stream)
-  with _on(prep.device):
-    code = _lib.lib().bz_rowdots(prep.ptrs, prep.n, center.data_ptr(), prep.d, out.data_ptr(), ws.data_ptr(), ws.numel(), prep.stream)
-  _lib.check(code, "bz_rowdots")
+  _run(prep.device, _lib.lib().bz_rowdots, (prep.ptrs, prep.n, center.data_ptr(), prep.d, out.data_ptr(), ws.data_ptr(), ws.numel(), prep.stream))
   return out
 
 def study_step(grad_sampleds, grad_honests, grad_attacks, grad_defense, pasts, momentum):
@@ -718,143 +725,108 @@ def _prepare_device(gradients, message="the sharded phases take CUDA tensors"):
     raise ValueError(message)
   return prep
 
-def pairdist_partial(gradients):
-  """ [n, n] fp64: this shard's share of the squared pairwise distances (entries i < j). """
-  prep = _prepare_device(gradients)
-  part = torch.empty((prep.n, prep.n), dtype=torch.float64, device=prep.device)
-  ws = _workspace(prep.device, prep.stream)
-  with _on(prep.device):
-    code = _lib.lib().bz_pairdist_partial(prep.ptrs, prep.n, prep.d, part.data_ptr(), ws.data_ptr(), ws.numel(), prep.stream)
-  _lib.check(code, "bz_pairdist_partial")
-  return part
+def _partial_call(prep, pair, center, part, ws):
+  """ (fn, args) of phase A: this shard's share of the squared pairwise distances (`pair`), or of the
+  squared distances of the rows to the address `center` (None: the origin), written to `part`. """
+  lib = _lib.lib()
+  if pair:
+    return lib.bz_pairdist_partial, (prep.ptrs, prep.n, prep.d, part, ws.data_ptr(), ws.numel(), prep.stream)
+  return lib.bz_rowdist_partial, (prep.ptrs, prep.n, center, prep.d, part, ws.data_ptr(), ws.numel(), prep.stream)
 
-def rowdist_partial(gradients, center=None):
-  """ [n] fp64: this shard's share of the squared distance of every row to `center` (None: origin). """
+def _partial(gradients, pair, center, out):
   prep = _prepare_device(gradients)
-  part = torch.empty(prep.n, dtype=torch.float64, device=prep.device)
-  ws = _workspace(prep.device, prep.stream)
-  cptr = None
   if center is not None:
-    if center.dtype != torch.float32 or center.shape != (prep.d,) or center.device != prep.device or not center.is_contiguous():
-      raise ValueError("center must be a contiguous float32 vector like the rows")
-    cptr = center.data_ptr()
-  with _on(prep.device):
-    code = _lib.lib().bz_rowdist_partial(prep.ptrs, prep.n, cptr, prep.d, part.data_ptr(), ws.data_ptr(), ws.numel(), prep.stream)
-  _lib.check(code, "bz_rowdist_partial")
-  return part
+    _check_like_rows(center, prep, "center")
+    center = center.data_ptr()
+  if out is None:
+    out = torch.empty((prep.n, prep.n) if pair else prep.n, dtype=torch.float64, device=prep.device)
+  _run(prep.device, *_partial_call(prep, pair, center, out.data_ptr(), _workspace(prep.device, prep.stream)))
+  return out
 
-def _select_common(parts, n):
-  if parts.dtype != torch.float64 or not parts.is_contiguous() or parts.device.type != "cuda":
-    raise ValueError("parts must be a contiguous float64 CUDA tensor")
-  nparts = parts.shape[0]
-  meta = torch.empty(n + 1, dtype=torch.int32, device=parts.device)
-  stream = torch.cuda.current_stream(parts.device).cuda_stream
-  return nparts, meta, stream
+def pairdist_partial(gradients, out=None):
+  """ [n, n] fp64: this shard's share of the squared pairwise distances (entries i < j); written
+  into `out` when given (e.g. this rank's slot of a symmetric buffer). """
+  return _partial(gradients, True, None, out)
+
+def rowdist_partial(gradients, center=None, out=None):
+  """ [n] fp64: this shard's share of the squared distance of every row to `center` (None: origin);
+  written into `out` when given. """
+  return _partial(gradients, False, center, out)
+
+def _select_call(rule, blocks, meta, stream):
+  """ (fn, args) of phase B writing the order (and status word) to the address `meta`: `bz_<rule>_select`
+  on the gathered blocks (a [R, ...] fp64 CUDA tensor), or `bz_<rule>_select_peers` on a list of R
+  device addresses of the ranks' blocks (rank order, mapped over NVLink: read in place). """
+  if isinstance(blocks, torch.Tensor):
+    if blocks.dtype != torch.float64 or not blocks.is_contiguous() or blocks.device.type != "cuda":
+      raise ValueError("parts must be a contiguous float64 CUDA tensor")
+    suffix, nparts, table = "", blocks.shape[0], blocks.data_ptr()
+  else:
+    if not 1 <= len(blocks) <= _lib.MAX_PEERS:
+      raise ValueError(f"{len(blocks)} peers, expected 1..{_lib.MAX_PEERS}")
+    suffix, nparts, table = "_peers", len(blocks), (ctypes.c_void_p * len(blocks))(*[int(p) for p in blocks])
+  status = (meta + 4 * rule.n,) if rule.status else ()
+  fn = getattr(_lib.lib(), "bz_" + rule.select + "_select" + suffix)
+  return fn, (table, nparts, rule.n) + rule.select_params + (meta,) + status + (stream,)
+
+def select(gar, blocks, n, f, m=None, device=None):
+  """ Phase B of a distance-based rule from the R partial blocks, `blocks` as in `_select_call`
+  (peer addresses: the selection goes to `device`).  Returns the selection at the rule's length (a
+  device int32 tensor), with the status word for bulyan and brute. """
+  rule = _rule(gar, n, f, m)
+  if isinstance(blocks, torch.Tensor):
+    device = blocks.device
+  meta = torch.empty(n + 1, dtype=torch.int32, device=device)
+  _run(device, *_select_call(rule, blocks, meta.data_ptr(), torch.cuda.current_stream(device).cuda_stream))
+  return (meta[:rule.length], meta[n:]) if rule.status else meta[:n]
 
 def krum_select(parts, n, f):
-  """ parts: [R, n, n] gathered partial blocks -> order (device int32[n]). """
-  nparts, meta, stream = _select_common(parts, n)
-  with _on(parts.device):
-    code = _lib.lib().bz_krum_select(parts.data_ptr(), nparts, n, int(f), meta.data_ptr(), stream)
-  _lib.check(code, "bz_krum_select")
-  return meta[:n]
+  return select("krum", parts, n, f)
 
 def bulyan_select(parts, n, f, m):
-  nparts, meta, stream = _select_common(parts, n)
-  with _on(parts.device):
-    code = _lib.lib().bz_bulyan_select(parts.data_ptr(), nparts, n, int(f), int(m), meta.data_ptr(), meta[n:].data_ptr(), stream)
-  _lib.check(code, "bz_bulyan_select")
-  return meta[:n], meta[n:]
+  return select("bulyan", parts, n, f, m)
 
 def brute_select(parts, n, f):
-  nparts, meta, stream = _select_common(parts, n)
-  with _on(parts.device):
-    code = _lib.lib().bz_brute_select(parts.data_ptr(), nparts, n, int(f), meta.data_ptr(), meta[n:].data_ptr(), stream)
-  _lib.check(code, "bz_brute_select")
-  return meta[:n - int(f)], meta[n:]
+  return select("brute", parts, n, f)
 
 def rowdist_select(parts, n, sqrt_norm):
-  nparts, meta, stream = _select_common(parts, n)
-  with _on(parts.device):
-    code = _lib.lib().bz_rowdist_select(parts.data_ptr(), nparts, n, 1 if sqrt_norm else 0, meta.data_ptr(), stream)
-  _lib.check(code, "bz_rowdist_select")
-  return meta[:n]
-
-# Peer-memory variants of phase B: `peer_ptrs` is a list of R device addresses (one per rank, rank
-# order) of the ranks' partial blocks, mapped over NVLink; the blocks are read in place.
-
-def _peers(peer_ptrs, n, device):
-  if not 1 <= len(peer_ptrs) <= _lib.MAX_PEERS:
-    raise ValueError(f"{len(peer_ptrs)} peers, expected 1..{_lib.MAX_PEERS}")
-  table = (ctypes.c_void_p * len(peer_ptrs))(*[int(p) for p in peer_ptrs])
-  meta = torch.empty(n + 1, dtype=torch.int32, device=device)
-  return table, meta, torch.cuda.current_stream(device).cuda_stream
+  return select("cge" if sqrt_norm else "aksel", parts, n, 0)     # the order of the row distances: f plays no part
 
 def krum_select_peers(peer_ptrs, n, f, device):
-  table, meta, stream = _peers(peer_ptrs, n, device)
-  with _on(device):
-    code = _lib.lib().bz_krum_select_peers(table, len(peer_ptrs), n, int(f), meta.data_ptr(), stream)
-  _lib.check(code, "bz_krum_select_peers")
-  return meta[:n]
+  return select("krum", peer_ptrs, n, f, device=device)
 
 def bulyan_select_peers(peer_ptrs, n, f, m, device):
-  table, meta, stream = _peers(peer_ptrs, n, device)
-  with _on(device):
-    code = _lib.lib().bz_bulyan_select_peers(table, len(peer_ptrs), n, int(f), int(m), meta.data_ptr(), meta[n:].data_ptr(), stream)
-  _lib.check(code, "bz_bulyan_select_peers")
-  return meta[:n], meta[n:]
+  return select("bulyan", peer_ptrs, n, f, m, device=device)
 
 def brute_select_peers(peer_ptrs, n, f, device):
-  table, meta, stream = _peers(peer_ptrs, n, device)
-  with _on(device):
-    code = _lib.lib().bz_brute_select_peers(table, len(peer_ptrs), n, int(f), meta.data_ptr(), meta[n:].data_ptr(), stream)
-  _lib.check(code, "bz_brute_select_peers")
-  return meta[:n - int(f)], meta[n:]
+  return select("brute", peer_ptrs, n, f, device=device)
 
 def rowdist_select_peers(peer_ptrs, n, sqrt_norm, device):
-  table, meta, stream = _peers(peer_ptrs, n, device)
-  with _on(device):
-    code = _lib.lib().bz_rowdist_select_peers(table, len(peer_ptrs), n, 1 if sqrt_norm else 0, meta.data_ptr(), stream)
-  _lib.check(code, "bz_rowdist_select_peers")
-  return meta[:n]
+  return select("cge" if sqrt_norm else "aksel", peer_ptrs, n, 0, device=device)
 
-def pairdist_partial_into(gradients, part):
-  """ Phase A writing straight into `part` (e.g. this rank's slot of a symmetric buffer). """
-  prep = _prepare_device(gradients)
-  ws = _workspace(prep.device, prep.stream)
-  with _on(prep.device):
-    code = _lib.lib().bz_pairdist_partial(prep.ptrs, prep.n, prep.d, part.data_ptr(), ws.data_ptr(), ws.numel(), prep.stream)
-  _lib.check(code, "bz_pairdist_partial")
-  return part
+def _average_call(prep, selection, count, zero_init, divisor, status, out):
+  return _lib.lib().bz_average_selected, (prep.ptrs, prep.n, selection, int(count), 1 if zero_init else 0, float(divisor), status, prep.d, out, prep.stream)
 
-def rowdist_partial_into(gradients, center, part):
-  prep = _prepare_device(gradients)
-  ws = _workspace(prep.device, prep.stream)
-  cptr = None if center is None else center.data_ptr()
-  with _on(prep.device):
-    code = _lib.lib().bz_rowdist_partial(prep.ptrs, prep.n, cptr, prep.d, part.data_ptr(), ws.data_ptr(), ws.numel(), prep.stream)
-  _lib.check(code, "bz_rowdist_partial")
-  return part
+def _reduce_call(prep, rule, selection, status, out):
+  """ (fn, args) of phase C: the rule's reduce of the local shard over the selection, all addresses. """
+  if rule.gar == "bulyan":
+    return _lib.lib().bz_bulyan_reduce, (prep.ptrs, prep.n, rule.f, rule.m, selection, status, prep.d, out, prep.stream)
+  return _average_call(prep, selection, rule.count, rule.zero_init, rule.count, status if rule.status else None, out)
+
+def _ptr(tensor):
+  return None if tensor is None else tensor.data_ptr()
 
 def average_selected(gradients, selection, count, zero_init=True, divisor=None, status=None):
   """ Ordered-subset average of the local shard; `selection` is a device int32 tensor or None. """
   prep = _prepare_device(gradients)
   out = torch.empty(prep.d, dtype=torch.float32, device=prep.device)
-  sel_ptr = None if selection is None else selection.data_ptr()
-  st_ptr = None if status is None else status.data_ptr()
-  with _on(prep.device):
-    code = _lib.lib().bz_average_selected(prep.ptrs, prep.n, sel_ptr, int(count), 1 if zero_init else 0,
-                                          float(count if divisor is None else divisor), st_ptr, prep.d, out.data_ptr(), prep.stream)
-  _lib.check(code, "bz_average_selected")
+  _run(prep.device, *_average_call(prep, _ptr(selection), count, zero_init, count if divisor is None else divisor, _ptr(status), out.data_ptr()))
   return out
 
 def bulyan_reduce(gradients, f, m, order, status=None):
   prep = _prepare_device(gradients)
   out = torch.empty(prep.d, dtype=torch.float32, device=prep.device)
-  st_ptr = None if status is None else status.data_ptr()
-  with _on(prep.device):
-    code = _lib.lib().bz_bulyan_reduce(prep.ptrs, prep.n, int(f), int(m), order.data_ptr(), st_ptr, prep.d, out.data_ptr(), prep.stream)
-  _lib.check(code, "bz_bulyan_reduce")
+  _run(prep.device, *_reduce_call(prep, _rule("bulyan", prep.n, f, m), order.data_ptr(), _ptr(status), out.data_ptr()))
   return out
 
 # ---------------------------------------------------------------------------- #
@@ -878,14 +850,13 @@ class GradientStack:
   scale factor may differ by 1 ulp (ATen's fp32 norm order is build specific). """
   def __init__(self, n, d, device):
     self.n, self.d, self.device = n, d, torch.device(device)
-    pitch = (d + 63) // 64 * 64                     # rows 256-byte aligned: vector loads, TMA bulk copies
-    self._sampled = torch.empty((n, pitch), dtype=torch.float32, device=self.device)
+    self._sampled = _row_buffer(n, d, self.device)
+    self._pitch = self._sampled.stride(0)
     self._honest = None
-    self._pitch = pitch
     self._lib = _lib.lib()
   def _honest_buffer(self):
     if self._honest is None:
-      self._honest = torch.empty((self.n, self._pitch), dtype=torch.float32, device=self.device)
+      self._honest = _row_buffer(self.n, self.d, self.device)
     return self._honest
   def push(self, i, grad, clip=None, worker_momentum=None, server_momentum=None, mu=0., dampening=0.):
     """ Row i <- this worker's gradient.  Returns the sampled row (a view of the buffer). """
@@ -903,11 +874,8 @@ class GradientStack:
       raise ValueError("momentum must be a contiguous float32 vector like the gradient")
     stream = torch.cuda.current_stream(self.device).cuda_stream
     ws = _workspace(self.device, stream)
-    with _on(self.device):
-      code = self._lib.bz_gradient_row(grad.data_ptr(), self.d, float(clip) if clip is not None else 0., row.data_ptr(), mode,
-                                       None if mom is None else mom.data_ptr(), float(mu), 1. - float(dampening),
-                                       None if honest is None else honest.data_ptr(), ws.data_ptr(), ws.numel(), stream)
-    _lib.check(code, "bz_gradient_row")
+    _run(self.device, self._lib.bz_gradient_row, (grad.data_ptr(), self.d, float(clip) if clip is not None else 0., row.data_ptr(), mode,
+                                                  _ptr(mom), float(mu), 1. - float(dampening), _ptr(honest), ws.data_ptr(), ws.numel(), stream))
     # the kernel wrote through raw pointers: tell PyTorch (the identity/version keyed caches of this
     # package — prepared arguments, selection, distance table, study memo — rely on the counter;
     # views share it with their base, so every row of the buffer is invalidated: conservative)
@@ -943,7 +911,6 @@ class Plan:
     prep = _prepare(list(gradients))
     if prep.to_cpu:
       raise ValueError("Plan takes CUDA tensors (host tensors go through the plain call, which stages them)")
-    lib = _lib.lib()
     n, d = prep.n, prep.d
     self.gar, self.n, self.d, self.device = gar, n, d, prep.device
     self.rows = list(gradients)
@@ -951,40 +918,20 @@ class Plan:
       # a packed copy would neither stay alive nor follow in-place updates of the originals
       raise ValueError("Plan takes contiguous rows (the plain call accepts strided views and packs them)")
     self.out = torch.empty(d, dtype=torch.float32, device=prep.device) if out is None else out
-    if self.out.dtype != torch.float32 or self.out.shape != (d,) or self.out.device != prep.device or not self.out.is_contiguous():
-      raise ValueError("out must be a contiguous float32 vector like the rows")
-    self._ptrs = (ctypes.c_void_p * n)(*[g.data_ptr() for g in self.rows])
-    self._stream = prep.stream
+    _check_like_rows(self.out, prep, "out")
     self.selection = None
     self.status = None
-    o, st = self.out.data_ptr(), self._stream
-    if gar in ("average", "median"):
-      fn, args = getattr(lib, "bz_" + gar), (self._ptrs, n, d, o, st)
-    elif gar in ("trmean", "phocas", "meamed"):
-      fn, args = getattr(lib, "bz_" + gar), (self._ptrs, n, int(f), d, o, st)
+    if gar in _RULE_CODES:
+      fn, args = _coordinate_call(gar, prep, f, self.out.data_ptr())
     else:
+      rule = _rule(gar, n, f, m, mode)
       self._ws = _workspace(prep.device, prep.stream)
       self._meta = torch.empty(n + 1, dtype=torch.int32, device=prep.device)
-      ws, wn, meta, status = self._ws.data_ptr(), self._ws.numel(), self._meta.data_ptr(), self._meta[n:].data_ptr()
-      self.selection = self._meta[:n]
-      if gar == "krum":
-        m = n - f - 2 if m is None else m
-        fn, args = lib.bz_krum, (self._ptrs, n, int(f), int(m), d, o, meta, ws, wn, st)
-      elif gar == "bulyan":
-        m = n - f - 2 if m is None else m
+      self.selection = self._meta[:rule.length]
+      if rule.status:
         self.status = self._meta[n:]
-        fn, args = lib.bz_bulyan, (self._ptrs, n, int(f), int(m), d, o, meta, status, ws, wn, st)
-      elif gar == "brute":
-        self.status = self._meta[n:]
-        self.selection = self._meta[:n - int(f)]
-        fn, args = lib.bz_brute, (self._ptrs, n, int(f), d, o, meta, status, ws, wn, st)
-      elif gar == "aksel":
-        fn, args = lib.bz_aksel, (self._ptrs, n, int(f), _lib.AKSEL_MODES[mode], d, o, meta, ws, wn, st)
-      elif gar == "cge":
-        fn, args = lib.bz_cge, (self._ptrs, n, int(f), d, o, meta, ws, wn, st)
-      else:
-        raise KeyError(f"unknown aggregation rule {gar!r}")
-    self._fn, self._args, self._what = fn, args, "bz_" + gar
+      fn, args = rule.entry(prep.ptrs, d, self.out.data_ptr(), self._meta.data_ptr(), self._ws, prep.stream)
+    self._fn, self._args = fn, args
     self._graph = None
   def graph(self):
     """ Capture the prepared call in a CUDA graph and return `replay`: a callable that launches the
@@ -1000,8 +947,8 @@ class Plan:
         with torch.cuda.graph(graph):
           stream = torch.cuda.current_stream(self.device).cuda_stream      # the capture stream
           code = self._fn(*(self._args[:-1] + (stream,)))
-        if code != 0:
-          _lib.check(code, self._what)
+        if code != 0:                                    # raised after the capture has ended
+          _lib.check(code, self._fn.__name__)
       self._graph = graph
     graph, out = self._graph, self.out
     def replay():
@@ -1015,5 +962,5 @@ class Plan:
       with _on(self.device):           # the launches go to the device that owns the rows
         code = self._fn(*self._args)
     if code != 0:
-      _lib.check(code, self._what)
+      _lib.check(code, self._fn.__name__)
     return self.out

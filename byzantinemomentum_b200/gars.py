@@ -17,9 +17,9 @@ Differences with the reference, all deliberate:
 """
 
 import math
-import weakref
 
 from . import engine
+from .engine import _Memo as _Selection, _rule
 
 __all__ = ["gars", "make_gar", "register", "UserException", "last_selection"]
 
@@ -76,42 +76,11 @@ def _bad_m(gradients, f, m):
 # ---------------------------------------------------------------------------- #
 # Selection bookkeeping for `influence`
 
-class _Selection:
-  """ Last device-side selection.  The entry is valid only for the very tensor OBJECTS it was
-  computed on (held through weak references, compared with `is`, like `engine._CallCache`),
-  at the same addresses and in-place versions: a freed list whose ids / addresses are reused by
-  new tensors can never match, and a dead reference drops the entry. """
-  def __init__(self):
-    self.clear()
-  def clear(self):
-    self.rule = self.params = self.refs = self.state = self.indices = None
-  @staticmethod
-  def _state(gradients):
-    return tuple((g.data_ptr(), g._version) for g in gradients)
-  def store(self, rule, params, gradients, indices):
-    try:
-      refs = tuple(weakref.ref(g) for g in gradients)
-    except TypeError:
-      self.clear()
-      return
-    self.rule, self.params, self.refs, self.state, self.indices = rule, params, refs, self._state(gradients), indices
-  def lookup(self, rule, params, gradients):
-    if self.refs is None or self.rule != rule or self.params != params or len(self.refs) != len(gradients):
-      return None
-    for ref, grad in zip(self.refs, gradients):
-      if ref() is not grad:
-        if ref() is None:
-          self.clear()
-        return None
-    if self._state(gradients) != self.state:
-      return None
-    return self.indices
-
-_last = _Selection()
+_last = _Selection()          # the last device-side selection of a rule with its parameters
 
 def last_selection():
   """ Indices selected by the last distance-based aggregation (host list), or None. """
-  return None if _last.indices is None else _last.indices.tolist()
+  return None if _last.value is None else _last.value.tolist()
 
 def _accepted_ratio(indices, nb_honests, count):
   """ Share of the selected slots held by attack gradients: the reference tests object
@@ -169,11 +138,7 @@ register("meamed", _meamed, _trim_check)
 # ---------------------------------------------------------------------------- #
 # Multi-Krum (aggregators/krum.py)
 
-def _krum_m(n, f, m):
-  return n - f - 2 if m is None else m
-
 def _krum(gradients, f, m=None, **kwargs):
-  m = _krum_m(len(gradients), f, m)
   out, order = engine.krum(gradients, f, m)
   _last.store("krum", (f,), gradients, order)
   return out
@@ -186,11 +151,10 @@ def _krum_bound(n, f, d):
 
 def _krum_influence(honests, attacks, f, m=None, **kwargs):
   gradients = honests + attacks
-  m = _krum_m(len(gradients), f, m)
   order = _last.lookup("krum", (f,), gradients)
   if order is None:
     _, order = engine.krum(gradients, f, m)
-  return _accepted_ratio(order, len(honests), m)
+  return _accepted_ratio(order, len(honests), _rule("krum", len(gradients), f, m).count)
 
 register("krum", _krum, _krum_check, upper_bound=_krum_bound, influence=_krum_influence)
 
@@ -198,7 +162,6 @@ register("krum", _krum, _krum_check, upper_bound=_krum_bound, influence=_krum_in
 # Bulyan over Multi-Krum (aggregators/bulyan.py)
 
 def _bulyan(gradients, f, m=None, **kwargs):
-  m = _krum_m(len(gradients), f, m)
   out, _ = engine.bulyan(gradients, f, m)
   return out
 
@@ -233,13 +196,6 @@ register("brute", _brute, _brute_check, upper_bound=_brute_bound, influence=_bru
 # ---------------------------------------------------------------------------- #
 # aksel (aggregators/aksel.py)
 
-def _aksel_count(n, f, mode):
-  if mode == "mid":
-    return (n + 1) // 2
-  if mode == "n-f":
-    return n - f
-  raise NotImplementedError
-
 def _aksel(gradients, f, mode="mid", **kwargs):
   out, order = engine.aksel(gradients, f, mode)
   _last.store("aksel", (), gradients, order)
@@ -253,7 +209,7 @@ def _aksel_check(gradients, f, mode="mid", **kwargs):
 
 def _aksel_influence(honests, attacks, f, mode="mid", **kwargs):
   gradients = honests + attacks
-  count = _aksel_count(len(gradients), f, mode)
+  count = _rule("aksel", len(gradients), f, mode=mode).count
   order = _last.lookup("aksel", (), gradients)
   if order is None:
     _, order = engine.aksel(gradients, f, mode)

@@ -22,6 +22,7 @@ multi-GPU form of its `aggregate(gradients, f, ...)`.
 phases raise.
 """
 
+import ctypes
 import math
 
 import torch
@@ -33,7 +34,7 @@ from . import engine as _engine
 __all__ = ["aggregate", "aggregate_p2p", "compute_avg_dev_max", "replicate", "apply_update", "shard_bounds", "rows_aligned", "choose_exchange", "PeerExchange", "FusedExchange", "ShardedPlan", "COORDINATE_WISE", "DISTANCE_BASED"]
 
 COORDINATE_WISE = ("average", "median", "trmean", "phocas", "meamed")
-DISTANCE_BASED = ("krum", "bulyan", "brute", "aksel", "cge")
+DISTANCE_BASED = _engine.DISTANCE_BASED
 
 def _gather(part, group):
   """ All-gather one small fp64 block per rank -> [R, *part.shape], rank order. """
@@ -65,9 +66,9 @@ class PeerExchange:
     self.handle = symm_mem.rendezvous(self.buffer, self.group)
     self.peer_base = [int(p) for p in self.handle.buffer_ptrs]
     self.step = 0
-  def slot(self):
-    """ (this rank's slot as a tensor, the R peers' addresses of the same slot) for this step. """
-    off = (self.step % 2) * self.n * self.n
+  def slot(self, step=None):
+    """ (this rank's slot as a tensor, the R peers' addresses of the same slot) for `step` (default: this step). """
+    off = ((self.step if step is None else step) % 2) * self.n * self.n
     mine = self.buffer[off:off + self.n * self.n]
     return mine, [base + off * 8 for base in self.peer_base]
   def publish(self):
@@ -77,12 +78,16 @@ class PeerExchange:
 
 _exchanges = {}
 
-def peer_exchange(n, device, group=None):
+def _registered(registry, kind, n, device, group):
+  """ The exchange of this kind for (n, device, group), set up on first use. """
   key = (n, device.index, id(group))
-  ex = _exchanges.get(key)
+  ex = registry.get(key)
   if ex is None:
-    ex = _exchanges[key] = PeerExchange(n, device, group)
+    ex = registry[key] = kind(n, device, group)
   return ex
+
+def peer_exchange(n, device, group=None):
+  return _registered(_exchanges, PeerExchange, n, device, group)
 
 class FusedExchange:
   """ Symmetric buffer for the exchange that runs INSIDE the distance pass (`bz_krum_peers`,
@@ -110,7 +115,6 @@ class FusedExchange:
     self.epoch = 0
   def tables(self, slot):
     """ (ctypes array of the R block pointers, ctypes array of the R flag-array pointers) of a slot. """
-    import ctypes
     block = slot * self.n * self.n * 8
     flags = 2 * self.n * self.n * 8 + slot * self.FLAG_WORDS * 4
     return ((ctypes.c_void_p * self.world)(*[b + block for b in self.peer_base]),
@@ -119,11 +123,7 @@ class FusedExchange:
 _fused = {}
 
 def fused_exchange(n, device, group=None):
-  key = (n, device.index, id(group))
-  ex = _fused.get(key)
-  if ex is None:
-    ex = _fused[key] = FusedExchange(n, device, group)
-  return ex
+  return _registered(_fused, FusedExchange, n, device, group)
 
 def rows_aligned(rows):
   """ Whether the ring kernel takes these rows: every non-empty row 16-byte aligned (an empty shard
@@ -167,44 +167,37 @@ def choose_exchange(gar, exchange, aligned, symmetric, group=None):
     raise ValueError("the p2p exchange needs symmetric memory on every rank")
   return exchange
 
+def _phases(be, gar, gradients, f, m, mode, group, p2p):
+  """ (this rank's shard of the result, the selection) of a distance-based rule.  Phase A computes
+  this rank's partial block; the R blocks are all-gathered into [R, ...] in rank order, or (`p2p`)
+  written into this rank's slot of the PeerExchange and read in place by phase B, which derives the
+  selection; phase C reduces the local shard with it.  Phase B is the backend's
+  `<select>_select(blocks, n, *select_params)` or `<select>_select_peers(peers, n, *select_params, device)`. """
+  n = len(gradients)
+  rule = _engine._rule(gar, n, f, m, mode)
+  center = be.median(gradients) if rule.center else None           # coordinate-wise: local
+  into = {}
+  if p2p:
+    ex = peer_exchange(n, gradients[0].device, group)
+    mine, peers = ex.slot()
+    into = dict(out=mine if rule.pair else mine[:n])
+  part = be.pairdist_partial(gradients, **into) if rule.pair else be.rowdist_partial(gradients, center, **into)
+  if p2p:
+    ex.publish()
+    picked = getattr(be, rule.select + "_select_peers")(peers, n, *rule.select_params, part.device)
+  else:
+    picked = getattr(be, rule.select + "_select")(_gather(part, group), n, *rule.select_params)
+  sel, status = picked if rule.status else (picked, None)
+  if gar == "bulyan":
+    return be.bulyan_reduce(gradients, rule.f, rule.m, sel, status), sel
+  return be.average_selected(gradients, sel, rule.count, rule.zero_init, status=status), sel
+
 def aggregate_p2p(gar, gradients, f=None, m=None, mode="mid", group=None, return_selection=False):
   """ `aggregate` for the distance-based rules with the exchange fused into the selection kernel
   (peer memory over NVLink, see PeerExchange).  CUDA engine only. """
-  be = _engine
-  n = len(gradients)
   if gar in COORDINATE_WISE:
     return aggregate(gar, gradients, f=f, m=m, mode=mode, group=group, return_selection=return_selection)
-  device = gradients[0].device
-  ex = peer_exchange(n, device, group)
-  mine, peers = ex.slot()
-  if gar in ("krum", "bulyan", "brute"):
-    be.pairdist_partial_into(gradients, mine)
-    ex.publish()
-    if gar == "krum":
-      m = n - f - 2 if m is None else m
-      sel = be.krum_select_peers(peers, n, f, device)
-      out = be.average_selected(gradients, sel, m)
-    elif gar == "bulyan":
-      m = n - f - 2 if m is None else m
-      sel, status = be.bulyan_select_peers(peers, n, f, m, device)
-      out = be.bulyan_reduce(gradients, f, m, sel, status)
-    else:
-      sel, status = be.brute_select_peers(peers, n, f, device)
-      out = be.average_selected(gradients, sel, n - f, status=status)
-  elif gar == "aksel":
-    count = (n + 1) // 2 if mode == "mid" else n - f
-    center = be.median(gradients)
-    be.rowdist_partial_into(gradients, center, mine[:n])
-    ex.publish()
-    sel = be.rowdist_select_peers(peers, n, False, device)
-    out = be.average_selected(gradients, sel, count)
-  elif gar == "cge":
-    be.rowdist_partial_into(gradients, None, mine[:n])
-    ex.publish()
-    sel = be.rowdist_select_peers(peers, n, True, device)
-    out = be.average_selected(gradients, sel, n - f, zero_init=False)
-  else:
-    raise KeyError(f"unknown aggregation rule {gar!r}")
+  out, sel = _phases(_engine, gar, gradients, f, m, mode, group, True)
   return (out, sel) if return_selection else out
 
 class ShardedPlan:
@@ -231,8 +224,6 @@ class ShardedPlan:
   Both exchanges use the same fixed summation order: bitwise identical selections on every rank.
   Coordinate-wise rules need no exchange and simply wrap `engine.Plan`. """
   def __init__(self, gar, gradients, f=None, m=None, mode="mid", group=None, exchange="auto"):
-    import ctypes
-    from . import _lib
     self.gar, self.group = gar, group
     self.rows = list(gradients)
     n = self.n = len(self.rows)
@@ -244,129 +235,70 @@ class ShardedPlan:
       self.out = self._local.out
       self.exchange = "none"
       return
-    if gar not in DISTANCE_BASED:
-      raise KeyError(f"unknown aggregation rule {gar!r}")
+    rule = _engine._rule(gar, n, f, m, mode)
     self._local = None
-    lib = _lib.lib()
     prep = _engine._prepare_device(self.rows)
     if not all(g.is_contiguous() for g in self.rows):
       raise ValueError("ShardedPlan takes contiguous rows")
     device = self.device = prep.device
-    d = self.d = prep.d
-    self._ptrs = (ctypes.c_void_p * n)(*[g.data_ptr() for g in self.rows])
-    self._stream = prep.stream
-    self._ws = _engine._workspace(device, prep.stream)
-    ws, wn, st = self._ws.data_ptr(), self._ws.numel(), self._stream
-    self.out = torch.empty(d, dtype=torch.float32, device=device)
+    self.d = prep.d
+    ws = self._ws = _engine._workspace(device, prep.stream)
+    self.out = torch.empty(prep.d, dtype=torch.float32, device=device)
     self._meta = torch.empty(n + 1, dtype=torch.int32, device=device)
-    meta, status = self._meta.data_ptr(), self._meta[n:].data_ptr()
-    self.selection = self._meta[:n]
-    o = self.out.data_ptr()
-    pair = gar in ("krum", "bulyan", "brute")
-    width = n * n if pair else n
-    # ---- exchange: one choice for the whole group ------------------------------------------------
-    exchange = choose_exchange(gar, exchange, rows_aligned(self.rows), _symmetric_memory_importable(), group)
-    if exchange == "fused":
-      self._fx = fused_exchange(n, device, group)
-    elif exchange == "p2p":
-      self._ex = peer_exchange(n, device, group)
-    self.exchange = exchange
-    if exchange == "fused":
-      fx = self._fx
-      mm = n - f - 2 if m is None else m
+    meta, status, out = self._meta.data_ptr(), self._meta[n:].data_ptr(), self.out.data_ptr()
+    self.selection = self._meta[:rule.length]
+    if rule.status:
       self.status = self._meta[n:]
-      fn = lib.bz_krum_peers if gar == "krum" else lib.bz_bulyan_peers
-      self._fused_fn = fn
+    exchange = self.exchange = choose_exchange(gar, exchange, rows_aligned(self.rows), _symmetric_memory_importable(), group)
+    if exchange == "fused":
+      fx = self._fx = fused_exchange(n, device, group)
+      self.status = self._meta[n:]                          # krum too: a peer that never signals
+      self._fused_fn = getattr(_lib.lib(), f"bz_{gar}_peers")
       self._fused_tables = [fx.tables(0), fx.tables(1)]
-      self._fused_head = (self._ptrs, n, int(f), int(mm), d, o, meta, status, fx.rank, fx.world)
-      self._fused_tail = (ws, wn, st)
-      self._check = _lib.check
-      self._pre = None
+      self._fused_head = (prep.ptrs, n) + rule.params + (prep.d, out, meta, status, fx.rank, fx.world)
+      self._fused_tail = (ws.data_ptr(), ws.numel(), prep.stream)
       return
+    # aksel: the coordinate-wise median of the local shard is the center of phase A
+    self._median = _engine.Plan("median", self.rows) if rule.center else None
+    center = None if self._median is None else self._median.out.data_ptr()
+    def phases(part, blocks):
+      return _engine._partial_call(prep, rule.pair, center, part, ws), _engine._select_call(rule, blocks, meta, prep.stream)
+    width = n * n if rule.pair else n
     if exchange == "p2p":
-      ex = self._ex
       # two slots -> two prepared argument sets; the step counter of the exchange picks one
-      self._slots = []
-      for slot in range(2):
-        off = slot * n * n
-        mine = ex.buffer[off:off + width]
-        table = (ctypes.c_void_p * self.world)(*[base + off * 8 for base in ex.peer_base])
-        self._slots.append((mine, table))
+      self._ex = peer_exchange(n, device, group)
+      self._ab = [phases(mine.data_ptr(), peers) for mine, peers in map(self._ex.slot, range(2))]
     else:
       self._part = torch.empty(width, dtype=torch.float64, device=device)
       self._gathered = torch.empty((self.world, width), dtype=torch.float64, device=device)
-    # ---- phases ---------------------------------------------------------------------------------
-    if gar == "aksel":
-      self._center = torch.empty(d, dtype=torch.float32, device=device)
-      self._pre = (lib.bz_median, (self._ptrs, n, d, self._center.data_ptr(), st))
-      center = self._center.data_ptr()
-    else:
-      self._pre = None
-      center = None
-    def phase_a(part_ptr):
-      if pair:
-        return lib.bz_pairdist_partial, (self._ptrs, n, d, part_ptr, ws, wn, st)
-      return lib.bz_rowdist_partial, (self._ptrs, n, center, d, part_ptr, ws, wn, st)
-    def phase_b(parts_ptr, peers):
-      R = self.world
-      if gar == "krum":
-        return (lib.bz_krum_select_peers if peers else lib.bz_krum_select), (parts_ptr, R, n, int(f), meta, st)
-      if gar == "bulyan":
-        return (lib.bz_bulyan_select_peers if peers else lib.bz_bulyan_select), (parts_ptr, R, n, int(f), int(mm), meta, status, st)
-      if gar == "brute":
-        return (lib.bz_brute_select_peers if peers else lib.bz_brute_select), (parts_ptr, R, n, int(f), meta, status, st)
-      return (lib.bz_rowdist_select_peers if peers else lib.bz_rowdist_select), (parts_ptr, R, n, 1 if gar == "cge" else 0, meta, st)
-    mm = (n - f - 2 if m is None else m) if gar in ("krum", "bulyan") else None
-    if gar == "krum":
-      self._c = (lib.bz_average_selected, (self._ptrs, n, meta, int(mm), 1, float(mm), None, d, o, st))
-    elif gar == "bulyan":
-      self.status = self._meta[n:]
-      self._c = (lib.bz_bulyan_reduce, (self._ptrs, n, int(f), int(mm), meta, status, d, o, st))
-    elif gar == "brute":
-      self.status = self._meta[n:]
-      self.selection = self._meta[:n - int(f)]
-      self._c = (lib.bz_average_selected, (self._ptrs, n, meta, n - int(f), 1, float(n - int(f)), status, d, o, st))
-    elif gar == "aksel":
-      if mode not in _lib.AKSEL_MODES:
-        raise NotImplementedError(mode)
-      count = (n + 1) // 2 if mode == "mid" else n - int(f)
-      self._c = (lib.bz_average_selected, (self._ptrs, n, meta, count, 1, float(count), None, d, o, st))
-    else:  # cge
-      count = n - int(f)
-      self._c = (lib.bz_average_selected, (self._ptrs, n, meta, count, 0, float(count), None, d, o, st))
-    if exchange == "p2p":
-      self._ab = [(phase_a(mine.data_ptr()), phase_b(table, True)) for mine, table in self._slots]
-    else:
-      self._ab = [(phase_a(self._part.data_ptr()), phase_b(self._gathered.data_ptr(), False))]
-    self._check = _lib.check
+      self._ab = [phases(self._part.data_ptr(), self._gathered)]
+    self._c = _engine._reduce_call(prep, rule, meta, status if rule.status else None, out)
   def __call__(self):
     if self._local is not None:
       return self._local()
-    check = self._check
-    if self.exchange == "fused":
-      fx = self._fx
-      fx.epoch += 1
-      blocks, flags = self._fused_tables[fx.epoch % 2]
-      with _engine._on(self.device):
-        check(self._fused_fn(*self._fused_head, blocks, flags, fx.epoch, *self._fused_tail), "bz_*_peers")
-      return self.out
+    call = _engine._call
     with _engine._on(self.device):
-      if self._pre is not None:
-        check(self._pre[0](*self._pre[1]), "bz_median")
+      if self.exchange == "fused":
+        fx = self._fx
+        fx.epoch += 1
+        call(self._fused_fn, self._fused_head + self._fused_tables[fx.epoch % 2] + (fx.epoch,) + self._fused_tail)
+        return self.out
+      if self._median is not None:
+        self._median()
       if self.exchange == "p2p":
         ex = self._ex
-        (fa, aa), (fb, ab) = self._ab[ex.step % 2]
-        check(fa(*aa), "phase A")
+        a, b = self._ab[ex.step % 2]
+        call(*a)
         ex.publish()
       else:
-        (fa, aa), (fb, ab) = self._ab[0]
-        check(fa(*aa), "phase A")
+        a, b = self._ab[0]
+        call(*a)
         if self.world > 1:
           dist.all_gather_into_tensor(self._gathered, self._part, group=self.group)
         else:
           self._gathered.copy_(self._part.unsqueeze(0))
-      check(fb(*ab), "phase B")
-      check(self._c[0](*self._c[1]), "phase C")
+      call(*b)
+      call(*self._c)
     return self.out
 
 def aggregate(gar, gradients, f=None, m=None, mode="mid", group=None, backend=None, return_selection=False):
@@ -383,44 +315,10 @@ def aggregate(gar, gradients, f=None, m=None, mode="mid", group=None, backend=No
     This rank's shard of the aggregated gradient (and the device-side selection if asked)
   """
   be = backend or _engine
-  n = len(gradients)
   if gar in COORDINATE_WISE:
-    if gar == "average":
-      out = be.average(gradients)
-    elif gar == "median":
-      out = be.median(gradients)
-    else:
-      out = getattr(be, gar)(gradients, f)
+    out = getattr(be, gar)(gradients) if gar in ("average", "median") else getattr(be, gar)(gradients, f)
     return (out, None) if return_selection else out
-  if gar == "krum":
-    m = n - f - 2 if m is None else m
-    parts = _gather(be.pairdist_partial(gradients), group)
-    order = be.krum_select(parts, n, f)
-    out = be.average_selected(gradients, order, m)
-    sel = order
-  elif gar == "bulyan":
-    m = n - f - 2 if m is None else m
-    parts = _gather(be.pairdist_partial(gradients), group)
-    order, status = be.bulyan_select(parts, n, f, m)
-    out = be.bulyan_reduce(gradients, f, m, order, status)
-    sel = order
-  elif gar == "brute":
-    parts = _gather(be.pairdist_partial(gradients), group)
-    sel, status = be.brute_select(parts, n, f)
-    out = be.average_selected(gradients, sel, n - f, status=status)
-  elif gar == "aksel":
-    count = (n + 1) // 2 if mode == "mid" else n - f
-    center = be.median(gradients)                                   # coordinate-wise: local
-    parts = _gather(be.rowdist_partial(gradients, center), group)
-    sel = be.rowdist_select(parts, n, False)
-    out = be.average_selected(gradients, sel, count)
-  elif gar == "cge":
-    count = n - f
-    parts = _gather(be.rowdist_partial(gradients, None), group)
-    sel = be.rowdist_select(parts, n, True)
-    out = be.average_selected(gradients, sel, count, zero_init=False)
-  else:
-    raise KeyError(f"unknown aggregation rule {gar!r}")
+  out, sel = _phases(be, gar, gradients, f, m, mode, group, False)
   return (out, sel) if return_selection else out
 
 def compute_avg_dev_max(samples, group=None, backend=None):

@@ -3,6 +3,4 @@
 
 def aggregate(gradients, f, m=None):
   from byzantinemomentum_b200 import engine
-  if m is None:
-    m = len(gradients) - f - 2
-  return engine.krum(gradients, f, m)[0]
+  return engine.krum(gradients, f, engine._rule("krum", len(gradients), f, m).m)[0]

@@ -49,19 +49,20 @@ def test_forced_host_path_is_used_without_sampling():
   finally:
     engine.forced_host_path = None
 
-def test_study_memo_matches_only_the_same_unmodified_tensor_objects():
-  memo = engine._StudyMemo()
+def test_study_metrics_memo_matches_only_the_same_unmodified_tensor_objects(monkeypatch):
+  memo = engine._Memo()
+  monkeypatch.setattr(engine, "_study_memo", memo)
   rows = [torch.arange(4.), torch.ones(4)]
   result = (torch.full((4,), 2.), 1., 2., 3.)
-  assert memo.lookup(rows) is None
-  memo.store(rows, result)
-  hit = memo.lookup(list(rows))                      # another list object, the same tensors
+  assert memo.lookup("avg_dev_max", (), rows) is None
+  memo.store("avg_dev_max", (), rows, result)
+  hit = engine.compute_avg_dev_max(list(rows))       # another list object, the same tensors: served by the memo
   assert hit is not None and torch.equal(hit[0], result[0]) and hit[1:] == (1., 2., 3.)
   assert hit[0] is not result[0]                     # callers own the average they get
-  assert memo.lookup(rows[:1]) is None
-  assert memo.lookup([rows[0], torch.ones(4)]) is None          # equal values, another object
+  assert memo.lookup("avg_dev_max", (), rows[:1]) is None
+  assert memo.lookup("avg_dev_max", (), [rows[0], torch.ones(4)]) is None          # equal values, another object
   rows[1].add_(1.)                                   # in-place update bumps the version
-  assert memo.lookup(rows) is None
+  assert memo.lookup("avg_dev_max", (), rows) is None
 
 def test_selection_cache_never_serves_a_recycled_identity():
   sel = gars._Selection()
