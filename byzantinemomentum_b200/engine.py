@@ -25,6 +25,7 @@ from . import _lib, hostmem
 __all__ = ["average", "median", "trmean", "phocas", "meamed", "krum", "bulyan", "brute", "aksel", "cge",
            "pairdist_partial", "rowdist_partial", "select", "krum_select", "bulyan_select", "brute_select",
            "rowdist_select", "average_selected", "bulyan_reduce", "avg_dev_max_async", "compute_avg_dev_max", "rowdots_async", "study_step",
+           "StudyPartials", "study_partials", "study_finish",
            "config", "Plan", "pair_cache_stats", "GradientStack", "host_path_report"]
 
 class _Config:
@@ -614,6 +615,23 @@ def _compute_avg_dev_max(samples, n):
   avg, stats = avg_dev_max_async(samples)
   return _study_tuple(avg, stats.tolist(), n)                 # the only synchronisation
 
+def _merge_ranks(parts, maxima):
+  """ One host vector from the R ranks' fp64 partial vectors `parts` (rank order, equal lengths) —
+  the rule of every sharded study scalar.  Entry k is ((p0[k] + p1[k]) + p2[k]) + ..., started from
+  rank 0's value rather than from 0.0, so that one rank's vector comes back unchanged (0.0 + (-0.0)
+  would turn a negative-zero dot product into +0.0); at the indices in `maxima` it is the largest
+  value instead, NaN when any rank has a NaN (torch's max propagates it, Python's max() may drop it). """
+  total = list(parts[0])
+  for part in parts[1:]:
+    for k, value in enumerate(part):
+      if k not in maxima:
+        total[k] += value
+      elif math.isnan(value) or math.isnan(total[k]):
+        total[k] = math.nan
+      elif value > total[k]:
+        total[k] = value
+  return total
+
 def fp32_overflow(sum_sq):
   """ +inf where an fp64 sum of squares rounds to +inf in fp32 (where ATen's fp32 `norm()` / `dot()`
   accumulator overflows), else the sum itself. """
@@ -647,36 +665,74 @@ def rowdots_async(center, rows):
   _run(prep.device, _lib.lib().bz_rowdots, (prep.ptrs, prep.n, center.data_ptr(), prep.d, out.data_ptr(), ws.data_ptr(), ws.numel(), prep.stream))
   return out
 
-def study_step(grad_sampleds, grad_honests, grad_attacks, grad_defense, pasts, momentum):
-  """ Everything attack.py:846-866 computes for one line of the study file, on the device:
-    * the three `tools.compute_avg_dev_max` calls (K6, one pass each; a repeated list is computed once),
-    * the norm and the largest |coordinate| of the defense gradient,
-    * the six cosines between the sampled / honest / attack averages and the defense gradient,
-    * the cosine with the last past gradient and the curvature sum over all past gradients
-  with THREE passes of `bz_rowdots` (one vector against many) instead of 7 + len(pasts) `torch.dot(...).item()`
-  and ONE device->host read for the whole step (the reference: 9 + len(samples) + len(pasts) `.item()`s).
+class StudyPartials:
+  """ One shard's share of attack.py:846-866 (`study_partials`): the shard of the three averages
+  (`attack_avg` is None without attack gradients), the list lengths `counts` = (ns, nh, na), the norms of
+  the past gradients, and `vector`: ONE fp64 device vector of sums and maxima over the shard's columns,
+      [0, 2 + ns)             K6 stats of the sampled gradients: ||avg||^2, max |avg|, ||g_i - avg||^2 per row
+      then 2 + nh             the same for the honest gradients
+      then 2 + na (na > 0)    the same for the attack gradients
+      then 2 + a + P          <s_avg, x> for x in (h_avg, [a_avg], defense, the P pasts)   (a = 1 if na > 0 else 0)
+      then a + 1              <h_avg, x> for x in ([a_avg], defense)
+      then a + 1              <defense, x> for x in ([a_avg], defense)
+      last                    max |defense| (0 for an empty shard: |x| >= 0, so 0 is no value)
+  The length depends on (ns, nh, na, P) only, so every rank of a d-sharded step has the same layout.  The
+  entries at `maxima()` merge across shards by max, every other one by addition. """
+  __slots__ = ("sampled_avg", "honest_avg", "attack_avg", "vector", "counts", "past_norms")
+  def maxima(self):
+    ns, nh, na = self.counts
+    return (1, 3 + ns) + ((5 + ns + nh,) if na else ()) + (self.vector.numel() - 1,)
+
+def study_partials(grad_sampleds, grad_honests, grad_attacks, grad_defense, pasts, backend=None):
+  """ The device half of `study_step` on one shard of the columns (the whole vectors on one GPU):
+  K6 over each list (the honest pass is skipped when `grad_honests` holds the very same tensors as
+  `grad_sampleds`, attack.py:808 without momentum placement; none without attack gradients), three
+  `bz_rowdots` passes and the defense's max |x|, all into one device vector.  No sync.
   Args:
-    grad_sampleds, grad_honests, grad_attacks  Lists of CUDA gradients (the attack list may be empty)
-    grad_defense  The aggregated gradient
-    pasts         Iterable of (gradient, norm) of the past sampled averages, most recent first
-    momentum      args.momentum
+    grad_sampleds, grad_honests, grad_attacks, grad_defense  As `study_step`, or this rank's columns of them
+    pasts    Iterable of (gradient or its shard, norm of the WHOLE gradient), most recent first
+    backend  Provider of `avg_dev_max_async` and `rowdots_async` (default: this module)
   Returns:
-    dict with the reference's variable names (attack.py:846-866) """
-  nan = math.nan
+    StudyPartials """
+  avg_dev_max = avg_dev_max_async if backend is None else backend.avg_dev_max_async
+  rowdots = rowdots_async if backend is None else backend.rowdots_async
   pasts = list(pasts)
   ns, nh, na = len(grad_sampleds), len(grad_honests), len(grad_attacks)
-  s_avg, s_stats = avg_dev_max_async(grad_sampleds)
-  same = nh == ns and all(a is b for a, b in zip(grad_sampleds, grad_honests))      # attack.py:808 without momentum placement
-  h_avg, h_stats = (s_avg, s_stats) if same else avg_dev_max_async(grad_honests)
+  s_avg, s_stats = avg_dev_max(grad_sampleds)
+  same = nh == ns and all(a is b for a, b in zip(grad_sampleds, grad_honests))
+  h_avg, h_stats = (s_avg, s_stats) if same else avg_dev_max(grad_honests)
   have_attack = na > 0
-  a_avg, a_stats = avg_dev_max_async(grad_attacks) if have_attack else (None, s_stats[:0])
-  # one vector against many, three times; every result lands in one device vector read once
+  a_avg, a_stats = avg_dev_max(grad_attacks) if have_attack else (None, s_stats[:0])
+  # one vector against many, three times; every result lands in one device vector
   first = [h_avg] + ([a_avg] if have_attack else []) + [grad_defense] + [g for g, _ in pasts]
   second = ([a_avg] if have_attack else []) + [grad_defense]
-  host = torch.cat([s_stats, h_stats, a_stats, rowdots_async(s_avg, first), rowdots_async(h_avg, second),
-                    rowdots_async(grad_defense, second), grad_defense.abs().max().double().reshape(1)]).tolist()    # the only synchronisation
+  d_max = grad_defense.abs().max().double().reshape(1) if grad_defense.numel() else s_stats.new_zeros(1)
+  out = StudyPartials()
+  out.sampled_avg, out.honest_avg, out.attack_avg = s_avg, h_avg, a_avg
+  out.vector = torch.cat([s_stats, h_stats, a_stats, rowdots(s_avg, first), rowdots(h_avg, second), rowdots(grad_defense, second), d_max])
+  out.counts = (ns, nh, na)
+  out.past_norms = [norm for _, norm in pasts]
+  return out
+
+def study_finish(partials, parts, momentum):
+  """ The host half of `study_step`: the dict of attack.py:846-866 from the R shards' partial vectors.
+  Every additive entry is summed across the shards in rank order in fp64, the maxima are merged
+  (`_merge_ranks`), and only then come the fp32 overflow rule, the norms and the fp32 divisions — so
+  every rank that holds the same R vectors returns bitwise the same scalars, and one shard gives
+  exactly the one-GPU result.
+  Args:
+    partials  This shard's StudyPartials (its averages, list lengths and past norms)
+    parts     R host sequences of floats, the shards' `vector`s in rank order (one: [vector.tolist()])
+    momentum  args.momentum
+  Returns:
+    dict with the reference's variable names; the averages are this shard's """
+  nan = math.nan
+  ns, nh, na = partials.counts
+  past_norms = partials.past_norms
+  host = _merge_ranks(parts, partials.maxima())
   _, s_norm, s_dev, s_max = _study_tuple(None, host[:2 + ns], ns)
   _, h_norm, h_dev, h_max = _study_tuple(None, host[2 + ns:4 + ns + nh], nh)
+  have_attack = na > 0
   if have_attack:
     _, a_norm, a_dev, a_max = _study_tuple(None, host[4 + ns + nh:6 + ns + nh + na], na)
     dots = host[6 + ns + nh + na:]
@@ -687,7 +743,7 @@ def study_step(grad_sampleds, grad_honests, grad_attacks, grad_defense, pasts, m
   sh = dots[k]; k += 1
   sa = dots[k] if have_attack else nan; k += 1 if have_attack else 0
   sd = dots[k]; k += 1
-  past_dots = dots[k:k + len(pasts)]; k += len(pasts)
+  past_dots = dots[k:k + len(past_norms)]; k += len(past_norms)
   ha = dots[k] if have_attack else nan; k += 1 if have_attack else 0
   hd = dots[k]; k += 1
   ad = dots[k] if have_attack else nan; k += 1 if have_attack else 0
@@ -701,20 +757,39 @@ def study_step(grad_sampleds, grad_honests, grad_attacks, grad_defense, pasts, m
     except ZeroDivisionError:
       return nan if a == 0 or math.isnan(a) else math.copysign(math.inf, a) * math.copysign(1., b)
   cos = lambda dot, na, nb: div(div(f32(dot), na), nb)
-  out = dict(sampled_grad_avg=s_avg, sampled_norm_avg=s_norm, sampled_norm_dev=s_dev, sampled_norm_max=s_max,
-             honest_grad_avg=h_avg, honest_norm_avg=h_norm, honest_norm_dev=h_dev, honest_norm_max=h_max,
-             attack_grad_avg=a_avg, attack_norm_avg=a_norm, attack_norm_dev=a_dev, attack_norm_max=a_max,
+  out = dict(sampled_grad_avg=partials.sampled_avg, sampled_norm_avg=s_norm, sampled_norm_dev=s_dev, sampled_norm_max=s_max,
+             honest_grad_avg=partials.honest_avg, honest_norm_avg=h_norm, honest_norm_dev=h_dev, honest_norm_max=h_max,
+             attack_grad_avg=partials.attack_avg, attack_norm_avg=a_norm, attack_norm_dev=a_dev, attack_norm_max=a_max,
              defense_norm_avg=d_norm, defense_norm_max=f32(d_max),
              cosin_splhon=cos(sh, s_norm, h_norm), cosin_splatt=cos(sa, s_norm, a_norm) if have_attack else nan,
              cosin_spldef=cos(sd, s_norm, d_norm), cosin_honatt=cos(ha, h_norm, a_norm) if have_attack else nan,
              cosin_hondef=cos(hd, h_norm, d_norm), cosin_attdef=cos(ad, a_norm, d_norm) if have_attack else nan)
-  if pasts:
-    out["cosin_sampled"] = cos(past_dots[0], s_norm, pasts[0][1])
+  if past_norms:
+    out["cosin_sampled"] = cos(past_dots[0], s_norm, past_norms[0])
     out["curv_sampled"] = momentum * sum((momentum ** i) * f32(dot) for i, dot in enumerate(past_dots))
   else:
     out["cosin_sampled"] = nan
     out["curv_sampled"] = nan
   return out
+
+def study_step(grad_sampleds, grad_honests, grad_attacks, grad_defense, pasts, momentum):
+  """ Everything attack.py:846-866 computes for one line of the study file, on the device:
+    * the three `tools.compute_avg_dev_max` calls (K6, one pass each; a repeated list is computed once),
+    * the norm and the largest |coordinate| of the defense gradient,
+    * the six cosines between the sampled / honest / attack averages and the defense gradient,
+    * the cosine with the last past gradient and the curvature sum over all past gradients
+  with THREE passes of `bz_rowdots` (one vector against many) instead of 7 + len(pasts) `torch.dot(...).item()`
+  and ONE device->host read for the whole step (the reference: 9 + len(samples) + len(pasts) `.item()`s).
+  `study_partials` + `study_finish` over one shard; `sharded.study_step` is the d-sharded form.
+  Args:
+    grad_sampleds, grad_honests, grad_attacks  Lists of CUDA gradients (the attack list may be empty)
+    grad_defense  The aggregated gradient
+    pasts         Iterable of (gradient, norm) of the past sampled averages, most recent first
+    momentum      args.momentum
+  Returns:
+    dict with the reference's variable names (attack.py:846-866) """
+  partials = study_partials(grad_sampleds, grad_honests, grad_attacks, grad_defense, pasts)
+  return study_finish(partials, [partials.vector.tolist()], momentum)            # the only synchronisation
 
 # ---------------------------------------------------------------------------- #
 # Phases of the d-sharded multi-GPU path (device tensors only)

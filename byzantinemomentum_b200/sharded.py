@@ -31,7 +31,7 @@ import torch.distributed as dist
 from . import _lib
 from . import engine as _engine
 
-__all__ = ["aggregate", "aggregate_p2p", "compute_avg_dev_max", "replicate", "apply_update", "shard_bounds", "rows_aligned", "choose_exchange", "PeerExchange", "FusedExchange", "ShardedPlan", "COORDINATE_WISE", "DISTANCE_BASED"]
+__all__ = ["aggregate", "aggregate_p2p", "compute_avg_dev_max", "study_step", "replicate", "apply_update", "shard_bounds", "rows_aligned", "choose_exchange", "PeerExchange", "FusedExchange", "ShardedPlan", "COORDINATE_WISE", "DISTANCE_BASED"]
 
 COORDINATE_WISE = ("average", "median", "trmean", "phocas", "meamed")
 DISTANCE_BASED = _engine.DISTANCE_BASED
@@ -337,23 +337,30 @@ def compute_avg_dev_max(samples, group=None, backend=None):
     return None, math.nan, math.nan, math.nan
   avg, stats = be.avg_dev_max_async(samples)
   gathered = _gather(stats, group).tolist()            # [R][2 + n]; the only synchronisation
-  norm_sq, norm_max, norm_var = 0., 0., 0.
-  for rank_stats in gathered:                          # rank order
-    norm_sq += rank_stats[0]
-    if math.isnan(rank_stats[1]) or math.isnan(norm_max):
-      norm_max = math.nan                              # torch's max propagates a NaN; Python's max() may drop it
-    elif rank_stats[1] > norm_max:
-      norm_max = rank_stats[1]
-  if n >= 2:
-    for i in range(n):                                 # sample order, ranks inside
-      dev = 0.
-      for rank_stats in gathered:
-        dev += rank_stats[2 + i]
-      norm_var += _engine.fp32_overflow(dev)           # the reference's fp32 dot(): +inf past FLT_MAX
-    norm_dev = math.sqrt(norm_var / (n - 1))
-  else:
-    norm_dev = math.nan
-  return avg, _engine.fp32_norm(norm_sq), norm_dev, norm_max          # an fp32 norm, as on one GPU
+  return _engine._study_tuple(avg, _engine._merge_ranks(gathered, (1,)), n)      # fp32 overflow rule after the sums
+
+def study_step(grad_sampleds, grad_honests, grad_attacks, grad_defense, pasts, momentum, group=None, backend=None):
+  """ `engine.study_step` (attack.py:846-866) over d-sharded vectors: every rank passes its columns
+  and gets its shards of the three averages plus the GLOBAL scalars, bitwise the same on every rank.
+  One `engine.study_partials` pass over the local shard, then ONE all-gather of its fp64 vector
+  (14 + ns + nh + na + P doubles with P past gradients, 9 + ns + nh + P without attack gradients: the
+  same length on every rank), then `engine.study_finish`: sums added in rank order, maxima merged, and
+  only then the fp32 overflow rule, the norms and the fp32 divisions.  A rank whose shard is empty
+  (d < R) still joins.
+  Against one GPU the averages are bit-identical per coordinate; the scalars differ only by the
+  order of the fp64 additions (the R per-rank blocks added in rank order).
+  Args:
+    grad_sampleds, grad_honests, grad_attacks, grad_defense  This rank's columns of them
+    pasts     Iterable of (this rank's shard of a past sampled average, its GLOBAL norm), most recent
+              first: (`sampled_grad_avg`, `sampled_norm_avg`) of an earlier call
+    momentum  args.momentum
+    group     Process group (default: the world)
+    backend   Provider of `avg_dev_max_async` and `rowdots_async` (default: the CUDA engine)
+  Returns:
+    dict with the reference's variable names
+  """
+  partials = _engine.study_partials(grad_sampleds, grad_honests, grad_attacks, grad_defense, pasts, backend=backend)
+  return _engine.study_finish(partials, _gather(partials.vector, group).tolist(), momentum)    # the only synchronisation
 
 def replicate(shard, group=None):
   """ All-gather the ranks' output shards into the full aggregated gradient on every rank

@@ -240,7 +240,8 @@ BZ_API int bz_avg_dev_max(const float* const* rows, int n, int64_t d, float* avg
 /* ---- Dot products of the study step (attack.py:854-866: 6 cosines + up to 20 dot products with past
  * gradients, each a `torch.dot(...).item()` with its own pass and host sync): out[i] = sum_k rows[i][k] *
  * center[k] for all n rows in ONE pass (fp32 products accumulated in fp32 over <= 32 terms, then fp64;
- * deterministic).  out: device double[n].  The caller reads the results with one copy. */
+ * deterministic).  out: device double[n].  The caller reads the results with one copy.  d = 0 writes
+ * zeros (center may then be NULL). */
 BZ_API int bz_rowdots(const float* const* rows, int n, const float* center, int64_t d, double* out,
                       void* ws, size_t ws_bytes, void* stream);
 
