@@ -1,5 +1,5 @@
 # coding: utf-8
-"""ctypes binding of `libbyzagg.so` (C ABI: `include/byzagg.h`).
+"""ctypes binding of `libbyzagg.so` (C ABI: `include/byzagg.h` and `include/byzagg_shards.h`).
 
 The library is loaded lazily, on the first call that needs it, and the load FAILS LOUDLY:
 there is no CPU or PyTorch fallback anywhere in this package.  Build it in-tree with
@@ -77,6 +77,12 @@ SIGNATURES = {
   "bz_bulyan_reduce": (_i, [_c_rows, _i, _i, _i, _vp, _vp, _i64, _vp, _vp]),
 }
 
+# the same for include/byzagg_shards.h (entry points of a d-sharded trainer besides the rules)
+SHARD_SIGNATURES = {
+  "bz_gradient_scatter": (_i, [_vp, _i64, _dbl, _i, _c_rows, _vp, _sz, _vp]),
+  "bz_gradient_momentum": (_i, [_c_rows, _i, _i64, _i, _c_rows, _vp, _dbl, _dbl, _c_rows, _vp]),
+}
+
 _lock = threading.Lock()
 _lib = None
 
@@ -95,7 +101,7 @@ def lib():
         handle = ctypes.CDLL(str(path))
       except OSError as err:
         raise LibraryError(f"unable to load {path}: {err}") from err
-      for name, (restype, argtypes) in SIGNATURES.items():
+      for name, (restype, argtypes) in list(SIGNATURES.items()) + list(SHARD_SIGNATURES.items()):
         try:
           fn = getattr(handle, name)
         except AttributeError as err:

@@ -26,7 +26,7 @@ __all__ = ["average", "median", "trmean", "phocas", "meamed", "krum", "bulyan", 
            "pairdist_partial", "rowdist_partial", "select", "krum_select", "bulyan_select", "brute_select",
            "rowdist_select", "average_selected", "bulyan_reduce", "avg_dev_max_async", "compute_avg_dev_max", "rowdots_async", "study_step",
            "StudyPartials", "study_partials", "study_finish",
-           "config", "Plan", "pair_cache_stats", "GradientStack", "host_path_report"]
+           "config", "Plan", "pair_cache_stats", "GradientStack", "gradient_scatter", "momentum_rows", "host_path_report"]
 
 class _Config:
   """ strict_status: after brute / bulyan, read the device status word (one 4-byte D2H copy,
@@ -966,6 +966,70 @@ class GradientStack:
   def honest(self, count=None):
     buf = self._honest_buffer()
     return [buf[i, :self.d] for i in range(self.n if count is None else count)]
+
+def gradient_scatter(grad, clip, slots):
+  """ `bz_gradient_scatter`: clip `grad` as `GradientStack.push` does (clip None or <= 0: no clipping)
+  and write columns [lo_r, hi_r) of the result into `slots[r]` (`sharded.shard_bounds` over R =
+  len(slots) ranks), in one pass.  The slots are contiguous fp32 CUDA vectors of hi_r - lo_r
+  elements, 16-byte aligned, addressable from `grad`'s GPU: its own memory or another GPU's mapped into
+  it (symmetric memory).  Their version counters are not bumped here, that is for the rank that owns
+  them to do. """
+  d, R = grad.numel(), len(slots)
+  if not 1 <= R <= _lib.MAX_PEERS:
+    raise ValueError(f"{R} slots, expected 1..{_lib.MAX_PEERS}")
+  per = (d + R - 1) // R
+  ptrs = []
+  for r, slot in enumerate(slots):
+    lo = min(d, r * per)
+    width = min(d, lo + per) - lo
+    if slot.dtype != torch.float32 or slot.numel() != width or not slot.is_contiguous() or slot.device.type != "cuda":
+      raise ValueError(f"slot {r} must be a contiguous float32 CUDA vector of the {width} columns of rank {r}")
+    ptrs.append(slot.data_ptr() if slot.numel() else None)
+  if grad.dtype != torch.float32 or grad.dim() != 1 or not grad.is_contiguous() or grad.device.type != "cuda":
+    raise ValueError("grad must be a contiguous float32 CUDA vector")
+  stream = torch.cuda.current_stream(grad.device).cuda_stream
+  ws = _workspace(grad.device, stream)
+  _run(grad.device, _lib.lib().bz_gradient_scatter, (grad.data_ptr(), d, float(clip) if clip is not None else 0., R,
+                                                     (ctypes.c_void_p * R)(*ptrs), ws.data_ptr(), ws.numel(), stream))
+
+def momentum_rows(rows, mu, dampening, momentums=None, server=None, honests=None):
+  """ The momentum placement of attack.py:799-810 on rows that are already clipped, one launch per 64
+  rows (`bz_gradient_momentum`): the arithmetic `GradientStack.push` applies after the clip, so the
+  results have the same bits.
+    momentums given       worker side: momentums[k] <- momentums[k] * mu + (1 - dampening) * rows[k],
+                          in place (:802); distinct vectors, one per row
+    server and honests    server side: honests[k] <- rows[k] * (1 - dampening) + mu * server (:807)
+  Every vector is a contiguous fp32 CUDA vector of the rows' length, all on one GPU; rows of zero
+  columns (an empty shard) are a no-op.  Bumps the version counter of what it writes.
+  Returns the honest rows (`momentums` on the worker side). """
+  rows = list(rows)
+  worker = momentums is not None
+  if worker == (server is not None or honests is not None):
+    raise ValueError("give either momentums (worker side) or server and honests (server side)")
+  if not worker and (server is None or honests is None):
+    raise ValueError("the server side needs both server and honests")
+  outs = list(momentums if worker else honests)
+  if len(outs) != len(rows) or not rows:
+    raise ValueError(f"{len(outs)} output vectors for {len(rows)} rows")
+  shape, device = rows[0].shape, rows[0].device
+  for what, vs in (("row", rows), ("momentum" if worker else "honest", outs), ("server", [] if worker else [server])):
+    for v in vs:
+      if v.dtype != torch.float32 or v.dim() != 1 or v.shape != shape or not v.is_contiguous() or v.device != device or device.type != "cuda":
+        raise ValueError(f"every {what} must be a contiguous float32 CUDA vector like the first row")
+  if shape[0] == 0:
+    return outs                                    # an empty tensor's address may be 0: nothing to launch
+  lib, table = _lib.lib(), ctypes.c_void_p * _lib.MAX_N
+  stream = torch.cuda.current_stream(device).cuda_stream
+  for k in range(0, len(rows), _lib.MAX_N):
+    part = slice(k, k + _lib.MAX_N)
+    ptrs = table(*[r.data_ptr() for r in rows[part]])
+    written = table(*[o.data_ptr() for o in outs[part]])
+    _run(device, lib.bz_gradient_momentum, (ptrs, len(rows[part]), shape[0], 1 if worker else 2, written if worker else None,
+                                            None if worker else server.data_ptr(), float(mu), 1. - float(dampening),
+                                            None if worker else written, stream))
+  for o in outs:
+    torch.autograd.graph.increment_version(o)
+  return outs
 
 # ---------------------------------------------------------------------------- #
 # Prepared calls

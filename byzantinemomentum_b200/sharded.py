@@ -31,7 +31,7 @@ import torch.distributed as dist
 from . import _lib
 from . import engine as _engine
 
-__all__ = ["aggregate", "aggregate_p2p", "compute_avg_dev_max", "study_step", "replicate", "apply_update", "shard_bounds", "rows_aligned", "choose_exchange", "PeerExchange", "FusedExchange", "ShardedPlan", "COORDINATE_WISE", "DISTANCE_BASED"]
+__all__ = ["aggregate", "aggregate_p2p", "compute_avg_dev_max", "study_step", "replicate", "apply_update", "shard_bounds", "rows_aligned", "choose_exchange", "PeerExchange", "FusedExchange", "ShardedPlan", "GradientShards", "choose_delivery", "COORDINATE_WISE", "DISTANCE_BASED"]
 
 COORDINATE_WISE = ("average", "median", "trmean", "phocas", "meamed")
 DISTANCE_BASED = _engine.DISTANCE_BASED
@@ -139,6 +139,17 @@ def _symmetric_memory_importable():
 
 EXCHANGES = ("auto", "fused", "p2p", "nccl")
 
+def _agree(facts, group):
+  """ The element-wise minimum over the ranks of `group` of every rank's list of local facts (ints):
+  one all-reduce (MIN), none on a single rank. """
+  world = dist.get_world_size(group) if dist.is_initialized() else 1
+  if world == 1:
+    return list(facts)
+  device = torch.device("cuda", torch.cuda.current_device()) if dist.get_backend(group) == "nccl" else torch.device("cpu")
+  agreed = torch.tensor(facts, dtype=torch.int32, device=device)
+  dist.all_reduce(agreed, op=dist.ReduceOp.MIN, group=group)
+  return agreed.tolist()
+
 def choose_exchange(gar, exchange, aligned, symmetric, group=None):
   """ The exchange of `ShardedPlan`, the same on every rank of `group`.  The two ranks' protocols do
   not mix (different symmetric buffers, flags nobody raises), so the local facts — `aligned`: this
@@ -149,13 +160,7 @@ def choose_exchange(gar, exchange, aligned, symmetric, group=None):
   if exchange not in EXCHANGES:
     raise ValueError(f"unknown exchange {exchange!r}")
   world = dist.get_world_size(group) if dist.is_initialized() else 1
-  facts = [int(bool(aligned)), int(bool(symmetric))]
-  if world > 1:
-    device = torch.device("cuda", torch.cuda.current_device()) if dist.get_backend(group) == "nccl" else torch.device("cpu")
-    agreed = torch.tensor(facts, dtype=torch.int32, device=device)
-    dist.all_reduce(agreed, op=dist.ReduceOp.MIN, group=group)
-    facts = agreed.tolist()
-  aligned, symmetric = bool(facts[0]), bool(facts[1])
+  aligned, symmetric = map(bool, _agree([int(bool(aligned)), int(bool(symmetric))], group))
   fusable = gar in ("krum", "bulyan") and aligned
   if exchange == "auto":
     if world == 1 or world > _lib.MAX_PEERS or not symmetric:
@@ -300,6 +305,170 @@ class ShardedPlan:
       call(*b)
       call(*self._c)
     return self.out
+
+DELIVERIES = ("auto", "p2p", "collective")
+
+def choose_delivery(exchange, symmetric, group=None):
+  """ The exchange of `GradientShards`, the same on every rank of `group`: the local fact `symmetric`
+  (symmetric memory can be set up here) is agreed on with one all-reduce (MIN), as in
+  `choose_exchange`.  "auto" takes "p2p" on several ranks that all have symmetric memory, else
+  "collective"; an explicit "p2p" that some rank cannot serve raises on every rank. """
+  if exchange not in DELIVERIES:
+    raise ValueError(f"unknown exchange {exchange!r}")
+  world = dist.get_world_size(group) if dist.is_initialized() else 1
+  (symmetric,) = map(bool, _agree([int(bool(symmetric))], group))
+  if exchange == "auto":
+    return "p2p" if world > 1 and symmetric else "collective"
+  if exchange == "p2p" and not symmetric:
+    raise ValueError("the p2p exchange needs symmetric memory on every rank")
+  return exchange
+
+class _SymmetricRows:
+  """ A fp32 buffer of `shape` in symmetric memory (one allocation mapped into every rank of the group
+  over NVLink / NVSwitch), `peers[r]`: rank r's buffer as a tensor on this GPU, `barrier()`: the
+  stream-ordered device barrier of the group. """
+  def __init__(self, shape, device, group):
+    if not dist.is_initialized():
+      raise ValueError("the p2p exchange needs an initialised process group: its symmetric buffer is set up across the group's ranks")
+    import torch.distributed._symmetric_memory as symm_mem
+    group = group if group is not None else dist.group.WORLD
+    self.buffer = symm_mem.empty(*shape, dtype=torch.float32, device=device)
+    self.handle = symm_mem.rendezvous(self.buffer, group)
+    self.peers = [self.handle.get_buffer(r, tuple(shape), torch.float32) for r in range(dist.get_world_size(group))]
+  def barrier(self):
+    self.handle.barrier(channel=0)
+
+def _symmetric_rows(shape, device, group):
+  return _SymmetricRows(shape, device, group)
+
+class GradientShards:
+  """ Delivery of the worker gradients to the d-sharded path (the multi-GPU counterpart of
+  `engine.GradientStack`).  Worker i is backpropagated on rank i % R, where it is one full [d] vector;
+  the rules need columns [lo_r, hi_r) (`shard_bounds`) of all n workers on every rank r.  `push` clips
+  the gradient and writes each rank's columns straight into that rank's memory in ONE pass
+  (`bz_gradient_scatter`); `deliver` makes them visible to their owners.
+
+      shards = sharded.GradientShards(n, d, device)            # once; exchange="auto"
+      for i in shards.workers():                              # this rank's workers: i % R == rank
+        grad, loss = model.backprop(outloss=True)
+        shards.push(i, grad, clip=args.gradient_clip)
+      sampled = shards.deliver()                              # n rows of this rank's hi - lo columns
+      honest = shards.honests_worker(gmtm_shards, mu, dampening)   # or honests_server(server_shard, ...), or `sampled`
+      out = plans[shards.slot]()                              # a ShardedPlan per slot over shards.rows(slot)
+
+  exchange: "p2p"         every rank owns a SYMMETRIC buffer of two slots of [n, pitch] fp32 (pitch:
+                          ceil(d / R) rounded up to 64 floats); `push` writes slot `step % 2` of every
+                          rank over NVLink and `deliver` crosses one device-side barrier.  Two slots make
+                          that barrier enough: a producer rewrites slot s only after the barrier of the
+                          step in between, which every owner reaches only after its reads of slot s.
+            "collective"  `push` writes into this rank's [R, ceil(n / R), pitch] send buffer, `deliver`
+                          does one `all_to_all_single` into the matching receive buffer (a copy on a
+                          single rank); row i is `recv[i % R, i // R, :hi - lo]`.
+            "auto"        "p2p" when every rank of several has symmetric memory, else "collective"; the
+                          ranks agree on it (`choose_delivery`).
+  Both exchanges deliver the same bits: those of `GradientStack.push`'s sampled row, sliced.
+  Momentum is placed by the owner on its columns, all rows in one launch (`honests_worker` /
+  `honests_server`, `bz_gradient_momentum`: the arithmetic of `GradientStack.push` after the clip):
+  only the clipped gradient crosses NVLink, and the momentum buffers stay local shards.
+
+  Contract: the rows of a step stay valid until this rank calls `deliver()` of the next step.  A rank
+  whose shard is empty (rank r * ceil(d / R) >= d: when d < R, but also e.g. rank 3 for d = 9, R = 4)
+  has rows of zero columns and still joins every barrier and collective.
+  `push` of a worker this rank does not produce raises, and so does `deliver` while one of this rank's
+  workers has not been pushed.  Build one `ShardedPlan` per slot (`slots` of them) over `rows(slot)`.
+
+  `backend` provides `gradient_scatter` and `momentum_rows` (default: the CUDA engine). """
+  def __init__(self, n, d, device, group=None, exchange="auto", backend=None):
+    self.n, self.d, self.group = int(n), int(d), group
+    self.device = torch.device(device)
+    if self.device.type == "cuda" and self.device.index is None:
+      self.device = torch.device("cuda", torch.cuda.current_device())
+    self.world = dist.get_world_size(group) if dist.is_initialized() else 1
+    self.rank = dist.get_rank(group) if dist.is_initialized() else 0
+    if self.world > _lib.MAX_PEERS:
+      raise ValueError(f"GradientShards serves at most {_lib.MAX_PEERS} ranks (BZ_MAX_PEERS): the group has {self.world}")
+    self._be = backend or _engine
+    self.lo, self.hi = shard_bounds(self.d, self.world, self.rank)
+    width = self.hi - self.lo
+    self.pitch = ((self.d + self.world - 1) // self.world + 63) // 64 * 64
+    bounds = [shard_bounds(self.d, self.world, r) for r in range(self.world)]
+    self.exchange = choose_delivery(exchange, _symmetric_memory_importable(), group)
+    R = self.world
+    if self.exchange == "p2p":
+      sym = self._sym = _symmetric_rows((2, self.n, self.pitch), self.device, group)
+      self.slots = 2
+      self._local = sym.buffer
+      self._dest = {(s, i): [sym.peers[r][s, i, :hi - lo] for r, (lo, hi) in enumerate(bounds)]
+                    for s in range(2) for i in self.workers()}
+      self._rows = [[sym.buffer[s, i, :width] for i in range(self.n)] for s in range(2)]
+    else:
+      self._local = torch.empty((R, (self.n + R - 1) // R, self.pitch), dtype=torch.float32, device=self.device)
+      self._send = torch.empty_like(self._local)     # also on one rank: a push must not overwrite delivered rows
+      self.slots = 1
+      self._dest = {(0, i): [self._send[r, i // R, :hi - lo] for r, (lo, hi) in enumerate(bounds)] for i in self.workers()}
+      self._rows = [[self._local[i % R, i // R, :width] for i in range(self.n)]]
+    self._honest = None
+    self._pushed = set()
+    self.step = 0
+  def workers(self):
+    """ The workers this rank produces: i % R == rank. """
+    return range(self.rank, self.n, self.world)
+  @property
+  def slot(self):
+    """ The slot of the last delivered step (0 with the collective exchange). """
+    if self.step == 0:
+      raise RuntimeError("nothing delivered yet")
+    return (self.step - 1) % self.slots
+  def rows(self, slot=None):
+    """ This rank's columns of the n workers in `slot` (default: the last delivered step's), as views. """
+    return list(self._rows[self.slot if slot is None else slot])
+  def push(self, i, grad, clip=None):
+    """ Clip worker i's full gradient (clip None or <= 0: no clipping) and write every rank's columns
+    of it into that rank's row i of this step. """
+    if not 0 <= i < self.n or i % self.world != self.rank:
+      raise ValueError(f"worker {i} is produced on rank {i % self.world} of {self.world}, not on rank {self.rank}")
+    if grad.numel() != self.d or grad.device != self.device:
+      raise ValueError(f"grad must hold d = {self.d} elements on {self.device}: it has {grad.numel()} on {grad.device}")
+    self._be.gradient_scatter(grad, clip, self._dest[(self.step % self.slots, i)])
+    self._pushed.add(i)
+  def deliver(self):
+    """ Finish the step: every rank's pushes reach their owners.  Returns this rank's n rows. """
+    missing = [i for i in self.workers() if i not in self._pushed]
+    if missing:
+      raise RuntimeError(f"workers {missing} of rank {self.rank} were not pushed this step")
+    if self.exchange == "p2p":
+      self._sym.barrier()
+    elif self.world > 1:
+      dist.all_to_all_single(self._local, self._send, group=self.group)
+    else:
+      self._local.copy_(self._send)
+    # other GPUs' kernels (or the collective) wrote the rows: tell PyTorch, whose version counter the
+    # identity / version keyed caches of this package rely on (views share their base's counter)
+    torch.autograd.graph.increment_version(self._local)
+    self._pushed.clear()
+    self.step += 1
+    return self.rows()
+  def honests_worker(self, momentums, mu, dampening):
+    """ Worker-side momentum (attack.py:799-803) on this rank's columns: momentums[k] <- momentums[k] *
+    mu + (1 - dampening) * row k, in place, for the first len(momentums) rows.  Returns `momentums`. """
+    momentums = list(momentums)
+    if len(momentums) > self.n:
+      raise ValueError(f"{len(momentums)} momentum vectors for {self.n} workers")
+    if momentums:
+      self._be.momentum_rows(self.rows()[:len(momentums)], mu, dampening, momentums=momentums)
+    return momentums
+  def honests_server(self, server, mu, dampening, count=None):
+    """ Server-side momentum (attack.py:805-808) on this rank's columns: honest row k = row k * (1 -
+    dampening) + mu * server, for the first `count` rows (default n), into a buffer of this object
+    (rewritten by the next call).  `server` is this rank's shard of the server momentum (the previous
+    `ShardedPlan.out`).  Returns the honest rows. """
+    rows = self.rows()[:self.n if count is None else count]
+    if self._honest is None:
+      self._honest = _engine._row_buffer(self.n, self.hi - self.lo, self.device)
+    honest = [self._honest[k, :self.hi - self.lo] for k in range(len(rows))]
+    if rows:
+      self._be.momentum_rows(rows, mu, dampening, server=server, honests=honest)
+    return honest
 
 def aggregate(gar, gradients, f=None, m=None, mode="mid", group=None, backend=None, return_selection=False):
   """ Aggregate this rank's shard.

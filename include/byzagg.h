@@ -5,6 +5,9 @@
  * are relative to the reference root) and is what the reference's optional `native`
  * hook (`native.<gar>.aggregate`, aggregators/median.py:41-49, krum.py:82-96,
  * bulyan.py:86-100, brute.py:82-91) or an `aggregators.register(...)` plugin binds.
+ * The entry points of a d-sharded trainer that are not aggregation rules (delivery of the worker
+ * gradients to the GPUs that own their columns, and the owners' momentum placement) are declared in
+ * byzagg_shards.h, included at the end.
  *
  * Conventions
  *   - `rows` is a HOST array of n DEVICE pointers; row i is a contiguous fp32 vector of
@@ -264,4 +267,10 @@ BZ_API int bz_gradient_row(const float* grad, int64_t d, double clip, float* sam
 #ifdef __cplusplus
 }
 #endif
+
+/* Gradient delivery for a d-sharded trainer: bz_gradient_scatter clips one worker gradient and writes
+ * each rank's columns into that rank's memory in one pass; bz_gradient_momentum places the momentum
+ * of an owner's rows in one launch. */
+#include "byzagg_shards.h"
+
 #endif /* BYZAGG_H */
