@@ -4,6 +4,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <type_traits>
 
 #include "launch.cuh"
 #include "dist.cuh"
@@ -69,6 +70,20 @@ static int check_rows(const float* const* rows, int n, int64_t d, const void* ou
 static void fill_table(RowTable& t, const float* const* rows, int n) {
   for (int r = 0; r < n; ++r) t.p[r] = rows[r];
   for (int r = n; r < kMaxN; ++r) t.p[r] = rows[0];
+}
+
+// Unique rows by pointer equality: uniq[k] = first row with that address, to_unique[i] = its k.
+// by_address = false: every row counts as distinct (rows of an empty shard: every empty tensor has
+// address 0, so equal addresses say nothing there).
+static int dedupe_rows(const float* const* rows, int n, const float** uniq, int* to_unique, bool by_address = true) {
+  int u = 0;
+  for (int i = 0; i < n; ++i) {
+    int k = by_address ? 0 : u;
+    while (k < u && uniq[k] != rows[i]) ++k;
+    if (k == u) uniq[u++] = rows[i];
+    to_unique[i] = k;
+  }
+  return u;
 }
 
 static bool launch_median(int n, const RowTable& t, const Geom& g, float* out, cudaStream_t st) {
@@ -216,13 +231,9 @@ int bz_coordinate_host(int rule, const float* const* host_rows, int n, int f, in
   if (chunks < 1 || chunks > BZ_MAX_HOST_CHUNKS) return fail(BZ_EINVAL, "bz_coordinate_host: chunks = %d outside 1..%d", chunks, BZ_MAX_HOST_CHUNKS);
   cudaStream_t st = (cudaStream_t)stream, sin = (cudaStream_t)in_stream, sout = (cudaStream_t)out_stream;
   // every distinct host row is staged once (the attack rows of the reference are one tensor f times)
-  int slot[kMaxN], first[kMaxN], u = 0;
-  for (int i = 0; i < n; ++i) {
-    int k = 0;
-    while (k < u && host_rows[first[k]] != host_rows[i]) ++k;
-    if (k == u) first[u++] = i;
-    slot[i] = k;
-  }
+  const float* uniq[kMaxN];
+  int slot[kMaxN];
+  const int u = dedupe_rows(host_rows, n, uniq, slot);
   int64_t cs = (d + chunks - 1) / chunks;
   cs = (cs + 63) / 64 * 64;                       // chunk starts keep the 256-byte alignment of the staged rows
   cudaEvent_t ev[2 * BZ_MAX_HOST_CHUNKS + 2];
@@ -244,7 +255,7 @@ int bz_coordinate_host(int rule, const float* const* host_rows, int n, int f, in
     void* srcs[kMaxN];
     for (int k = 0; k < u; ++k) {
       dsts[k] = staging + (size_t)k * pitch + c0;
-      srcs[k] = const_cast<float*>(host_rows[first[k]] + c0);
+      srcs[k] = const_cast<float*>(uniq[k] + c0);
     }
     h2d_rows(dsts, srcs, u, (size_t)cnt * sizeof(float), sin);
     if (sin != st) cudaStreamWaitEvent(st, event_on(sin), 0);

@@ -105,17 +105,15 @@ inline unsigned long long brute_total(int n, int f) {
 }
 
 // ---- K5: scoring / selection (single CTA each) --------------------------------------------------
-// to_unique[n] / u: optional alias map (rows i, j with to_unique[i] == to_unique[j] are the same
-// tensor); the blocks are then u x u tables over the unique rows.
-void launch_krum_select(const double* parts, int nparts, int n, int f, int32_t* order, cudaStream_t st, const int* to_unique = nullptr, int u = 0);
-void launch_bulyan_select(const double* parts, int nparts, int n, int f, int m, int32_t* order, int32_t* status, cudaStream_t st, const int* to_unique = nullptr, int u = 0);
-int  launch_brute_select(const double* parts, int nparts, int n, int f, int32_t* sel, int32_t* status, cudaStream_t st, const int* to_unique = nullptr, int u = 0);
+// The scoring step of rule `sel` (kinds 1-3, the fields the distance pass would read) on `nparts`
+// blocks; brute's subset limit is the caller's to check.  sel.to_unique / u: optional alias map
+// (rows i, j with to_unique[i] == to_unique[j] are the same tensor); the blocks are then u x u
+// tables over the unique rows.
+void launch_select(const SelectTail& sel, const double* parts, int nparts, cudaStream_t st, int u = 0);
 void launch_rowdist_select(const double* parts, int nparts, int n, int sqrt_norm, int32_t* order, cudaStream_t st);
 
 // Same, reading block p IN PLACE from peers[p] (peer GPU memory over NVLink): fused exchange.
-void launch_krum_select_peers(const double* const* peers, int npeers, int n, int f, int32_t* order, cudaStream_t st);
-void launch_bulyan_select_peers(const double* const* peers, int npeers, int n, int f, int m, int32_t* order, int32_t* status, cudaStream_t st);
-int  launch_brute_select_peers(const double* const* peers, int npeers, int n, int f, int32_t* sel, int32_t* status, cudaStream_t st);
+void launch_select(const SelectTail& sel, const double* const* peers, int npeers, cudaStream_t st);
 void launch_rowdist_select_peers(const double* const* peers, int npeers, int n, int sqrt_norm, int32_t* order, cudaStream_t st);
 
 // ---- K4: Bulyan stage 1 means + coordinate-wise averaged median ----------------------------------

@@ -65,24 +65,24 @@ static void opt_in_once(K kernel, size_t bytes, unsigned long long& mask) {
 constexpr size_t kScoreSmemMax = (size_t)(2 * kMaxN * kMaxN + kMaxN) * sizeof(double);
 constexpr size_t kBruteSmemMax = (size_t)kMaxN * kMaxN * sizeof(double) + (size_t)(kMaxN + 1) * (kMaxN + 1) * sizeof(unsigned long long) + 512;
 
+// Brute (kind 3) runs k5_brute_select; Multi-Krum and Bulyan run k5_score_select, where only
+// Bulyan's step reads the status word (as in the distance pass's tail).
 template <class Parts>
-static void score_select(const Parts& parts, const RowMap& map, int nparts, int n, int count, int32_t* order, int32_t* status, int f, int m,
-                         int bulyan, cudaStream_t st) {
-  const size_t smem = (size_t)(2 * n * n + n) * sizeof(double);
-  static unsigned long long opted = 0;
-  opt_in_once(k5_score_select<Parts>, kScoreSmemMax, opted);
-  k5_score_select<Parts><<<1, kK5Threads, smem, st>>>(parts, map, nparts, n, count, order, status, f, m, bulyan);
-}
-
-template <class Parts>
-static int brute_select(const Parts& parts, const RowMap& map, int nparts, int n, int f, int32_t* sel, int32_t* status, cudaStream_t st) {
-  const unsigned long long total = brute_total(n, f);
-  if (total > (1ull << 31)) return -1;
-  const size_t smem = (size_t)n * n * sizeof(double) + (size_t)(n + 1) * (n + 1) * sizeof(unsigned long long) + 64 * sizeof(double);
-  static unsigned long long opted = 0;
-  opt_in_once(k5_brute_select<Parts>, kBruteSmemMax, opted);
-  k5_brute_select<Parts><<<1, kK5Threads, smem, st>>>(parts, map, nparts, n, f, total, sel, status);
-  return 0;
+static void rule_select(const Parts& parts, const RowMap& map, int nparts, const SelectTail& s, cudaStream_t st) {
+  const int n = s.n;
+  if (s.kind == 3) {
+    const size_t smem = (size_t)n * n * sizeof(double) + (size_t)(n + 1) * (n + 1) * sizeof(unsigned long long) + 64 * sizeof(double);
+    static unsigned long long opted = 0;
+    opt_in_once(k5_brute_select<Parts>, kBruteSmemMax, opted);
+    k5_brute_select<Parts><<<1, kK5Threads, smem, st>>>(parts, map, nparts, n, s.f, s.total, s.order, s.status);
+  } else {
+    const int bulyan = s.kind == 2;
+    const size_t smem = (size_t)(2 * n * n + n) * sizeof(double);
+    static unsigned long long opted = 0;
+    opt_in_once(k5_score_select<Parts>, kScoreSmemMax, opted);
+    k5_score_select<Parts><<<1, kK5Threads, smem, st>>>(parts, map, nparts, n, s.count, s.order, bulyan ? s.status : nullptr,
+                                                        s.f, s.m, bulyan);
+  }
 }
 
 static PeerParts make_peers(const double* const* ptrs, int npeers) {
@@ -91,32 +91,17 @@ static PeerParts make_peers(const double* const* ptrs, int npeers) {
   return p;
 }
 
-// to_unique / u: optional alias map (see RowMap); the blocks are then u x u tables.
-void launch_krum_select(const double* parts, int nparts, int n, int f, int32_t* order, cudaStream_t st, const int* to_unique, int u) {
-  const RowMap map = make_map(to_unique, n, u);
-  score_select(StridedParts{parts, (size_t)map.u * map.u}, map, nparts, n, n - f - 1, order, nullptr, f, 0, 0, st);
-}
-void launch_bulyan_select(const double* parts, int nparts, int n, int f, int m, int32_t* order, int32_t* status, cudaStream_t st, const int* to_unique, int u) {
-  const RowMap map = make_map(to_unique, n, u);
-  score_select(StridedParts{parts, (size_t)map.u * map.u}, map, nparts, n, m, order, status, f, m, 1, st);
-}
-int launch_brute_select(const double* parts, int nparts, int n, int f, int32_t* sel, int32_t* status, cudaStream_t st, const int* to_unique, int u) {
-  const RowMap map = make_map(to_unique, n, u);
-  return brute_select(StridedParts{parts, (size_t)map.u * map.u}, map, nparts, n, f, sel, status, st);
+void launch_select(const SelectTail& sel, const double* parts, int nparts, cudaStream_t st, int u) {
+  const RowMap map = make_map(sel.to_unique, sel.n, u);
+  rule_select(StridedParts{parts, (size_t)map.u * map.u}, map, nparts, sel, st);
 }
 void launch_rowdist_select(const double* parts, int nparts, int n, int sqrt_norm, int32_t* order, cudaStream_t st) {
   k5_rowdist_select<StridedParts><<<1, kRowSelThreads, 0, st>>>(StridedParts{parts, (size_t)n}, nparts, n, sqrt_norm, order);
 }
 
 // Peer variants: block p is read from peers[p] (NVLink peer memory)
-void launch_krum_select_peers(const double* const* peers, int npeers, int n, int f, int32_t* order, cudaStream_t st) {
-  score_select(make_peers(peers, npeers), identity_map(n), npeers, n, n - f - 1, order, nullptr, f, 0, 0, st);
-}
-void launch_bulyan_select_peers(const double* const* peers, int npeers, int n, int f, int m, int32_t* order, int32_t* status, cudaStream_t st) {
-  score_select(make_peers(peers, npeers), identity_map(n), npeers, n, m, order, status, f, m, 1, st);
-}
-int launch_brute_select_peers(const double* const* peers, int npeers, int n, int f, int32_t* sel, int32_t* status, cudaStream_t st) {
-  return brute_select(make_peers(peers, npeers), identity_map(n), npeers, n, f, sel, status, st);
+void launch_select(const SelectTail& sel, const double* const* peers, int npeers, cudaStream_t st) {
+  rule_select(make_peers(peers, npeers), identity_map(sel.n), npeers, sel, st);
 }
 void launch_rowdist_select_peers(const double* const* peers, int npeers, int n, int sqrt_norm, int32_t* order, cudaStream_t st) {
   k5_rowdist_select<PeerParts><<<1, kRowSelThreads, 0, st>>>(make_peers(peers, npeers), npeers, n, sqrt_norm, order);

@@ -242,6 +242,26 @@ def test_error_codes():
   torch.cuda.synchronize()
   assert torch.equal(before, x)
 
+def test_krum_peers_leaves_the_status_word_alone_when_a_check_fails():
+  """ `bz_krum_peers` zeroes its status word only once every argument has passed: a bad f or an
+  undersized workspace returns an error and writes no device memory. """
+  lib = _lib()
+  n, f, m, d = 11, 2, 3, 64
+  x = torch.randn(n, d, device=DEV)
+  out = torch.empty(d, device=DEV)
+  order = torch.empty(n, dtype=torch.int32, device=DEV)
+  status = torch.full((1,), 7, dtype=torch.int32, device=DEV)
+  blocks = torch.zeros(2, n * n, dtype=torch.float64, device=DEV)
+  flags = torch.zeros(2, 32, dtype=torch.int32, device=DEV)
+  table = lambda t: (ctypes.c_void_p * 2)(*[t[r].data_ptr() for r in range(2)])
+  ws, nbytes = _ws()
+  for bad_f, ws_bytes, code in ((n - 1, nbytes, -1), (f, 16, -4)):
+    rc = lib.bz_krum_peers(_ptrs([x[i] for i in range(n)]), n, bad_f, m, d, out.data_ptr(), order.data_ptr(), status.data_ptr(),
+                           0, 2, table(blocks), table(flags), 1, ws.data_ptr(), ws_bytes, _stream())
+    assert rc == code, lib.bz_last_error()
+  torch.cuda.synchronize()
+  assert status.item() == 7
+
 def test_cpu_tensors_are_staged():
   """ Reference-facing call with HOST tensors (attack.py --device-gar cpu): staged, result on the CPU. """
   import byzantinemomentum_b200 as bz
