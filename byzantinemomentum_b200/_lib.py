@@ -1,5 +1,6 @@
 # coding: utf-8
-"""ctypes binding of `libbyzagg.so` (C ABI: `include/byzagg.h` and `include/byzagg_shards.h`).
+"""ctypes binding of `libbyzagg.so` (C ABI: `include/byzagg.h`, `include/byzagg_shards.h` and
+`include/byzagg_attack.h`).
 
 The library is loaded lazily, on the first call that needs it, and the load FAILS LOUDLY:
 there is no CPU or PyTorch fallback anywhere in this package.  Build it in-tree with
@@ -83,6 +84,12 @@ SHARD_SIGNATURES = {
   "bz_gradient_momentum": (_i, [_c_rows, _i, _i64, _i, _c_rows, _vp, _dbl, _dbl, _c_rows, _vp]),
 }
 
+# the same for include/byzagg_attack.h (the attacks' line search)
+ATTACK_SIGNATURES = {
+  "bz_line_search_workspace_bytes": (_sz, [_i]),
+  "bz_line_search": (_i, [_i, _c_rows, _i, _i, _i, _i, _i, _vp, _vp, _i64, _i, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+}
+
 _lock = threading.Lock()
 _lib = None
 
@@ -101,7 +108,7 @@ def lib():
         handle = ctypes.CDLL(str(path))
       except OSError as err:
         raise LibraryError(f"unable to load {path}: {err}") from err
-      for name, (restype, argtypes) in list(SIGNATURES.items()) + list(SHARD_SIGNATURES.items()):
+      for name, (restype, argtypes) in list(SIGNATURES.items()) + list(SHARD_SIGNATURES.items()) + list(ATTACK_SIGNATURES.items()):
         try:
           fn = getattr(handle, name)
         except AttributeError as err:

@@ -281,3 +281,4 @@ int bz_coordinate_host(int rule, const float* const* host_rows, int n, int f, in
 }  // extern "C"
 
 #include "api_dist.inc"
+#include "api_search.inc"

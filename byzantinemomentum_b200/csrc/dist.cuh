@@ -80,6 +80,31 @@ int launch_rowdist(const RowTable& rows, int n, const float* const* host_rows, c
                    double* parts, cudaStream_t st, int reverse = 0, int32_t* order = nullptr, unsigned* ticket = nullptr,
                    int sqrt_norm = 0, int dot = 0);
 
+// ---- The attacks' line search (bz_line_search, api_search.inc) -------------------------------------
+// State of `line_maximize` (tools/misc.py:468-513) in device memory, carried from one evaluation to the next.
+struct SearchState {
+  double next_x;     // x of the next evaluation (= prop_x after the first)
+  double best_x, best_y, delta, prop_x;
+  int phase;         // 1 = expansion, 2 = contraction
+  unsigned ticket;   // last-CTA election of the score pass; 0 between passes
+};
+// What the score pass's last CTA does after summing evaluation k's score y.
+struct SearchTail {
+  SearchState* state;
+  double* trace;               // (x_k, y_k) at [2k], [2k + 1]; the chosen factor at [2 * evals]
+  const int32_t* eval_status;  // this evaluation's status word (NULL: the rule has none)
+  int32_t* status;             // first non-zero status word of the search
+  int k, evals;
+};
+// K2' over the one row `out` against `center`, chained by PDL after the rule, its last CTA rounding the
+// sum to fp32 (y) and running one transition of the search.
+int launch_rowdist_search(const float* out, const float* center, int64_t d, double* parts, const SearchTail& tail,
+                          cudaStream_t st);
+// K8 (k8_candidate.cu): byz <- the candidate row of x (which: 0 = start 0.0, also resets the state's ticket;
+// 1 = state->next_x; 2 = state->best_x, the attack's result), chained by PDL.
+int launch_candidate(const float* avg, const float* att, float* byz, int64_t d, SearchState* state, int which,
+                     int negative, int empire, cudaStream_t st);
+
 // ---- K6: study metrics in one pass (k6_study.cu) -------------------------------------------------
 // avg = (rows[0] + rows[1] + ...)/n; stats[0] = sum avg^2, stats[1] = max |avg|,
 // stats[2+i] = sum_k (rows[i][k] - avg[k])^2.  `parts` needs kMaxParts*(n+1) doubles (n >= 2) and

@@ -22,13 +22,57 @@ constexpr int kRdWarps = kRdThreads / 32;
 constexpr int kRdChunk = 4;      // rows loaded together (4 x VEC values in flight per thread)
 constexpr int kRdFlush = 8;      // vectors between two flushes
 
+// One transition of `line_maximize` (tools/misc.py:468-513, start = 0, delta = 1, ratio = 0.8) after the
+// evaluation of x = state->next_x scored y: the Python statements in the same order, in fp64 with
+// explicit rounding (no contraction).  NaN never compares greater, as in Python.
+__device__ void search_step(const SearchTail& s, const double y) {
+  SearchState* st = s.state;
+  const double x = st->next_x;
+  s.trace[2 * s.k] = x;
+  s.trace[2 * s.k + 1] = y;
+  int32_t code = s.k == 0 ? 0 : *s.status;
+  if (code == 0 && s.eval_status != nullptr) code = *s.eval_status;
+  *s.status = code;
+  double best_x, best_y, delta, prop_x = x;
+  int phase;
+  if (s.k == 0) {                       // best_x = start; best_y = scape(best_x)
+    best_x = x; best_y = y; delta = 1.; phase = 1;
+  } else {
+    best_x = st->best_x; best_y = st->best_y; delta = st->delta; phase = st->phase;
+    if (phase == 1) {                   // expansion
+      if (y > best_y) { best_y = y; best_x = prop_x; delta = __dmul_rn(delta, 2.); }
+      else            { delta = __dmul_rn(delta, 0.8); phase = 2; }
+    } else {                            // contraction
+      if (y > best_y) { best_y = y; best_x = prop_x; }
+      delta = __dmul_rn(delta, 0.8);
+    }
+  }
+  // the x the next evaluation (if any) takes
+  if (phase == 1) {
+    prop_x = __dadd_rn(best_x, delta);
+  } else if (prop_x < best_x) {
+    prop_x = __dadd_rn(prop_x, delta);
+  } else {
+    double t = __dsub_rn(prop_x, delta);
+    while (t < 0.) t = __ddiv_rn(__dadd_rn(t, prop_x), 2.);
+    prop_x = t;
+  }
+  st->best_x = best_x; st->best_y = best_y; st->delta = delta; st->prop_x = prop_x; st->phase = phase;
+  st->next_x = prop_x;
+  if (s.k == s.evals - 1) s.trace[2 * s.evals] = best_x;
+}
+
 // DOT: sum_k x_r[k] * c[k] instead of the squared distance (the dot products of the study step,
 // attack.py:854-866: one vector against up to 64 others in one pass).
-template <bool CENTER, int VEC, bool DOT = false>
+// SEARCH: the score of the attacks' line search (one row, `search` set): launched by PDL after the rule,
+// the last CTA rounds the sum to fp32 and runs `search_step` instead of the selection.
+template <bool CENTER, int VEC, bool DOT = false, bool SEARCH = false>
 __global__ void __launch_bounds__(kRdThreads, 2)
 k2_rowdist(const __grid_constant__ RowTable rows, const int n, const float* __restrict__ center, const Geom g,
-           double* __restrict__ parts, int32_t* __restrict__ order, unsigned* __restrict__ ticket, const int sqrt_norm) {
+           double* __restrict__ parts, int32_t* __restrict__ order, unsigned* __restrict__ ticket, const int sqrt_norm,
+           const SearchTail search) {
   __shared__ double warp_tot[kRdWarps][kMaxN];
+  if (SEARCH) pdl_wait();      // the rule's output is valid from here
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   float acc[kMaxN];
 #pragma unroll
@@ -107,7 +151,8 @@ k2_rowdist(const __grid_constant__ RowTable rows, const int n, const float* __re
     for (int w = 0; w < kRdWarps; ++w) s += warp_tot[w][threadIdx.x];
     parts[(size_t)blockIdx.x * n + threadIdx.x] = s;
   }
-  if (order == nullptr) return;
+  if (!SEARCH && order == nullptr) return;
+  if (SEARCH) ticket = &search.state->ticket;
   // The selection step (aksel.py:49 / cge.py:38: stable order of the n keys) in the LAST CTA to
   // finish instead of a single-CTA launch: blocks summed in S interleaved classes with every load in
   // flight, class sums added in class order (fixed for a given grid), keys as in k5_rowdist_select.
@@ -144,10 +189,15 @@ k2_rowdist(const __grid_constant__ RowTable rows, const int n, const float* __re
       v = (double)fp32_norm(sum);                    // cge.py:36-37: fp32 norm, non-finite -> +inf
       if (!finite_d(v)) v = CUDART_INF;
     } else {
-      v = (double)(float)sum;                        // aksel.py:41: fp32 sum of squares
+      v = (double)(float)sum;                        // aksel.py:41 (and the search's `dot`): fp32 sum of squares
+    }
+    if (SEARCH) {
+      search_step(search, v);
+      *ticket = 0u;
     }
     key[threadIdx.x] = v;
   }
+  if (SEARCH) return;
   __syncthreads();
   stable_order(key, n, order);
   if (threadIdx.x == 0) *ticket = 0u;
@@ -165,19 +215,35 @@ int launch_rowdist(const RowTable& rows, int n, const float* const* host_rows, c
   if (grid > kMaxParts) grid = kMaxParts;
   if (grid < 1) grid = 1;
   if (dot && center != nullptr) {
-    if (g.vec == 4) k2_rowdist<true, 4, true><<<(unsigned)grid, kRdThreads, 0, st>>>(rows, n, center, g, parts, nullptr, nullptr, 0);
-    else            k2_rowdist<true, 1, true><<<(unsigned)grid, kRdThreads, 0, st>>>(rows, n, center, g, parts, nullptr, nullptr, 0);
+    if (g.vec == 4) k2_rowdist<true, 4, true><<<(unsigned)grid, kRdThreads, 0, st>>>(rows, n, center, g, parts, nullptr, nullptr, 0, SearchTail{});
+    else            k2_rowdist<true, 1, true><<<(unsigned)grid, kRdThreads, 0, st>>>(rows, n, center, g, parts, nullptr, nullptr, 0, SearchTail{});
     return (int)grid;
   }
   if (order != nullptr) cudaMemsetAsync(ticket, 0, sizeof(unsigned), st);
   if (g.vec == 4) {
-    if (center) k2_rowdist<true, 4><<<(unsigned)grid, kRdThreads, 0, st>>>(rows, n, center, g, parts, order, ticket, sqrt_norm);
-    else        k2_rowdist<false, 4><<<(unsigned)grid, kRdThreads, 0, st>>>(rows, n, center, g, parts, order, ticket, sqrt_norm);
+    if (center) k2_rowdist<true, 4><<<(unsigned)grid, kRdThreads, 0, st>>>(rows, n, center, g, parts, order, ticket, sqrt_norm, SearchTail{});
+    else        k2_rowdist<false, 4><<<(unsigned)grid, kRdThreads, 0, st>>>(rows, n, center, g, parts, order, ticket, sqrt_norm, SearchTail{});
   } else {
-    if (center) k2_rowdist<true, 1><<<(unsigned)grid, kRdThreads, 0, st>>>(rows, n, center, g, parts, order, ticket, sqrt_norm);
-    else        k2_rowdist<false, 1><<<(unsigned)grid, kRdThreads, 0, st>>>(rows, n, center, g, parts, order, ticket, sqrt_norm);
+    if (center) k2_rowdist<true, 1><<<(unsigned)grid, kRdThreads, 0, st>>>(rows, n, center, g, parts, order, ticket, sqrt_norm, SearchTail{});
+    else        k2_rowdist<false, 1><<<(unsigned)grid, kRdThreads, 0, st>>>(rows, n, center, g, parts, order, ticket, sqrt_norm, SearchTail{});
   }
   return (int)grid;
+}
+
+int launch_rowdist_search(const float* out, const float* center, int64_t d, double* parts, const SearchTail& tail,
+                          cudaStream_t st) {
+  RowTable rows;
+  for (int r = 0; r < kMaxN; ++r) rows.p[r] = out;
+  const Geom g = make_geom(&out, 1, center, nullptr, d, 4);
+  int64_t grid = (g.nv + kRdThreads - 1) / kRdThreads;
+  const int64_t cap = (int64_t)sm_count() * 2;
+  if (grid > cap) grid = cap;
+  if (grid > kMaxParts) grid = kMaxParts;
+  if (grid < 1) grid = 1;
+  const cudaError_t err = g.vec == 4
+      ? launch_after(k2_rowdist<true, 4, false, true>, (unsigned)grid, kRdThreads, 0, st, rows, 1, center, g, parts, nullptr, nullptr, 0, tail)
+      : launch_after(k2_rowdist<true, 1, false, true>, (unsigned)grid, kRdThreads, 0, st, rows, 1, center, g, parts, nullptr, nullptr, 0, tail);
+  return err == cudaSuccess ? (int)grid : -1;
 }
 
 }  // namespace bz

@@ -26,7 +26,7 @@ __all__ = ["average", "median", "trmean", "phocas", "meamed", "krum", "bulyan", 
            "pairdist_partial", "rowdist_partial", "select", "krum_select", "bulyan_select", "brute_select",
            "rowdist_select", "average_selected", "bulyan_reduce", "avg_dev_max_async", "compute_avg_dev_max", "rowdots_async", "study_step",
            "StudyPartials", "study_partials", "study_finish",
-           "config", "Plan", "pair_cache_stats", "GradientStack", "gradient_scatter", "momentum_rows", "host_path_report"]
+           "LineSearch", "line_search", "config", "Plan", "pair_cache_stats", "GradientStack", "gradient_scatter", "momentum_rows", "host_path_report"]
 
 class _Config:
   """ strict_status: after brute / bulyan, read the device status word (one 4-byte D2H copy,
@@ -546,6 +546,90 @@ def aksel(gradients, f, mode="mid"):
 
 def cge(gradients, f):
   return _distance("cge", gradients, f)
+
+# ---------------------------------------------------------------------------- #
+# The attacks' line search (attacks/identical.py:67-77, attacks/empire.py:51-59, tools/misc.py:468-513)
+
+_SEARCH_RULES = dict(_RULE_CODES, krum=5, bulyan=6, brute=7, aksel=8, cge=9)      # BZ_RULE_*
+_SEARCH_KINDS = {"identical": 0, "empire-strict": 1}                             # BZ_ATTACK_*
+
+class LineSearch:
+  """ A prepared `bz_line_search`: `line_maximize(eval_factor, evals)` of the identical-family attacks
+  (kind "identical": candidate `grad_avg + s * grad_att`, s = -x when `negative`) or of empire-strict
+  (kind "empire-strict": `grad_avg.mul(-x)`) against the rule `gar` with its defaults and f = f_decl,
+  every evaluation, score and next factor computed on the device.  Like `Plan`, `search()` only issues
+  the call (no allocation, no synchronisation; `graph()` captures it) and holds what it reads and writes:
+      byz     the candidate row; after the call the attack's Byzantine gradient for the chosen factor
+      record  fp64 [2 * evals + 2]: (x_k, y_k) per evaluation, the chosen factor, then the status word
+  `result()` reads `record` once and returns (factor, trace), raising where the plain rule raises. """
+  def __init__(self, gar, grad_honests, f_real, f_decl, grad_avg, grad_att, evals, negative=False, kind="identical"):
+    if gar not in _SEARCH_RULES:
+      raise KeyError(f"unknown aggregation rule {gar!r}")
+    if kind not in _SEARCH_KINDS:
+      raise ValueError(f"unknown attack kind {kind!r}, expected one of {sorted(_SEARCH_KINDS)}")
+    honest = list(grad_honests)
+    prep = _prepare(honest)
+    if prep.to_cpu:
+      raise ValueError("the line search takes CUDA tensors")
+    if not all(g.is_contiguous() for g in honest):
+      raise ValueError("the line search takes contiguous honest gradients")
+    self.gar, self.evals, self.device = gar, int(evals), prep.device
+    self.rows = honest
+    self.vectors = [grad_avg] if grad_att is None else [grad_avg, grad_att]
+    for vector in self.vectors:
+      _check_like_rows(vector, prep, "grad_avg and grad_att")
+    self.byz = torch.empty(prep.d, dtype=torch.float32, device=prep.device)
+    self._out = torch.empty(prep.d, dtype=torch.float32, device=prep.device)
+    self.record = torch.empty(2 * max(self.evals, 0) + 2, dtype=torch.float64, device=prep.device)
+    n = prep.n + int(f_real)
+    self._ws = torch.empty(int(_lib.lib().bz_line_search_workspace_bytes(min(max(n, 1), _lib.MAX_N))), dtype=torch.uint8, device=prep.device)
+    status = self.record.data_ptr() + 8 * (self.record.numel() - 1)
+    self._fn = _lib.lib().bz_line_search
+    self._args = (_SEARCH_RULES[gar], prep.ptrs, prep.n, int(f_real), int(f_decl), _SEARCH_KINDS[kind], int(bool(negative)),
+                  grad_avg.data_ptr(), None if grad_att is None else grad_att.data_ptr(), prep.d, self.evals,
+                  self.byz.data_ptr(), self._out.data_ptr(), self.record.data_ptr(), status,
+                  self._ws.data_ptr(), self._ws.numel(), prep.stream)
+    self._graph = None
+  def __call__(self):
+    """ Enqueue the search on the current stream of the rows' device. """
+    with _on(self.device):
+      _call(self._fn, self._args[:-1] + (torch.cuda.current_stream(self.device).cuda_stream,))
+    return self.byz
+  def graph(self):
+    """ Capture the search in a CUDA graph; returns `replay`, which launches it and returns `byz`. """
+    if self._graph is None:
+      with _on(self.device):
+        self()                                           # warm-up outside the capture
+        torch.cuda.synchronize(self.device)
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph):
+          code = self._fn(*(self._args[:-1] + (torch.cuda.current_stream(self.device).cuda_stream,)))
+        if code != 0:
+          _lib.check(code, self._fn.__name__)
+      self._graph = graph
+    graph, byz = self._graph, self.byz
+    def replay():
+      graph.replay()
+      return byz
+    return replay
+  def result(self):
+    """ (factor, trace) from ONE device->host read: trace = [(x_k, y_k), ...].  With
+    `config.strict_status`, a failed evaluation of Bulyan or brute raises what the plain call raises. """
+    host = self.record.cpu()
+    code = int(host[-1:].view(torch.int32)[0])
+    if config.strict_status:
+      _raise_status(code)
+    values = host.tolist()
+    return values[2 * self.evals], [(values[2 * k], values[2 * k + 1]) for k in range(self.evals)]
+
+def line_search(gar, grad_honests, f_real, f_decl, grad_avg, grad_att, evals, negative=False, kind="identical"):
+  """ The attacks' factor search on the device (see `LineSearch`).  Returns (factor, byz): the factor
+  `tools.line_maximize` picks, a Python float, and the Byzantine gradient the attack returns for it, a
+  device tensor (the reference returns it `f_real` times, aliased). """
+  search = LineSearch(gar, grad_honests, f_real, f_decl, grad_avg, grad_att, evals, negative, kind)
+  byz = search()
+  factor, _ = search.result()
+  return factor, byz
 
 # ---------------------------------------------------------------------------- #
 # Study metrics on the same stack (tools/pytorch.py:97-125, attack.py:846-848)

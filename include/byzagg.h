@@ -273,4 +273,8 @@ BZ_API int bz_gradient_row(const float* grad, int64_t d, double clip, float* sam
  * of an owner's rows in one launch. */
 #include "byzagg_shards.h"
 
+/* The attacks' line search on the device: every evaluation of the rule, its score and the choice of the
+ * next factor enqueued back to back, one host read for the outcome. */
+#include "byzagg_attack.h"
+
 #endif /* BYZAGG_H */

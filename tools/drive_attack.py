@@ -6,8 +6,9 @@ The reference downloads its datasets (torchvision); here `experiments.make_datas
 at call time by attack.py:530 — is replaced by a generator of synthetic batches of the right
 shape (`experiments/dataset.py:187-190` accepts a generator), the rules of this repository are
 registered through the reference's own `aggregators.register` under `b200-<name>`
-(`plugin.install`), optionally the study metrics are swapped (`plugin.install_tools`), and
-`attack.py` is executed with `runpy` exactly as `python3 attack.py <args>` would.
+(`plugin.install`), optionally the study metrics are swapped (`plugin.install_tools`) and the
+line-searching attacks replaced (`plugin.install_attacks`), and `attack.py` is executed with `runpy`
+exactly as `python3 attack.py <args>` would.
 
     python tools/drive_attack.py --reference /path/to/ByzantineMomentum --shape mnist -- \\
         --gar b200-krum --nb-workers 11 --nb-decl-byz 3 --nb-real-byz 3 --attack empire \\
@@ -154,6 +155,8 @@ def main():
     help="execute attack.py with its per-worker clip/clone/momentum statements (attack.py:775-780, 790-795, 799-808) replaced IN MEMORY by GradientStack.push (the file on disk is not touched; every anchor must match exactly)")
   parser.add_argument("--fuse-study", action="store_true",
     help="execute attack.py with its study block (attack.py:846-866: three compute_avg_dev_max, the defense norm, six cosines, the past cosine and the curvature: 9 + nb_for_study_past host syncs) replaced IN MEMORY by engine.study_step (one host read for all dot products)")
+  parser.add_argument("--fuse-attacks", action="store_true",
+    help="replace the little, empire, bulyan and empire-strict attacks (plugin.install_attacks): with a negative factor against a b200 rule, the whole line search (attacks/identical.py:67-77: 16 rule calls and 16 host syncs per step by default) runs on the device with one host read")
   parser.add_argument("--batch", default=None, help="JSON file with a list of {tag, args}: run attack.py once per entry in this process")
   parser.add_argument("rest", nargs=argparse.REMAINDER, help="arguments of attack.py (after --)")
   args = parser.parse_args()
@@ -170,6 +173,7 @@ def main():
 
   import torch
   import aggregators
+  import attacks
   import experiments
   import tools
   import byzantinemomentum_b200 as bz
@@ -190,6 +194,8 @@ def main():
   if args.install_tools:
     bz.plugin.install_tools(tools)
   cuda_study = tools.compute_avg_dev_max
+  if args.fuse_attacks:
+    names += [f"attack {name}" for name in bz.plugin.install_attacks(attacks)]
   print(f"registered: {', '.join(names)}", flush=True)
   counts = {}
   if args.count_calls:

@@ -1,8 +1,17 @@
 #!/usr/bin/env python3
 # coding: utf-8
 """Per-evaluation time of the attacks' line search (attacks/identical.py:68-77): 16 evaluations of
-the rule on the same honest rows with a new Byzantine row each, with and without distance reuse."""
-import json, pathlib, sys
+the rule on the same honest rows with a new Byzantine row each, with and without distance reuse.
+
+With --search: the time of one step's whole search instead (`little`'s direction, factor -16):
+  host_ms    the reference's statements (identical.py:67-77) over `bz.gars`: per evaluation the
+             candidate row, the rule, `sub_`, `dot(...).item()` (one host sync each), at the x values
+             the device search visits (the host search makes the same choices up to score ties);
+  device_ms  `engine.LineSearch` issued and read once (`result()`), eager;
+  graph_ms   the same search replayed from a CUDA graph, then read once.
+Wall clock around work that ends in a synchronisation, median of REPS, after warm-up.  The card's name
+and power limit are read in the same run."""
+import json, pathlib, subprocess, sys, time
 sys.path.insert(0, str(pathlib.Path(__file__).resolve().parent.parent))
 import torch
 import byzantinemomentum_b200 as bz
@@ -11,6 +20,70 @@ dev = torch.device("cuda", 0)
 bz.config.strict_status = False
 out = []
 QUICK = "--quick" in sys.argv
+
+def card():
+  query = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                         capture_output=True, text=True).stdout.strip().splitlines()
+  return query[0] if query else torch.cuda.get_device_name(dev)
+
+def median_ms(fn, reps):
+  times = []
+  for _ in range(reps):
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    fn()
+    torch.cuda.synchronize()
+    times.append((time.perf_counter() - t0) * 1e3)
+  times.sort()
+  return times[len(times) // 2]
+
+def search_times():
+  """ One step's whole search, old host loop vs the device search (eager and graph-replayed). """
+  reps = 5 if QUICK else 21
+  cases = (("trmean", 51, 12, 79_510), ("median", 51, 12, 79_510), ("krum", 25, 5, 79_510),
+           ("trmean", 25, 5, 1_310_922), ("median", 25, 5, 1_310_922), ("krum", 25, 5, 1_310_922))
+  result = dict(card=card(), cases=[])
+  for gar, n, f, d in cases[:1] if QUICK else cases:
+    gen = torch.Generator(device=dev).manual_seed(2)
+    honest = [torch.randn(d, device=dev, generator=gen) * (1 + i / n) for i in range(n - f)]
+    stck = torch.stack(honest)
+    avg, att = stck.mean(dim=0), stck.var(dim=0).sqrt_()
+    search = engine.LineSearch(gar, honest, f, f, avg, att, 16)
+    search()
+    factor, trace = search.result()
+    xs = [x for x, _ in trace]
+    def host():
+      for x in xs:                                       # identical.py:67-74 at the visited factors
+        grad_attack = avg + x * att
+        aggregated = bz.gars[gar](gradients=honest + [grad_attack] * f, f=f)
+        aggregated.sub_(avg)
+        aggregated.dot(aggregated).item()
+      byz = avg.clone()
+      byz.add_(att.mul(factor))
+    def device():
+      search()
+      search.result()
+    replay = search.graph()
+    def graphed():
+      replay()
+      search.result()
+    for fn in (host, device, graphed):
+      fn()                                               # warm-up: modules, allocator, distance table
+    rec = dict(gar=gar, n=n, f=f, d=d, evals=16, factor=factor)
+    for name, fn in (("host_ms", host), ("device_ms", device), ("graph_ms", graphed)):
+      rec[name] = round(median_ms(fn, reps), 4)
+    rec["device_speedup"] = round(rec["host_ms"] / rec["device_ms"], 3)
+    rec["graph_speedup"] = round(rec["host_ms"] / rec["graph_ms"], 3)
+    result["cases"].append(rec)
+    print(json.dumps(rec), flush=True)
+  return result
+
+if "--search" in sys.argv:
+  result = search_times()
+  print(json.dumps(dict(card=result["card"])), flush=True)
+  if len(sys.argv) > 1 and not sys.argv[1].startswith("--"):
+    pathlib.Path(sys.argv[1]).write_text(json.dumps(result, indent=1))
+  sys.exit(0)
 REPS = 5
 CASES = (("krum", 25, 5, 5, 1_310_922),) if QUICK else (("krum", 25, 5, 5, 1_310_922), ("bulyan", 25, 5, 5, 1_310_922), ("krum", 51, 12, 12, 1_310_922), ("krum", 11, 3, 3, 1_310_922),
                          ("krum", 25, 5, 5, 79_510), ("krum", 51, 12, 12, 79_510))
