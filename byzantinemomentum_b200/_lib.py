@@ -1,6 +1,6 @@
 # coding: utf-8
-"""ctypes binding of `libbyzagg.so` (C ABI: `include/byzagg.h`, `include/byzagg_shards.h` and
-`include/byzagg_attack.h`).
+"""ctypes binding of `libbyzagg.so` (C ABI: `include/byzagg.h`, `include/byzagg_shards.h`,
+`include/byzagg_attack.h` and `include/byzagg_search_shards.h`).
 
 The library is loaded lazily, on the first call that needs it, and the load FAILS LOUDLY:
 there is no CPU or PyTorch fallback anywhere in this package.  Build it in-tree with
@@ -90,6 +90,16 @@ ATTACK_SIGNATURES = {
   "bz_line_search": (_i, [_i, _c_rows, _i, _i, _i, _i, _i, _vp, _vp, _i64, _i, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
 }
 
+# the same for include/byzagg_search_shards.h (the line search on a d-sharded trainer)
+SEARCH_SHARD_SIGNATURES = {
+  "bz_pairdist_partial_reuse": (_i, [_c_rows, _i, _i64, _vp, _vp, _vp, _i, _vp, _vp, _vp, _sz, _vp]),
+  "bz_search_candidate": (_i, [_vp, _vp, _vp, _i64, _vp, _i, _i, _i, _vp]),
+  "bz_search_score_partial": (_i, [_vp, _vp, _i64, _vp, _vp, _vp, _sz, _vp]),
+  "bz_search_step": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _i, _i, _vp]),
+}
+SEARCH_STATE_BYTES = 64                     # BZ_SEARCH_STATE_BYTES
+CANDIDATE_FIRST, CANDIDATE_NEXT, CANDIDATE_FINAL = 0, 1, 2
+
 _lock = threading.Lock()
 _lib = None
 
@@ -108,7 +118,8 @@ def lib():
         handle = ctypes.CDLL(str(path))
       except OSError as err:
         raise LibraryError(f"unable to load {path}: {err}") from err
-      for name, (restype, argtypes) in list(SIGNATURES.items()) + list(SHARD_SIGNATURES.items()) + list(ATTACK_SIGNATURES.items()):
+      tables = (SIGNATURES, SHARD_SIGNATURES, ATTACK_SIGNATURES, SEARCH_SHARD_SIGNATURES)
+      for name, (restype, argtypes) in [item for table in tables for item in table.items()]:
         try:
           fn = getattr(handle, name)
         except AttributeError as err:

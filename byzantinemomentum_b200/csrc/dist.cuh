@@ -72,6 +72,8 @@ int launch_pairdist_ring(const RowTable& rows, int n, int64_t d, double* parts, 
 // Runs the ring, or the cp.async kernel of k2_pairdist.cu when the ring returns -1.
 int launch_pairdist_auto(const RowTable& rows, int u, int64_t d, double* parts, cudaStream_t st,
                          const int* to_unique, int n_orig, SelectTail* select = nullptr);
+// The unique rows whose self distance is needed (more than one original row maps to them); returns their count.
+int aliased_rows(const int* to_unique, int u, int n_orig, unsigned char* self_rows);
 
 // K2': parts[x*n + i] = share of sum_k (rows[i][k] - center[k])^2 (center NULL: the origin).
 // order != NULL: the last CTA also sums the blocks and writes the stable order of the n keys
@@ -95,6 +97,8 @@ struct SearchTail {
   const int32_t* eval_status;  // this evaluation's status word (NULL: the rule has none)
   int32_t* status;             // first non-zero status word of the search
   int k, evals;
+  double* partial;             // non-NULL (d-sharded search): the score pass writes its fp64 sum here instead
+                               // of running the transition (bz_search_step adds the ranks' sums first)
 };
 // K2' over the one row `out` against `center`, chained by PDL after the rule, its last CTA rounding the
 // sum to fp32 (y) and running one transition of the search.
@@ -104,6 +108,9 @@ int launch_rowdist_search(const float* out, const float* center, int64_t d, doub
 // 1 = state->next_x; 2 = state->best_x, the attack's result), chained by PDL.
 int launch_candidate(const float* avg, const float* att, float* byz, int64_t d, SearchState* state, int which,
                      int negative, int empire, cudaStream_t st);
+// K9 (k9_search_step.cu): one CTA adds the R score partials in rank order, rounds the sum to fp32 (y) and
+// runs the transition of evaluation tail.k.
+int launch_search_step(const double* partials, int nparts, const SearchTail& tail, cudaStream_t st);
 
 // ---- K6: study metrics in one pass (k6_study.cu) -------------------------------------------------
 // avg = (rows[0] + rows[1] + ...)/n; stats[0] = sum avg^2, stats[1] = max |avg|,

@@ -246,9 +246,7 @@ static int launch_pairdist(const RowTable& rows, int n, int64_t d, double* parts
   return gx;
 }
 
-int launch_pairdist_auto(const RowTable& rows, int u, int64_t d, double* parts, cudaStream_t st,
-                         const int* to_unique, int n_orig, SelectTail* select) {
-  unsigned char self_rows[kMaxN];
+int aliased_rows(const int* to_unique, int u, int n_orig, unsigned char* self_rows) {
   int nself = 0;
   if (to_unique != nullptr && u < n_orig) {
     int mult[kMaxN] = {0};
@@ -256,6 +254,13 @@ int launch_pairdist_auto(const RowTable& rows, int u, int64_t d, double* parts, 
     for (int k = 0; k < u; ++k)
       if (mult[k] > 1) self_rows[nself++] = (unsigned char)k;
   }
+  return nself;
+}
+
+int launch_pairdist_auto(const RowTable& rows, int u, int64_t d, double* parts, cudaStream_t st,
+                         const int* to_unique, int n_orig, SelectTail* select) {
+  unsigned char self_rows[kMaxN];
+  const int nself = aliased_rows(to_unique, u, n_orig, self_rows);
   const int nparts = launch_pairdist_ring(rows, u, d, parts, st, self_rows, nself, select);
   if (nparts > 0) return nparts;
   if (select != nullptr) select->fused = 0;

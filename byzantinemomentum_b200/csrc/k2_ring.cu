@@ -64,7 +64,8 @@ struct SelfList {
 // longer needs: the rule's K5 step without its launch (k5_device.cuh).
 struct RingTail {
   int kind;                 // 0 = none, 1 = Multi-Krum order, 2 = Bulyan order + status, 3 = brute subset,
-                            // 4 = only the reduced u x u block, written to `order` (a double*)
+                            // 4 = only the reduced block, in the N x N layout of the original rows, written to
+                            //     `order` (a double*)
   int n, f, m, count, slices;
   unsigned long long total; // brute: C(n, n - f)
   int32_t* order;
@@ -561,12 +562,38 @@ k2_ring(const __grid_constant__ RowTable rows, const __grid_constant__ SelfList 
         __threadfence();
         double* sm = reinterpret_cast<double*>(smem_raw);
         if (tail.kind == 4) {
-          // phase A of the d-sharded path: this rank's reduced block (entries outside i < j are 0)
-          double* out_block = reinterpret_cast<double*>(tail.order);
+          // Phase A of the d-sharded path: this rank's reduced block.  The u x u table over the unique rows
+          // first (pairs of two rows of a previous table from `cache_in`, every other pair and the alias
+          // flags on the diagonal from this pass, group blocks added in index order), kept in `cache_out`
+          // when asked; then the block in the N x N layout of the original rows, as the exchange below
+          // publishes it: entry (i, j), i < j, is the pair of their distinct rows (the alias flag when both
+          // are one tensor), every other entry 0.
+          const int N = tail.n;
+          const RowMap& map = tail.map;
           for (int e = threadIdx.x; e < len; e += kThreads) {
-            double sum = 0.;
-            for (int g = 0; g < ngroups; ++g) sum += __ldcg(gblocks + (size_t)g * len + e);
-            out_block[e] = (e / n < e % n) ? sum : 0.;
+            const int i = e / n, j = e - i * n;
+            double v = 0.;
+            if (i <= j) {
+              const int oi = tail.old_index[i], oj = tail.old_index[j];
+              if (i < j && tail.cache_in != nullptr && oi >= 0 && oj >= 0) {
+                v = __ldcg(tail.cache_in + (size_t)min(oi, oj) * tail.u_old + max(oi, oj));
+              } else {
+                for (int g = 0; g < ngroups; ++g) v += __ldcg(gblocks + (size_t)g * len + e);
+              }
+            }
+            sm[e] = v;
+            if (tail.cache_out != nullptr) tail.cache_out[e] = v;
+          }
+          __syncthreads();
+          double* out_block = reinterpret_cast<double*>(tail.order);
+          for (int e = threadIdx.x; e < N * N; e += kThreads) {
+            const int i = e / N, j = e - i * N;
+            double v = 0.;
+            if (i < j) {
+              const int a = map.to_unique[i], b = map.to_unique[j];
+              v = sm[min(a, b) * n + max(a, b)];
+            }
+            out_block[e] = v;
           }
         } else {
           // The summed u x u table, group blocks added in index order (canonical: a pair has the same
@@ -675,7 +702,8 @@ static bool ring_shape(int n, int& shape, int& C) {
 }
 
 // Whether the scoring step's tables fit the ring's stage area, where it works once the ring is drained
-// (the barriers behind the stages stay untouched).  Kind 4 writes its block to global memory only.
+// (the barriers behind the stages stay untouched).  Kind 4 keeps only the u x u table there, which the
+// stages of u rows always hold (u * u * 8 bytes <= 3 stages of u rows of 256 floats).
 static bool tail_fits(const SelectTail& sel, size_t stage_area) {
   if (sel.kind == 4) return true;
   const size_t nn = (size_t)sel.n * sel.n * sizeof(double);
@@ -783,7 +811,7 @@ int launch_pairdist_ring(const RowTable& rows, int n, int64_t d, double* parts, 
     // taken when 1..kStarMax unique rows are new, every other one is in the table, and that table
     // came out of the same launch shape and cluster size (functions of the row count) — then every
     // pair has the bits the full pass would give it.
-    if (select->cache_in != nullptr && select->old_index != nullptr && select->u_old >= 1 && select->kind != 4) {
+    if (select->cache_in != nullptr && select->old_index != nullptr && select->u_old >= 1) {
       int fresh[kMaxN], nfresh = 0;
       bool ok = true;
       for (int k = 0; k < n; ++k) {

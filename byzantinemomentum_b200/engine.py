@@ -615,12 +615,17 @@ class LineSearch:
   def result(self):
     """ (factor, trace) from ONE device->host read: trace = [(x_k, y_k), ...].  With
     `config.strict_status`, a failed evaluation of Bulyan or brute raises what the plain call raises. """
-    host = self.record.cpu()
-    code = int(host[-1:].view(torch.int32)[0])
-    if config.strict_status:
-      _raise_status(code)
-    values = host.tolist()
-    return values[2 * self.evals], [(values[2 * k], values[2 * k + 1]) for k in range(self.evals)]
+    return _search_outcome(self.record, self.evals)
+
+def _search_outcome(record, evals):
+  """ (factor, trace) of a search's record (fp64 [2 * evals + 2]: the trace, the factor, the status word),
+  read with one device->host copy; raises on a failed evaluation with `config.strict_status`. """
+  host = record.cpu()
+  code = int(host[-1:].view(torch.int32)[0])
+  if config.strict_status:
+    _raise_status(code)
+  values = host.tolist()
+  return values[2 * evals], [(values[2 * k], values[2 * k + 1]) for k in range(evals)]
 
 def line_search(gar, grad_honests, f_real, f_decl, grad_avg, grad_att, evals, negative=False, kind="identical"):
   """ The attacks' factor search on the device (see `LineSearch`).  Returns (factor, byz): the factor

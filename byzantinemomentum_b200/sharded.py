@@ -31,7 +31,7 @@ import torch.distributed as dist
 from . import _lib
 from . import engine as _engine
 
-__all__ = ["aggregate", "aggregate_p2p", "compute_avg_dev_max", "study_step", "replicate", "apply_update", "shard_bounds", "rows_aligned", "choose_exchange", "PeerExchange", "FusedExchange", "ShardedPlan", "GradientShards", "choose_delivery", "COORDINATE_WISE", "DISTANCE_BASED"]
+__all__ = ["aggregate", "aggregate_p2p", "compute_avg_dev_max", "study_step", "replicate", "apply_update", "shard_bounds", "rows_aligned", "choose_exchange", "PeerExchange", "FusedExchange", "ShardedPlan", "GradientShards", "choose_delivery", "ShardedLineSearch", "line_search", "COORDINATE_WISE", "DISTANCE_BASED"]
 
 COORDINATE_WISE = ("average", "median", "trmean", "phocas", "meamed")
 DISTANCE_BASED = _engine.DISTANCE_BASED
@@ -469,6 +469,197 @@ class GradientShards:
     if rows:
       self._be.momentum_rows(rows, mu, dampening, server=server, honests=honest)
     return honest
+
+_CACHE_DOUBLES = _lib.MAX_N * _lib.MAX_N            # BZ_CACHE_DOUBLES
+
+class _SearchShard:
+  """ One rank's device side of `ShardedLineSearch`: the calls of every stage resolved once (row pointers,
+  buffers, workspace, the current stream at construction), for `world` ranks.
+    blocks, part   [world, width] gathered partial blocks of the rule / this rank's block (blocks[0] on one rank)
+    scores, score  [world] gathered score shares / this rank's share (scores[:1] on one rank) """
+  def __init__(self, gar, grad_honests, f_real, f_decl, grad_avg, grad_att, evals, negative, kind, world):
+    honest = list(grad_honests)
+    f_real = int(f_real)
+    n = len(honest) + f_real
+    if f_real < 1 or n > _lib.MAX_N:
+      raise ValueError(f"f_real = {f_real} with {len(honest)} honest rows: expected f_real >= 1 and at most {_lib.MAX_N} rows")
+    prep = _engine._prepare_device(honest, "the line search takes CUDA tensors")
+    if not all(g.is_contiguous() for g in honest):
+      raise ValueError("the line search takes contiguous honest gradients")
+    for vector in [grad_avg] if grad_att is None else [grad_avg, grad_att]:
+      _engine._check_like_rows(vector, prep, "grad_avg and grad_att")
+    device, d, stream = prep.device, prep.d, prep.stream
+    self.device, self.evals = device, evals
+    self.byz = torch.empty(d, dtype=torch.float32, device=device)
+    self.out = torch.empty(d, dtype=torch.float32, device=device)
+    self.record = torch.zeros(2 * evals + 2, dtype=torch.float64, device=device)
+    self._state = torch.zeros(_lib.SEARCH_STATE_BYTES // 8, dtype=torch.float64, device=device)
+    self.scores = torch.zeros(world, dtype=torch.float64, device=device)
+    self.score = self.scores[:1] if world == 1 else torch.zeros(1, dtype=torch.float64, device=device)
+    inputs = honest + [self.byz] * f_real
+    rows = _engine._prepare_device(inputs)
+    ws = self._ws = _engine._workspace(device, stream)
+    lib = _lib.lib()
+    state, out, avg = self._state.data_ptr(), self.out.data_ptr(), grad_avg.data_ptr()
+    att = None if grad_att is None else grad_att.data_ptr()
+    self._candidates = [(lib.bz_search_candidate, (avg, att, self.byz.data_ptr(), d, state, which, int(bool(negative)),
+                                                   _engine._SEARCH_KINDS[kind], stream))
+                        for which in (_lib.CANDIDATE_FIRST, _lib.CANDIDATE_NEXT, _lib.CANDIDATE_FINAL)]
+    self._score = (lib.bz_search_score_partial, (out, avg, d, state, self.score.data_ptr(), ws.data_ptr(), ws.numel(), stream))
+    self._stream = stream
+    self.distance = gar in DISTANCE_BASED
+    eval_status = None
+    self._pair = False
+    if not self.distance:
+      self._coordinate = _engine._coordinate_call(gar, rows, f_decl, out)
+    else:
+      rule = self._rule = _engine._rule(gar, n, f_decl)
+      width = n * n if rule.pair else n
+      self.blocks = torch.zeros((world, width), dtype=torch.float64, device=device)
+      self.part = self.blocks[0] if world == 1 else torch.zeros(width, dtype=torch.float64, device=device)
+      self._meta = torch.zeros(n + 1, dtype=torch.int32, device=device)      # order[n] + status
+      meta = self._meta.data_ptr()
+      status = meta + 4 * n if rule.status else None
+      eval_status = None if rule.gar == "krum" else status
+      part = self.part.data_ptr()
+      self._pair = rule.pair
+      if rule.pair:
+        # the honest rows keep their place in the table from one evaluation to the next, the candidate row
+        # (one tensor f_real times, new content) is new at every evaluation; an empty shard's rows are all
+        # distinct, as bz_pairdist_partial_reuse counts them
+        first = {}
+        to_unique = [first.setdefault(g.data_ptr() if d > 0 else i, len(first)) for i, g in enumerate(inputs)]
+        u = len(first)
+        old_index = (ctypes.c_int32 * n)(*[to_unique[i] if i < len(honest) else -1 for i in range(n)])
+        self._tables = torch.empty((2, _CACHE_DOUBLES), dtype=torch.float64, device=device)
+        self._mode = ctypes.c_int(-1)
+        tables = [t.data_ptr() for t in self._tables]
+        def phase_a(cache_in, cache_out):
+          reuse = (old_index, cache_in, u) if cache_in is not None else (None, None, 0)
+          return lib.bz_pairdist_partial_reuse, (rows.ptrs, n, d, part) + reuse + (cache_out, ctypes.byref(self._mode),
+                                                                                  ws.data_ptr(), ws.numel(), stream)
+        # [k % 2][reuse]: evaluation k writes table k % 2, reading table (k - 1) % 2
+        self._phase_a = [[phase_a(None, tables[s]), phase_a(tables[1 - s], tables[s])] for s in (0, 1)]
+      else:
+        # aksel: the local coordinate-wise median is the centre; it goes to `out`, which the reduce rewrites (bz_aksel's order)
+        self._median = _engine._coordinate_call("median", rows, None, out) if rule.center else None
+        self._phase_a = _engine._partial_call(rows, False, out if rule.center else None, part, ws)
+      self._select = _engine._select_call(rule, self.blocks, meta, stream)
+      self._reduce = _engine._reduce_call(rows, rule, meta, status, out)
+    record = self.record.data_ptr()
+    self._steps = [(lib.bz_search_step, (self.scores.data_ptr(), world, state, record, eval_status, record + 8 * (2 * evals + 1),
+                                         k, evals, stream)) for k in range(evals)]
+  def evaluate(self, k):
+    call = _engine._call
+    with _engine._on(self.device):
+      call(*self._candidates[_lib.CANDIDATE_FIRST if k == 0 else _lib.CANDIDATE_NEXT])
+      if not self.distance:
+        call(*self._coordinate)
+        call(*self._score)
+        return self.score
+      if self._pair:
+        call(*self._phase_a[k % 2][int(k > 0 and self._mode.value >= 0)])
+      else:
+        if self._median is not None:
+          call(*self._median)
+        call(*self._phase_a)
+    return self.part
+  def conclude(self, blocks):
+    select = self._select if blocks is self.blocks else _engine._select_call(self._rule, blocks, self._meta.data_ptr(), self._stream)
+    with _engine._on(self.device):
+      _engine._call(*select)
+      _engine._call(*self._reduce)
+      _engine._call(*self._score)
+    return self.score
+  def step(self, k, scores):
+    fn, args = self._steps[k]
+    if scores is not self.scores:
+      args = (scores.data_ptr(), scores.numel()) + args[2:]
+    _engine._run(self.device, fn, args)
+  def finish(self):
+    _engine._run(self.device, *self._candidates[_lib.CANDIDATE_FINAL])
+    return self.byz
+
+class ShardedLineSearch:
+  """ The attacks' line search (`engine.LineSearch`: `line_maximize(eval_factor, evals)` of the identical-family
+  attacks or of empire-strict against the rule `gar` with its defaults and f = f_decl) on a d-sharded
+  trainer.  Every rank passes its columns of the honest rows, of `grad_avg` and of `grad_att`; a score is
+  a sum over all d columns, so each evaluation is, on every rank:
+    1. the candidate row of the current factor (this rank's columns);
+    2. the rule on honest + [byz] * f_real: coordinate-wise rules locally, with no exchange; Multi-Krum,
+       Bulyan and brute: phase A with distance reuse (only the candidate's pairs after the first
+       evaluation), ONE `all_gather_into_tensor` of the n x n blocks, phases B and C; Aksel (its local
+       median) and CGE: the row distances, one all-gather of n doubles, phases B and C;
+    3. this rank's fp64 share of the score, one all-gather of R doubles;
+    4. the transition: y = fl32 of the R shares added in rank order, then the next factor, bitwise the
+       same on every rank.
+  A last candidate writes this rank's shard of the Byzantine gradient (`byz`) for the chosen factor.
+  `evals` is fixed in advance, so every rank issues the same launches and collectives and no host-side
+  decision is shared; a rank with an empty shard joins every collective.  On one rank there is no
+  collective, and the trace, the factor, `byz` and the rule's last output are those of `engine.LineSearch`.
+  Like `ShardedPlan`, `search()` only issues the work on the stream that was current at construction (no
+  allocation, no synchronisation), and holds what it reads and writes; `result()` reads `record` once.
+
+  The caller forms the shard of the attack direction: for `little` and `empire` the columns of the
+  full-vector direction; for `bulyan` (a one-hot vector at `target_idx`) that column lies on exactly one
+  rank (shard_bounds), every other rank's shard of it is zero.
+
+  Each evaluation's work between two exchanges is one stage method (`evaluate`, `conclude`, `step`,
+  `finish`), so that `search()` is those stages plus the collectives.  `backend`, for tests, provides
+  `search_shard(gar, grad_honests, f_real, f_decl, grad_avg, grad_att, evals, negative, kind, world)`, an
+  object with the stages (default: the CUDA library). """
+  def __init__(self, gar, grad_honests, f_real, f_decl, grad_avg, grad_att, evals, negative=False, kind="identical",
+               group=None, backend=None):
+    if gar not in _engine._SEARCH_RULES:
+      raise KeyError(f"unknown aggregation rule {gar!r}")
+    if kind not in _engine._SEARCH_KINDS:
+      raise ValueError(f"unknown attack kind {kind!r}, expected one of {sorted(_engine._SEARCH_KINDS)}")
+    if int(evals) < 1:
+      raise ValueError(f"evals = {evals}, expected evals >= 1")
+    self.gar, self.evals, self.group = gar, int(evals), group
+    self.world = dist.get_world_size(group) if dist.is_initialized() else 1
+    make = _SearchShard if backend is None else backend.search_shard
+    self._shard = make(gar, grad_honests, f_real, f_decl, grad_avg, grad_att, self.evals, negative, kind, self.world)
+    self.byz, self.record = self._shard.byz, self._shard.record
+  def evaluate(self, k):
+    """ Evaluation k up to its first exchange: the candidate row, then the rule's phase A (distance rules:
+    returns this rank's partial block) or the whole rule and the score share (coordinate-wise rules:
+    returns the share). """
+    return self._shard.evaluate(k)
+  def conclude(self, blocks):
+    """ Distance rules, between the two exchanges: phases B and C on the [R, ...] gathered blocks, then the
+    score share (returned). """
+    return self._shard.conclude(blocks)
+  def step(self, k, scores):
+    """ The transition of evaluation k from the [R] gathered score shares. """
+    self._shard.step(k, scores)
+  def finish(self):
+    """ The Byzantine gradient's shard for the chosen factor (returned). """
+    return self._shard.finish()
+  def _exchange(self, gathered, part):
+    if self.world > 1:
+      dist.all_gather_into_tensor(gathered.view(-1), part, group=self.group)
+    return gathered
+  def __call__(self):
+    shard = self._shard
+    for k in range(self.evals):
+      part = self.evaluate(k)
+      if shard.distance:
+        part = self.conclude(self._exchange(shard.blocks, part))
+      self.step(k, self._exchange(shard.scores, part))
+    return self.finish()
+  def result(self):
+    """ (factor, trace) from ONE device->host read, the same on every rank; with `engine.config.strict_status`,
+    a failed evaluation of Bulyan or brute raises what the plain call raises. """
+    return _engine._search_outcome(self.record, self.evals)
+
+def line_search(gar, grad_honests, f_real, f_decl, grad_avg, grad_att, evals, negative=False, kind="identical", group=None):
+  """ `engine.line_search` on a d-sharded trainer (see `ShardedLineSearch`): returns (factor, this rank's
+  shard of the Byzantine gradient), the factor the same Python float on every rank. """
+  search = ShardedLineSearch(gar, grad_honests, f_real, f_decl, grad_avg, grad_att, evals, negative, kind, group)
+  byz = search()
+  factor, _ = search.result()
+  return factor, byz
 
 def aggregate(gar, gradients, f=None, m=None, mode="mid", group=None, backend=None, return_selection=False):
   """ Aggregate this rank's shard.

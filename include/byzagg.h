@@ -277,4 +277,8 @@ BZ_API int bz_gradient_row(const float* grad, int64_t d, double clip, float* sam
  * next factor enqueued back to back, one host read for the outcome. */
 #include "byzagg_attack.h"
 
+/* The same search on a d-sharded trainer: each evaluation cut at its exchanges (the rule's partial block,
+ * the score's R shares), which the caller all-gathers; every rank then takes the same next factor. */
+#include "byzagg_search_shards.h"
+
 #endif /* BYZAGG_H */
