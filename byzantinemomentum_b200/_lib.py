@@ -1,6 +1,6 @@
 # coding: utf-8
 """ctypes binding of `libbyzagg.so` (C ABI: `include/byzagg.h`, `include/byzagg_shards.h`,
-`include/byzagg_attack.h` and `include/byzagg_search_shards.h`).
+`include/byzagg_attack.h`, `include/byzagg_search_shards.h` and `include/byzagg_search_peers.h`).
 
 The library is loaded lazily, on the first call that needs it, and the load FAILS LOUDLY:
 there is no CPU or PyTorch fallback anywhere in this package.  Build it in-tree with
@@ -97,6 +97,13 @@ SEARCH_SHARD_SIGNATURES = {
   "bz_search_score_partial": (_i, [_vp, _vp, _i64, _vp, _vp, _vp, _sz, _vp]),
   "bz_search_step": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _i, _i, _vp]),
 }
+# the same for include/byzagg_search_peers.h (that search with its exchanges over peer memory)
+SEARCH_PEER_SIGNATURES = {
+  "bz_pairdist_reuse_peers": (_i, [_i, _c_rows, _i, _i, _i, _i64, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _i, _i, _c_rows, _c_rows,
+                                   ctypes.c_uint, _vp, _sz, _vp]),
+  "bz_rowdist_peers": (_i, [_i, _c_rows, _i, _i, _i, _vp, _i64, _vp, _vp, _vp, _i, _i, _c_rows, _c_rows, ctypes.c_uint, _vp, _sz, _vp]),
+  "bz_search_score_peers": (_i, [_vp, _vp, _i64, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _c_rows, _c_rows, ctypes.c_uint, _vp, _sz, _vp]),
+}
 SEARCH_STATE_BYTES = 64                     # BZ_SEARCH_STATE_BYTES
 CANDIDATE_FIRST, CANDIDATE_NEXT, CANDIDATE_FINAL = 0, 1, 2
 
@@ -118,7 +125,7 @@ def lib():
         handle = ctypes.CDLL(str(path))
       except OSError as err:
         raise LibraryError(f"unable to load {path}: {err}") from err
-      tables = (SIGNATURES, SHARD_SIGNATURES, ATTACK_SIGNATURES, SEARCH_SHARD_SIGNATURES)
+      tables = (SIGNATURES, SHARD_SIGNATURES, ATTACK_SIGNATURES, SEARCH_SHARD_SIGNATURES, SEARCH_PEER_SIGNATURES)
       for name, (restype, argtypes) in [item for table in tables for item in table.items()]:
         try:
           fn = getattr(handle, name)

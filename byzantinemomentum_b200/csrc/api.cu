@@ -283,3 +283,4 @@ int bz_coordinate_host(int rule, const float* const* host_rows, int n, int f, in
 #include "api_dist.inc"
 #include "api_search.inc"
 #include "api_search_shards.inc"
+#include "api_search_peers.inc"

@@ -82,6 +82,24 @@ int launch_rowdist(const RowTable& rows, int n, const float* const* host_rows, c
                    double* parts, cudaStream_t st, int reverse = 0, int32_t* order = nullptr, unsigned* ticket = nullptr,
                    int sqrt_norm = 0, int dot = 0);
 
+// The exchange of K2''s last CTA over peer memory (bz_rowdist_peers, bz_search_score_peers; protocol in
+// peers.cuh): this rank's fp64 block (n doubles, or the one score share) goes to block[rank], the flags of
+// `epoch` are raised and awaited, and the R blocks are added in rank order, ((p0 + p1) + p2) + ...
+struct PeerTail {
+  int nranks, rank;
+  unsigned epoch;
+  int32_t* status;                 // rowdist: 0, or BZ_STATUS_PEER_TIMEOUT; search: the search's status word,
+                                   // set to BZ_STATUS_PEER_TIMEOUT on a timeout after the transition
+  double* block[BZ_MAX_PEERS];     // this step's slot on every rank ([rank] is local)
+  unsigned* flag[BZ_MAX_PEERS];    // this step's flag array (nranks words) on every rank
+};
+// K2' over the rows against `center` (NULL: the origin) in bz_rowdist_partial's geometry, its last CTA
+// summing the blocks in k_reduce_parts's order (the block the collective path all-gathers), exchanging
+// it, and writing the stable order of the n keys (sqrt_norm as in bz_rowdist_select).  Any d >= 0.
+int launch_rowdist_peers(const RowTable& rows, int n, const float* const* host_rows, const float* center, int64_t d,
+                         double* parts, cudaStream_t st, int32_t* order, unsigned* ticket, int sqrt_norm,
+                         const PeerTail& peers);
+
 // ---- The attacks' line search (bz_line_search, api_search.inc) -------------------------------------
 // State of `line_maximize` (tools/misc.py:468-513) in device memory, carried from one evaluation to the next.
 struct SearchState {
@@ -101,9 +119,10 @@ struct SearchTail {
                                // of running the transition (bz_search_step adds the ranks' sums first)
 };
 // K2' over the one row `out` against `center`, chained by PDL after the rule, its last CTA rounding the
-// sum to fp32 (y) and running one transition of the search.
+// sum to fp32 (y) and running one transition of the search.  `peers` (d-sharded search, any d >= 0): the
+// share is exchanged first and y is fl32 of the R shares added in rank order, as in K9.
 int launch_rowdist_search(const float* out, const float* center, int64_t d, double* parts, const SearchTail& tail,
-                          cudaStream_t st);
+                          cudaStream_t st, const PeerTail* peers = nullptr);
 // K8 (k8_candidate.cu): byz <- the candidate row of x (which: 0 = start 0.0, also resets the state's ticket;
 // 1 = state->next_x; 2 = state->best_x, the attack's result), chained by PDL.
 int launch_candidate(const float* avg, const float* att, float* byz, int64_t d, SearchState* state, int which,
@@ -121,7 +140,9 @@ void launch_study(const RowTable& rows, int n, const float* const* host_rows, in
 
 // Sum `nparts` blocks of `len` doubles in index order into `block` (fixed order: deterministic).
 // pair_n > 0: the block is a pair_n x pair_n table of which only entries i < j are defined; the
-// others are written as 0.
+// others are written as 0.  The order: class w = the blocks p = w mod kReduceWarps, each summed in p
+// order from 0.0, then the class sums in class order from 0.0 (K2' in peers mode sums its blocks so too).
+constexpr int kReduceWarps = 8;
 void launch_reduce_parts(const double* parts, int nparts, int len, int pair_n, double* block, cudaStream_t st);
 
 // C(n, n - f), saturating at 2^64 - 1.

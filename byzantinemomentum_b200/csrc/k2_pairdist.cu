@@ -194,7 +194,6 @@ k2_pairdist(const __grid_constant__ RowTable rows, const int n, const int T, con
 // ---- fixed-order reduction of partial blocks --------------------------------------------------
 // One CTA per 32 entries; warp w adds the blocks p = w, w + 8, ... (coalesced 256-byte rows of
 // 32 entries), the 8 warp sums are then added in warp order: a fixed order, whatever the grid.
-constexpr int kReduceWarps = 8;
 __global__ void __launch_bounds__(kReduceWarps * 32)
 k_reduce_parts(const double* __restrict__ parts, int nparts, int len, int pair_n, double* __restrict__ block) {
   __shared__ double partial[kReduceWarps][32];

@@ -29,6 +29,7 @@
 #include "dist.cuh"
 #include "k5_device.cuh"
 #include "launch.cuh"
+#include "peers.cuh"
 #include "reduce.cuh"
 #include "tma.cuh"
 
@@ -81,31 +82,15 @@ struct RingTail {
   int u_old;
   signed char old_index[kMaxN];
   // Exchange fused into this launch (d-sharded path, one process per GPU): the last CTA writes the rank's
-  // reduced block into its slot of a buffer mapped on every GPU (peer memory over NVLink), raises its flag
-  // in every peer's flag array, waits for the peers' flags, then adds the R blocks IN PLACE from the R GPUs
-  // (plain loads on peer addresses, rank order: bitwise the same table on every rank) and scores.
+  // reduced block (from its own table, reuse included) into its slot of a buffer mapped on every GPU (peer
+  // memory over NVLink), raises its flag in every peer's flag array, waits for the peers' flags, then adds
+  // the R blocks IN PLACE from the R GPUs (plain loads on peer addresses, rank order: bitwise the same
+  // table on every rank) and scores.
   int nranks, rank;                       // nranks == 0: single GPU
   unsigned epoch;                         // step number, > the previous step's
   double* peer_block[BZ_MAX_PEERS];       // this step's slot on every rank ([rank] is local)
   unsigned* peer_flag[BZ_MAX_PEERS];      // this step's flag array (nranks words) on every rank
 };
-
-__device__ __forceinline__ void st_release_sys(unsigned* p, unsigned v) {
-  asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
-__device__ __forceinline__ unsigned ld_acquire_sys(const unsigned* p) {
-  unsigned v;
-  asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-}
-// Coherent at system scope, never from a stale L1 line (the slot is rewritten every other step); NOT
-// `volatile` asm, so that the R loads of a table entry are issued together (a volatile load per rank made
-// the entry cost R NVLink round trips).
-__device__ __forceinline__ double ld_relaxed_sys_f64(const double* p) {
-  double v;
-  asm("ld.relaxed.sys.global.f64 %0, [%1];" : "=d"(v) : "l"(p));
-  return v;
-}
 
 // New rows of a reuse call: star task = one new row against 25 consecutive rows.
 constexpr int kStarMax = 4;
@@ -609,31 +594,42 @@ k2_ring(const __grid_constant__ RowTable rows, const __grid_constant__ SelfList 
             // pair of their distinct rows (the alias flag when both are one tensor), every other entry 0.
             // That layout is the same on every rank whatever its rows alias — a rank with an empty shard
             // cannot tell, an empty tensor has no address — and holds nothing the workspace left behind.
+            // This rank's u x u table first, as the plain pass below builds it (reuse included), kept in
+            // `cache_out` when asked: this rank's own pairs, which the next call's star pass reuses.
             const int NN = N * N;
+            double* local = sm + NN;            // behind the N x N table the exchange sums into
+            for (int e = threadIdx.x; e < len; e += kThreads) {
+              const int i = e / n, j = e - i * n;
+              double v = 0.;
+              if (i <= j) {
+                const int oi = tail.old_index[i], oj = tail.old_index[j];
+                if (i < j && tail.cache_in != nullptr && oi >= 0 && oj >= 0) {
+                  v = __ldcg(tail.cache_in + (size_t)min(oi, oj) * tail.u_old + max(oi, oj));
+                } else {
+                  for (int g = 0; g < ngroups; ++g) v += __ldcg(gblocks + (size_t)g * len + e);
+                }
+              }
+              local[e] = v;
+              if (tail.cache_out != nullptr) tail.cache_out[e] = v;
+            }
+            __syncthreads();
             double* mine = tail.peer_block[tail.rank];
             for (int e = threadIdx.x; e < NN; e += kThreads) {
               const int i = e / N, j = e - i * N;
               double v = 0.;
               if (i < j) {
                 const int a = map.to_unique[i], b = map.to_unique[j];
-                const size_t k = (size_t)min(a, b) * n + max(a, b);
-                for (int g = 0; g < ngroups; ++g) v += __ldcg(gblocks + (size_t)g * len + k);
+                v = local[min(a, b) * n + max(a, b)];
               }
               mine[e] = v;
             }
             map.u = N;                          // the summed table below is N x N already
             __threadfence_system();
             __syncthreads();
-            if ((int)threadIdx.x < tail.nranks) {
-              st_release_sys(tail.peer_flag[threadIdx.x] + tail.rank, tail.epoch);       // "rank's block of step `epoch` is there"
-              const unsigned* wait_on = tail.peer_flag[tail.rank] + threadIdx.x;
-              // bounded wait (~2 s): a peer that never shows up must not hang the GPU; the status word says so
-              unsigned spins = 0;
-              while ((int)(ld_acquire_sys(wait_on) - tail.epoch) < 0) {
-                __nanosleep(100);
-                if (++spins > (1u << 24)) { peer_timeout = 1; break; }
-              }
-            }
+            // flag, bounded wait (peers.cuh): a peer that never shows up sets the status word
+            if ((int)threadIdx.x < tail.nranks &&
+                peer_signal_wait(tail.peer_flag[threadIdx.x] + tail.rank, tail.peer_flag[tail.rank] + threadIdx.x, tail.epoch))
+              peer_timeout = 1;
             __syncthreads();
             asm volatile("" ::: "memory");      // the block loads below stay below the flag wait
             for (int e = threadIdx.x; e < NN; e += kThreads) {

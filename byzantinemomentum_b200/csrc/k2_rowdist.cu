@@ -13,6 +13,7 @@
 #include "dist.cuh"
 #include "k5_device.cuh"
 #include "launch.cuh"
+#include "peers.cuh"
 #include "reduce.cuh"
 #include "search.cuh"
 
@@ -28,11 +29,14 @@ constexpr int kRdFlush = 8;      // vectors between two flushes
 // SEARCH: the score of the attacks' line search (one row, `search` set): launched by PDL after the rule,
 // the last CTA rounds the sum to fp32 and runs `search_step` (search.cuh) instead of the selection, or,
 // with `search.partial` set (one rank of the d-sharded search), writes the fp64 sum there unrounded.
-template <bool CENTER, int VEC, bool DOT = false, bool SEARCH = false>
-__global__ void __launch_bounds__(kRdThreads, 2)
-k2_rowdist(const __grid_constant__ RowTable rows, const int n, const float* __restrict__ center, const Geom g,
-           double* __restrict__ parts, int32_t* __restrict__ order, unsigned* __restrict__ ticket, const int sqrt_norm,
-           const SearchTail search) {
+// PEERS (kernel k2_rowdist_peers): the last CTA exchanges its sum over peer memory first (`peers`,
+// PeerTail): the selection, or the transition, then runs on the R ranks' sums added in rank order,
+// bitwise the same on every rank.
+template <bool CENTER, int VEC, bool DOT, bool SEARCH, bool PEERS>
+__device__ __forceinline__ void
+rowdist_body(const RowTable& rows, const int n, const float* __restrict__ center, const Geom g,
+             double* __restrict__ parts, int32_t* __restrict__ order, unsigned* __restrict__ ticket, const int sqrt_norm,
+             const SearchTail search, const PeerTail& peers) {
   __shared__ double warp_tot[kRdWarps][kMaxN];
   if (SEARCH) pdl_wait();      // the rule's output is valid from here
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -119,33 +123,65 @@ k2_rowdist(const __grid_constant__ RowTable rows, const int n, const float* __re
   // finish instead of a single-CTA launch: blocks summed in S interleaved classes with every load in
   // flight, class sums added in class order (fixed for a given grid), keys as in k5_rowdist_select.
   __shared__ bool last;
+  __shared__ int peer_timeout;
   __threadfence();
   __syncthreads();
   if (threadIdx.x == 0) last = atomicAdd(ticket, 1u) == gridDim.x - 1;
   __syncthreads();
   if (!last) return;
   __threadfence();
-  double* partial = &warp_tot[0][0];                // S * n <= 256 doubles
+  double* partial = &warp_tot[0][0];                // S * n <= 256 doubles (PEERS: kReduceWarps * n <= 512)
   double* key = partial + kRdThreads;               // n <= 64 doubles behind them (the table holds 512)
-  const int S = kRdThreads / n;
-  const int c = threadIdx.x % n, cls = threadIdx.x / n;
-  if (cls < S) {
-    double sum = 0.;
-    int p = cls;
-    for (; p + 7 * S < (int)gridDim.x; p += 8 * S) {
-      double t[8];
-#pragma unroll
-      for (int u = 0; u < 8; ++u) t[u] = __ldcg(parts + (size_t)(p + u * S) * n + c);
-#pragma unroll
-      for (int u = 0; u < 8; ++u) sum += t[u];
+  double sum = 0.;                                  // thread c < n: the sum of entry c over the blocks
+  if (PEERS && !SEARCH) {
+    // the block bz_rowdist_partial gives (k_reduce_parts's order), so that every rank publishes what the
+    // collective path all-gathers
+    for (int idx = threadIdx.x; idx < kReduceWarps * n; idx += kRdThreads) {
+      const int w = idx / n, c = idx - w * n;
+      double s = 0.;
+      for (int p = w; p < (int)gridDim.x; p += kReduceWarps) s += __ldcg(parts + (size_t)p * n + c);
+      partial[idx] = s;
     }
-    for (; p < (int)gridDim.x; p += S) sum += __ldcg(parts + (size_t)p * n + c);
-    partial[cls * n + c] = sum;
+    __syncthreads();
+    if (threadIdx.x < n)
+      for (int w = 0; w < kReduceWarps; ++w) sum += partial[w * n + threadIdx.x];
+  } else {
+    const int S = kRdThreads / n;
+    const int c = threadIdx.x % n, cls = threadIdx.x / n;
+    if (cls < S) {
+      double s = 0.;
+      int p = cls;
+      for (; p + 7 * S < (int)gridDim.x; p += 8 * S) {
+        double t[8];
+#pragma unroll
+        for (int u = 0; u < 8; ++u) t[u] = __ldcg(parts + (size_t)(p + u * S) * n + c);
+#pragma unroll
+        for (int u = 0; u < 8; ++u) s += t[u];
+      }
+      for (; p < (int)gridDim.x; p += S) s += __ldcg(parts + (size_t)p * n + c);
+      partial[cls * n + c] = s;
+    }
+    __syncthreads();
+    if (threadIdx.x < n)
+      for (int k = 0; k < S; ++k) sum += partial[k * n + threadIdx.x];
   }
-  __syncthreads();
+  if (PEERS) {
+    // publish, flag, wait (peers.cuh), then ((p0 + p1) + p2) + ... over the R ranks
+    if (threadIdx.x == 0) peer_timeout = 0;
+    if (threadIdx.x < n) peers.block[peers.rank][threadIdx.x] = sum;
+    __threadfence_system();
+    __syncthreads();
+    if ((int)threadIdx.x < peers.nranks &&
+        peer_signal_wait(peers.flag[threadIdx.x] + peers.rank, peers.flag[peers.rank] + threadIdx.x, peers.epoch))
+      peer_timeout = 1;
+    __syncthreads();
+    asm volatile("" ::: "memory");      // the block loads below stay below the flag wait
+    if (threadIdx.x < n) {
+      sum = ld_relaxed_sys_f64(peers.block[0] + threadIdx.x);
+      for (int r = 1; r < peers.nranks; ++r) sum += ld_relaxed_sys_f64(peers.block[r] + threadIdx.x);
+    }
+  }
   if (threadIdx.x < n) {
-    double sum = 0.;
-    for (int k = 0; k < S; ++k) sum += partial[k * n + threadIdx.x];
     double v;
     if (sqrt_norm) {
       v = (double)fp32_norm(sum);                    // cge.py:36-37: fp32 norm, non-finite -> +inf
@@ -160,52 +196,96 @@ k2_rowdist(const __grid_constant__ RowTable rows, const int n, const float* __re
     }
     key[threadIdx.x] = v;
   }
+  // the status word after the transition, which rewrites the search's
+  if (PEERS && threadIdx.x == 0 && peers.status != nullptr && (peer_timeout || !SEARCH))
+    *peers.status = peer_timeout ? BZ_STATUS_PEER_TIMEOUT : BZ_STATUS_OK;
   if (SEARCH) return;
   __syncthreads();
   stable_order(key, n, order);
   if (threadIdx.x == 0) *ticket = 0u;
 }
 
+template <bool CENTER, int VEC, bool DOT = false, bool SEARCH = false>
+__global__ void __launch_bounds__(kRdThreads, 2)
+k2_rowdist(const __grid_constant__ RowTable rows, const int n, const float* __restrict__ center, const Geom g,
+           double* __restrict__ parts, int32_t* __restrict__ order, unsigned* __restrict__ ticket, const int sqrt_norm,
+           const SearchTail search) {
+  rowdist_body<CENTER, VEC, DOT, SEARCH, false>(rows, n, center, g, parts, order, ticket, sqrt_norm, search, PeerTail{});
+}
+
+template <bool CENTER, int VEC, bool SEARCH>
+__global__ void __launch_bounds__(kRdThreads, 2)
+k2_rowdist_peers(const __grid_constant__ RowTable rows, const int n, const float* __restrict__ center, const Geom g,
+                 double* __restrict__ parts, int32_t* __restrict__ order, unsigned* __restrict__ ticket, const int sqrt_norm,
+                 const SearchTail search, const __grid_constant__ PeerTail peers) {
+  rowdist_body<CENTER, VEC, false, SEARCH, true>(rows, n, center, g, parts, order, ticket, sqrt_norm, search, peers);
+}
+
+// Blocks of a K2' launch over the vectors of g: up to two per SM, at least one (an empty shard too).
+static unsigned rowdist_grid(const Geom& g) {
+  int64_t grid = (g.nv + kRdThreads - 1) / kRdThreads;
+  const int64_t cap = (int64_t)sm_count() * 2;
+  if (grid > cap) grid = cap;
+  if (grid > kMaxParts) grid = kMaxParts;
+  if (grid < 1) grid = 1;
+  return (unsigned)grid;
+}
 
 int launch_rowdist(const RowTable& rows, int n, const float* const* host_rows, const float* center, int64_t d,
                    double* parts, cudaStream_t st, int reverse, int32_t* order, unsigned* ticket, int sqrt_norm, int dot) {
   // The centre doubles as the alignment reference ("out") of the geometry
   Geom g = make_geom(host_rows, n, center ? (const void*)center : (const void*)host_rows[0], nullptr, d, 4);
   g.reverse = reverse;
-  int64_t grid = (g.nv + kRdThreads - 1) / kRdThreads;
-  const int64_t cap = (int64_t)sm_count() * 2;
-  if (grid > cap) grid = cap;
-  if (grid > kMaxParts) grid = kMaxParts;
-  if (grid < 1) grid = 1;
+  const unsigned grid = rowdist_grid(g);
   if (dot && center != nullptr) {
-    if (g.vec == 4) k2_rowdist<true, 4, true><<<(unsigned)grid, kRdThreads, 0, st>>>(rows, n, center, g, parts, nullptr, nullptr, 0, SearchTail{});
-    else            k2_rowdist<true, 1, true><<<(unsigned)grid, kRdThreads, 0, st>>>(rows, n, center, g, parts, nullptr, nullptr, 0, SearchTail{});
+    if (g.vec == 4) k2_rowdist<true, 4, true><<<grid, kRdThreads, 0, st>>>(rows, n, center, g, parts, nullptr, nullptr, 0, SearchTail{});
+    else            k2_rowdist<true, 1, true><<<grid, kRdThreads, 0, st>>>(rows, n, center, g, parts, nullptr, nullptr, 0, SearchTail{});
     return (int)grid;
   }
   if (order != nullptr) cudaMemsetAsync(ticket, 0, sizeof(unsigned), st);
   if (g.vec == 4) {
-    if (center) k2_rowdist<true, 4><<<(unsigned)grid, kRdThreads, 0, st>>>(rows, n, center, g, parts, order, ticket, sqrt_norm, SearchTail{});
-    else        k2_rowdist<false, 4><<<(unsigned)grid, kRdThreads, 0, st>>>(rows, n, center, g, parts, order, ticket, sqrt_norm, SearchTail{});
+    if (center) k2_rowdist<true, 4><<<grid, kRdThreads, 0, st>>>(rows, n, center, g, parts, order, ticket, sqrt_norm, SearchTail{});
+    else        k2_rowdist<false, 4><<<grid, kRdThreads, 0, st>>>(rows, n, center, g, parts, order, ticket, sqrt_norm, SearchTail{});
   } else {
-    if (center) k2_rowdist<true, 1><<<(unsigned)grid, kRdThreads, 0, st>>>(rows, n, center, g, parts, order, ticket, sqrt_norm, SearchTail{});
-    else        k2_rowdist<false, 1><<<(unsigned)grid, kRdThreads, 0, st>>>(rows, n, center, g, parts, order, ticket, sqrt_norm, SearchTail{});
+    if (center) k2_rowdist<true, 1><<<grid, kRdThreads, 0, st>>>(rows, n, center, g, parts, order, ticket, sqrt_norm, SearchTail{});
+    else        k2_rowdist<false, 1><<<grid, kRdThreads, 0, st>>>(rows, n, center, g, parts, order, ticket, sqrt_norm, SearchTail{});
+  }
+  return (int)grid;
+}
+
+int launch_rowdist_peers(const RowTable& rows, int n, const float* const* host_rows, const float* center, int64_t d,
+                         double* parts, cudaStream_t st, int32_t* order, unsigned* ticket, int sqrt_norm,
+                         const PeerTail& peers) {
+  // bz_rowdist_partial's geometry (forward walk), so that the blocks are the collective path's
+  const Geom g = make_geom(host_rows, n, center ? (const void*)center : (const void*)host_rows[0], nullptr, d, 4);
+  const unsigned grid = rowdist_grid(g);
+  cudaMemsetAsync(ticket, 0, sizeof(unsigned), st);
+  const SearchTail none = {};
+  if (g.vec == 4) {
+    if (center) k2_rowdist_peers<true, 4, false><<<grid, kRdThreads, 0, st>>>(rows, n, center, g, parts, order, ticket, sqrt_norm, none, peers);
+    else        k2_rowdist_peers<false, 4, false><<<grid, kRdThreads, 0, st>>>(rows, n, center, g, parts, order, ticket, sqrt_norm, none, peers);
+  } else {
+    if (center) k2_rowdist_peers<true, 1, false><<<grid, kRdThreads, 0, st>>>(rows, n, center, g, parts, order, ticket, sqrt_norm, none, peers);
+    else        k2_rowdist_peers<false, 1, false><<<grid, kRdThreads, 0, st>>>(rows, n, center, g, parts, order, ticket, sqrt_norm, none, peers);
   }
   return (int)grid;
 }
 
 int launch_rowdist_search(const float* out, const float* center, int64_t d, double* parts, const SearchTail& tail,
-                          cudaStream_t st) {
+                          cudaStream_t st, const PeerTail* peers) {
   RowTable rows;
   for (int r = 0; r < kMaxN; ++r) rows.p[r] = out;
   const Geom g = make_geom(&out, 1, center, nullptr, d, 4);
-  int64_t grid = (g.nv + kRdThreads - 1) / kRdThreads;
-  const int64_t cap = (int64_t)sm_count() * 2;
-  if (grid > cap) grid = cap;
-  if (grid > kMaxParts) grid = kMaxParts;
-  if (grid < 1) grid = 1;
-  const cudaError_t err = g.vec == 4
-      ? launch_after(k2_rowdist<true, 4, false, true>, (unsigned)grid, kRdThreads, 0, st, rows, 1, center, g, parts, nullptr, nullptr, 0, tail)
-      : launch_after(k2_rowdist<true, 1, false, true>, (unsigned)grid, kRdThreads, 0, st, rows, 1, center, g, parts, nullptr, nullptr, 0, tail);
+  const unsigned grid = rowdist_grid(g);
+  cudaError_t err;
+  if (peers != nullptr)
+    err = g.vec == 4
+        ? launch_after(k2_rowdist_peers<true, 4, true>, grid, kRdThreads, 0, st, rows, 1, center, g, parts, nullptr, nullptr, 0, tail, *peers)
+        : launch_after(k2_rowdist_peers<true, 1, true>, grid, kRdThreads, 0, st, rows, 1, center, g, parts, nullptr, nullptr, 0, tail, *peers);
+  else
+    err = g.vec == 4
+        ? launch_after(k2_rowdist<true, 4, false, true>, grid, kRdThreads, 0, st, rows, 1, center, g, parts, nullptr, nullptr, 0, tail)
+        : launch_after(k2_rowdist<true, 1, false, true>, grid, kRdThreads, 0, st, rows, 1, center, g, parts, nullptr, nullptr, 0, tail);
   return err == cudaSuccess ? (int)grid : -1;
 }
 

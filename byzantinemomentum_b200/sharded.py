@@ -31,7 +31,7 @@ import torch.distributed as dist
 from . import _lib
 from . import engine as _engine
 
-__all__ = ["aggregate", "aggregate_p2p", "compute_avg_dev_max", "study_step", "replicate", "apply_update", "shard_bounds", "rows_aligned", "choose_exchange", "PeerExchange", "FusedExchange", "ShardedPlan", "GradientShards", "choose_delivery", "ShardedLineSearch", "line_search", "COORDINATE_WISE", "DISTANCE_BASED"]
+__all__ = ["aggregate", "aggregate_p2p", "compute_avg_dev_max", "study_step", "replicate", "apply_update", "shard_bounds", "rows_aligned", "choose_exchange", "choose_search_exchange", "PeerExchange", "FusedExchange", "ShardedPlan", "GradientShards", "choose_delivery", "ShardedLineSearch", "line_search", "COORDINATE_WISE", "DISTANCE_BASED"]
 
 COORDINATE_WISE = ("average", "median", "trmean", "phocas", "meamed")
 DISTANCE_BASED = _engine.DISTANCE_BASED
@@ -96,7 +96,11 @@ class FusedExchange:
   waits for the R flags, and adds the R blocks in place over NVLink — no barrier op, no collective, no
   separate selection kernel.  `epoch` (the step number) tells this step's flags from older ones; two
   slots make that enough (a rank rewrites slot s only after every peer has signalled the step in
-  between, i.e. finished reading s). """
+  between, i.e. finished reading s).
+  `ShardedLineSearch(exchange="fused")` runs its exchanges (the rule's block, the score's share) over the
+  same buffer: one per call here, each advancing `epoch` by one.  That relies on one condition: the calls
+  that share a FusedExchange (the search and the `ShardedPlan` of the same n) are issued on ONE stream, in
+  the same order on every rank. """
   FLAG_WORDS = 16
   def __init__(self, n, device, group=None):
     import torch.distributed._symmetric_memory as symm_mem
@@ -113,6 +117,15 @@ class FusedExchange:
     torch.cuda.synchronize(device)
     self.peer_base = [int(p) for p in self.handle.buffer_ptrs]
     self.epoch = 0
+  @classmethod
+  def local(cls, n, device):
+    """ The same layout on a plain device buffer, for one rank: no process group, no symmetric memory. """
+    fx = cls.__new__(cls)
+    fx.n, fx.device, fx.group, fx.world, fx.rank, fx.epoch = n, device, None, 1, 0, 0
+    fx.buffer = torch.zeros(2 * n * n + cls.FLAG_WORDS, dtype=torch.float64, device=device)
+    fx.handle = None
+    fx.peer_base = [fx.buffer.data_ptr()]
+    return fx
   def tables(self, slot):
     """ (ctypes array of the R block pointers, ctypes array of the R flag-array pointers) of a slot. """
     block = slot * self.n * self.n * 8
@@ -306,6 +319,29 @@ class ShardedPlan:
       call(*self._c)
     return self.out
 
+SEARCH_EXCHANGES = ("auto", "fused", "nccl")
+
+def choose_search_exchange(exchange, aligned, symmetric, engine, group=None):
+  """ The exchange of `ShardedLineSearch`, the same on every rank of `group`: the local facts — `aligned`:
+  this rank's rows suit the rule's fused call (16-byte aligned for Multi-Krum, Bulyan and brute, any for
+  the others); `symmetric`: symmetric memory can be set up here; `engine`: the CUDA library runs the
+  stages — are agreed on with one all-reduce (MIN), as in `choose_exchange`.  "auto" takes "fused" on 2 to
+  16 ranks that all have the facts, else "nccl" (one rank, or a stand-in backend, keeps the collective
+  path).  An explicit "fused" needs `aligned` on every rank, and symmetric memory on every one of at most
+  16 ranks unless there is one rank (its buffer is then plain device memory); otherwise it raises on every
+  rank.  Returns "fused" or "nccl". """
+  if exchange not in SEARCH_EXCHANGES:
+    raise ValueError(f"unknown exchange {exchange!r}")
+  world = dist.get_world_size(group) if dist.is_initialized() else 1
+  aligned, symmetric, engine = map(bool, _agree([int(bool(aligned)), int(bool(symmetric)), int(bool(engine))], group))
+  fusable = aligned and (world == 1 or (symmetric and world <= _lib.MAX_PEERS))
+  if exchange == "auto":
+    return "fused" if world > 1 and engine and fusable else "nccl"
+  if exchange == "fused" and not fusable:
+    raise ValueError(f"the fused exchange of the line search needs 16-byte aligned rows for krum / bulyan / brute on every rank, "
+                     f"and symmetric memory on every one of at most {_lib.MAX_PEERS} ranks")
+  return exchange
+
 DELIVERIES = ("auto", "p2p", "collective")
 
 def choose_delivery(exchange, symmetric, group=None):
@@ -476,7 +512,8 @@ class _SearchShard:
   """ One rank's device side of `ShardedLineSearch`: the calls of every stage resolved once (row pointers,
   buffers, workspace, the current stream at construction), for `world` ranks.
     blocks, part   [world, width] gathered partial blocks of the rule / this rank's block (blocks[0] on one rank)
-    scores, score  [world] gathered score shares / this rank's share (scores[:1] on one rank) """
+    scores, score  [world] gathered score shares / this rank's share (scores[:1] on one rank)
+  `fuse(fx)` prepares the stages of the fused exchange over the FusedExchange `fx` as well. """
   def __init__(self, gar, grad_honests, f_real, f_decl, grad_avg, grad_att, evals, negative, kind, world):
     honest = list(grad_honests)
     f_real = int(f_real)
@@ -497,10 +534,11 @@ class _SearchShard:
     self.scores = torch.zeros(world, dtype=torch.float64, device=device)
     self.score = self.scores[:1] if world == 1 else torch.zeros(1, dtype=torch.float64, device=device)
     inputs = honest + [self.byz] * f_real
-    rows = _engine._prepare_device(inputs)
+    rows = self._rows = _engine._prepare_device(inputs)
     ws = self._ws = _engine._workspace(device, stream)
     lib = _lib.lib()
     state, out, avg = self._state.data_ptr(), self.out.data_ptr(), grad_avg.data_ptr()
+    self._avg = avg
     att = None if grad_att is None else grad_att.data_ptr()
     self._candidates = [(lib.bz_search_candidate, (avg, att, self.byz.data_ptr(), d, state, which, int(bool(negative)),
                                                    _engine._SEARCH_KINDS[kind], stream))
@@ -534,12 +572,13 @@ class _SearchShard:
         self._tables = torch.empty((2, _CACHE_DOUBLES), dtype=torch.float64, device=device)
         self._mode = ctypes.c_int(-1)
         tables = [t.data_ptr() for t in self._tables]
-        def phase_a(cache_in, cache_out):
-          reuse = (old_index, cache_in, u) if cache_in is not None else (None, None, 0)
-          return lib.bz_pairdist_partial_reuse, (rows.ptrs, n, d, part) + reuse + (cache_out, ctypes.byref(self._mode),
-                                                                                  ws.data_ptr(), ws.numel(), stream)
-        # [k % 2][reuse]: evaluation k writes table k % 2, reading table (k - 1) % 2
-        self._phase_a = [[phase_a(None, tables[s]), phase_a(tables[1 - s], tables[s])] for s in (0, 1)]
+        # the reuse arguments of evaluation k writing table k % 2, after one reading table (k - 1) % 2 or not
+        self._reuse = [[((old_index, tables[1 - s], u) if reused else (None, None, 0)) + (tables[s], ctypes.byref(self._mode))
+                        for reused in (False, True)] for s in (0, 1)]
+        def phase_a(reuse):
+          return lib.bz_pairdist_partial_reuse, (rows.ptrs, n, d, part) + reuse + (ws.data_ptr(), ws.numel(), stream)
+        # [k % 2][reuse]
+        self._phase_a = [[phase_a(reuse) for reuse in self._reuse[s]] for s in (0, 1)]
       else:
         # aksel: the local coordinate-wise median is the centre; it goes to `out`, which the reduce rewrites (bz_aksel's order)
         self._median = _engine._coordinate_call("median", rows, None, out) if rule.center else None
@@ -549,6 +588,51 @@ class _SearchShard:
     record = self.record.data_ptr()
     self._steps = [(lib.bz_search_step, (self.scores.data_ptr(), world, state, record, eval_status, record + 8 * (2 * evals + 1),
                                          k, evals, stream)) for k in range(evals)]
+  def fuse(self, fx):
+    """ Prepare the stages of the fused exchange over `fx` (a `FusedExchange` of n rows): per evaluation the
+    rule's `*_peers` call (distance rules) and `bz_search_score_peers`, every argument but the slot's
+    tables and the epoch resolved here.  Every distance rule then reports a status word (0, or a peer that
+    did not show up), which the score's transition folds into the search's. """
+    lib = _lib.lib()
+    rows, ws, stream = self._rows, self._ws, self._stream
+    n, d, state, out, record = rows.n, rows.d, self._state.data_ptr(), self.out.data_ptr(), self.record.data_ptr()
+    self._slots = [fx.tables(0), fx.tables(1)]
+    self._tail = (ws.data_ptr(), ws.numel(), stream)
+    peers = (fx.rank, fx.world)
+    eval_status = None
+    if self.distance:
+      rule, meta = self._rule, self._meta.data_ptr()
+      code = _engine._SEARCH_RULES[rule.gar]
+      eval_status = meta + 4 * n
+      if self._pair:
+        head = (code, rows.ptrs, n, rule.f, rule.m, d, out, meta, eval_status)
+        self._rule_peers = [[(lib.bz_pairdist_reuse_peers, head + reuse + peers) for reuse in self._reuse[s]] for s in (0, 1)]
+      else:
+        mode = _lib.AKSEL_MODES["mid"] if rule.center else 0
+        self._rule_peers = (lib.bz_rowdist_peers, (code, rows.ptrs, n, rule.f, mode, out if rule.center else None, d, out, meta,
+                                                   eval_status) + peers)
+    self._score_peers = [(lib.bz_search_score_peers, (out, self._avg, d, state, record, eval_status, record + 8 * (2 * self.evals + 1),
+                                                      k, self.evals) + peers) for k in range(self.evals)]
+  def _with_slot(self, fn, head, epoch):
+    blocks, flags = self._slots[epoch % 2]
+    _engine._call(fn, head + (blocks, flags, epoch) + self._tail)
+  def evaluate_fused(self, k, epoch):
+    """ Evaluation k up to its score with the fused exchange: the candidate row, then the rule (distance
+    rules: its exchange at `epoch`; coordinate-wise rules: no exchange, `epoch` is None). """
+    with _engine._on(self.device):
+      _engine._call(*self._candidates[_lib.CANDIDATE_FIRST if k == 0 else _lib.CANDIDATE_NEXT])
+      if not self.distance:
+        _engine._call(*self._coordinate)
+      elif self._pair:
+        self._with_slot(*self._rule_peers[k % 2][int(k > 0 and self._mode.value >= 0)], epoch)
+      else:
+        if self._median is not None:
+          _engine._call(*self._median)
+        self._with_slot(*self._rule_peers, epoch)
+  def score_fused(self, k, epoch):
+    """ The score of evaluation k, its exchange at `epoch` and the transition. """
+    with _engine._on(self.device):
+      self._with_slot(*self._score_peers[k], epoch)
   def evaluate(self, k):
     call = _engine._call
     with _engine._on(self.device):
@@ -607,9 +691,23 @@ class ShardedLineSearch:
   Each evaluation's work between two exchanges is one stage method (`evaluate`, `conclude`, `step`,
   `finish`), so that `search()` is those stages plus the collectives.  `backend`, for tests, provides
   `search_shard(gar, grad_honests, f_real, f_decl, grad_avg, grad_att, evals, negative, kind, world)`, an
-  object with the stages (default: the CUDA library). """
+  object with the stages (default: the CUDA library).
+
+  exchange: "nccl"   the collectives above;
+            "fused"  no collective: every exchange runs inside the kernel that needs it, over the symmetric
+                     buffer of `fused_exchange(n, ...)` (the one `ShardedPlan(exchange="fused")` of the same n
+                     uses; a plain device buffer on one rank).  An evaluation is the candidate, [Aksel: the
+                     local median], the rule's `*_peers` call (`bz_pairdist_reuse_peers`: distances with
+                     reuse, exchange, scoring and reduce; `bz_rowdist_peers`), and `bz_search_score_peers`
+                     (the share's exchange and the transition): 2 exchanges per evaluation for a distance
+                     rule, 1 for the others, each advancing the buffer's epoch by one.  The same bits as
+                     "nccl".  The calls that share the buffer must be issued on one stream, in the same
+                     order on every rank.  Not for CUDA-graph capture: the epoch is passed by value;
+            "auto"   "fused" on 2..16 ranks with symmetric memory, the CUDA engine and (Multi-Krum, Bulyan,
+                     brute) 16-byte aligned rows on every rank, else "nccl"; the ranks agree on it
+                     (`choose_search_exchange`). """
   def __init__(self, gar, grad_honests, f_real, f_decl, grad_avg, grad_att, evals, negative=False, kind="identical",
-               group=None, backend=None):
+               group=None, backend=None, exchange="auto"):
     if gar not in _engine._SEARCH_RULES:
       raise KeyError(f"unknown aggregation rule {gar!r}")
     if kind not in _engine._SEARCH_KINDS:
@@ -618,9 +716,17 @@ class ShardedLineSearch:
       raise ValueError(f"evals = {evals}, expected evals >= 1")
     self.gar, self.evals, self.group = gar, int(evals), group
     self.world = dist.get_world_size(group) if dist.is_initialized() else 1
+    honest = list(grad_honests)
+    pair = gar in ("krum", "bulyan", "brute")
+    self.exchange = choose_search_exchange(exchange, not pair or rows_aligned(honest), _symmetric_memory_importable(),
+                                           backend is None, group)
     make = _SearchShard if backend is None else backend.search_shard
-    self._shard = make(gar, grad_honests, f_real, f_decl, grad_avg, grad_att, self.evals, negative, kind, self.world)
+    self._shard = make(gar, honest, f_real, f_decl, grad_avg, grad_att, self.evals, negative, kind, self.world)
     self.byz, self.record = self._shard.byz, self._shard.record
+    if self.exchange == "fused":
+      n, device = len(honest) + int(f_real), self._shard.device
+      self._fx = FusedExchange.local(n, device) if self.world == 1 else fused_exchange(n, device, group)
+      self._shard.fuse(self._fx)
   def evaluate(self, k):
     """ Evaluation k up to its first exchange: the candidate row, then the rule's phase A (distance rules:
     returns this rank's partial block) or the whole rule and the score share (coordinate-wise rules:
@@ -640,8 +746,17 @@ class ShardedLineSearch:
     if self.world > 1:
       dist.all_gather_into_tensor(gathered.view(-1), part, group=self.group)
     return gathered
+  def _epoch(self):
+    """ The epoch of the next exchange over the shared buffer. """
+    self._fx.epoch += 1
+    return self._fx.epoch
   def __call__(self):
     shard = self._shard
+    if self.exchange == "fused":
+      for k in range(self.evals):
+        shard.evaluate_fused(k, self._epoch() if shard.distance else None)
+        shard.score_fused(k, self._epoch())
+      return self.finish()
     for k in range(self.evals):
       part = self.evaluate(k)
       if shard.distance:
@@ -653,10 +768,12 @@ class ShardedLineSearch:
     a failed evaluation of Bulyan or brute raises what the plain call raises. """
     return _engine._search_outcome(self.record, self.evals)
 
-def line_search(gar, grad_honests, f_real, f_decl, grad_avg, grad_att, evals, negative=False, kind="identical", group=None):
+def line_search(gar, grad_honests, f_real, f_decl, grad_avg, grad_att, evals, negative=False, kind="identical", group=None,
+                exchange="auto"):
   """ `engine.line_search` on a d-sharded trainer (see `ShardedLineSearch`): returns (factor, this rank's
   shard of the Byzantine gradient), the factor the same Python float on every rank. """
-  search = ShardedLineSearch(gar, grad_honests, f_real, f_decl, grad_avg, grad_att, evals, negative, kind, group)
+  search = ShardedLineSearch(gar, grad_honests, f_real, f_decl, grad_avg, grad_att, evals, negative, kind, group,
+                             exchange=exchange)
   byz = search()
   factor, _ = search.result()
   return factor, byz

@@ -166,7 +166,8 @@ BZ_API int bz_brute_reuse(const float* const* rows, int n, int f, int64_t d, flo
  *                  each; [rank] is the local one).  Alternate between two slots from step to step.
  *   peer_flags     HOST array of nranks DEVICE pointers: the flag array (nranks uint32) of this step's
  *                  slot on every rank; zero before the first step
- *   epoch          step number: strictly increasing, the same on every rank for the same step
+ *   epoch          step number: strictly increasing, the same on every rank for the same step (the
+ *                  exchanges of byzagg_search_peers.h over the same slots count in the same sequence)
  *   status         DEVICE int32, required: BZ_STATUS_PEER_TIMEOUT when a peer did not show up
  * Rows must be 16-byte aligned (the ring kernel); otherwise BZ_EUNSUPPORTED: use the phases below.
  * The published block is n x n: entry (i, j), i < j, is this shard's sum of squared differences of
@@ -280,5 +281,8 @@ BZ_API int bz_gradient_row(const float* grad, int64_t d, double clip, float* sam
 /* The same search on a d-sharded trainer: each evaluation cut at its exchanges (the rule's partial block,
  * the score's R shares), which the caller all-gathers; every rank then takes the same next factor. */
 #include "byzagg_search_shards.h"
+
+/* The same search with every exchange over peer memory inside the kernel that needs it: no collective. */
+#include "byzagg_search_peers.h"
 
 #endif /* BYZAGG_H */

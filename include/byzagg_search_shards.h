@@ -17,6 +17,7 @@
  * and a last bz_search_candidate (BZ_CANDIDATE_FINAL) writes the Byzantine gradient's shard.  `evals` is
  * fixed in advance, so every rank issues the same launches and collectives; a rank with an empty shard
  * (d = 0) joins every exchange.  With one rank the trace is bz_line_search's, bit for bit.
+ * byzagg_search_peers.h runs the same evaluation with every exchange inside the kernels, over peer memory.
  */
 #ifndef BYZAGG_SEARCH_SHARDS_H
 #define BYZAGG_SEARCH_SHARDS_H

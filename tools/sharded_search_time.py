@@ -2,10 +2,12 @@
 # coding: utf-8
 """Times of the line search on the d-sharded path, on one GPU (one JSON line per measurement):
 
-  search     `sharded.ShardedLineSearch` at world size 1 against `engine.LineSearch`: 16 evaluations of
-             `little`'s direction (factor -16, `negative`), n = 25 (f = 5), for Multi-Krum, the trimmed
-             mean and the median, at d = 1,310,922 and at d_r = 163,866 (rank 0's shard at R = 8).  Both
-             searches issued and finished on the device (no result() read), CUDA events around each.
+  search     `sharded.ShardedLineSearch` at world size 1, with its collective exchange ("nccl") and with the
+             exchange inside its kernels ("fused", on a plain device buffer), against `engine.LineSearch`:
+             16 evaluations of `little`'s direction (factor -16, `negative`), n = 25 (f = 5), for
+             Multi-Krum, the trimmed mean and the median, at d = 1,310,922 and at d_r = 163,866 (rank 0's
+             shard at R = 8).  The searches issued and finished on the device (no result() read), CUDA
+             events around each; the three records are checked bit-identical.
   phase_a    phase A of one evaluation on that shard, n = 25 and n = 51: `bz_pairdist_partial_reuse`
              with the previous evaluation's table (only the candidate's pairs) and without a table.
 The two runs of a pair alternate, every shape is warmed up first; medians of REPS.  The card's name and
@@ -30,16 +32,17 @@ def event_ms(fn):
   end.synchronize()
   return start.elapsed_time(end)
 
-def alternate(a, b, warm=3):
-  """ Median ms of `a` and of `b`, run in turns after `warm` runs of each. """
+def alternate(*fns, warm=3):
+  """ Median ms of each of `fns`, run in turns after `warm` runs of each. """
   for _ in range(warm):
-    a(); b()
+    for fn in fns:
+      fn()
   torch.cuda.synchronize()
-  ta, tb = [], []
+  times = [[] for _ in fns]
   for _ in range(REPS):
-    ta.append(event_ms(a))
-    tb.append(event_ms(b))
-  return sorted(ta)[REPS // 2], sorted(tb)[REPS // 2]
+    for fn, t in zip(fns, times):
+      t.append(event_ms(fn))
+  return tuple(sorted(t)[REPS // 2] for t in times)
 
 def rows(n, d, seed):
   gen = torch.Generator(device=dev).manual_seed(seed)
@@ -54,10 +57,14 @@ def search_times(tag):
     avg, att = stck.mean(dim=0), stck.var(dim=0).sqrt_()
     for gar in ("krum", "trmean", "median"):
       single = engine.LineSearch(gar, honest, f, f, avg, att, 16, negative=True)
-      shard = sharded.ShardedLineSearch(gar, honest, f, f, avg, att, 16, negative=True)
-      t_single, t_shard = alternate(single, shard)
+      shard = sharded.ShardedLineSearch(gar, honest, f, f, avg, att, 16, negative=True, exchange="nccl")
+      fused = sharded.ShardedLineSearch(gar, honest, f, f, avg, att, 16, negative=True, exchange="fused")
+      t_single, t_shard, t_fused = alternate(single, shard, fused)
+      same = all(torch.equal(single.record[:-1].view(torch.int64), s.record[:-1].view(torch.int64)) for s in (shard, fused))
       print(json.dumps(dict(what="search", card=tag, gar=gar, n=n, d=d, evals=16, line_search_ms=round(t_single, 4),
-                            sharded_world1_ms=round(t_shard, 4), sharded_per_eval_extra_us=round((t_shard - t_single) / 16 * 1e3, 2))), flush=True)
+                            sharded_world1_ms=round(t_shard, 4), fused_world1_ms=round(t_fused, 4),
+                            sharded_per_eval_extra_us=round((t_shard - t_single) / 16 * 1e3, 2),
+                            fused_per_eval_extra_us=round((t_fused - t_single) / 16 * 1e3, 2), records_identical=same)), flush=True)
 
 def phase_a_times(tag):
   lib = _lib.lib()
