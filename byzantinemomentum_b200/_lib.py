@@ -1,6 +1,7 @@
 # coding: utf-8
 """ctypes binding of `libbyzagg.so` (C ABI: `include/byzagg.h`, `include/byzagg_shards.h`,
-`include/byzagg_attack.h`, `include/byzagg_search_shards.h` and `include/byzagg_search_peers.h`).
+`include/byzagg_attack.h`, `include/byzagg_search_shards.h`, `include/byzagg_search_peers.h` and
+`include/byzagg_coordinate.h`).
 
 The library is loaded lazily, on the first call that needs it, and the load FAILS LOUDLY:
 there is no CPU or PyTorch fallback anywhere in this package.  Build it in-tree with
@@ -12,10 +13,11 @@ import os
 import pathlib
 import threading
 
-__all__ = ["lib", "LibraryError", "library_path", "check", "MAX_N", "STATUS_MESSAGES",
+__all__ = ["lib", "LibraryError", "library_path", "check", "MAX_N", "MAX_N_COORDINATE", "STATUS_MESSAGES",
            "AKSEL_MODES", "STATUS_NO_FINITE_SET", "STATUS_DEGENERATE"]
 
 MAX_N = 64
+MAX_N_COORDINATE = 128      # BZ_MAX_N_COORDINATE: the coordinate-wise rules through bz_coordinate
 MAX_PEERS = 16
 STATUS_NO_FINITE_SET = 1
 STATUS_DEGENERATE = 2
@@ -104,6 +106,10 @@ SEARCH_PEER_SIGNATURES = {
   "bz_rowdist_peers": (_i, [_i, _c_rows, _i, _i, _i, _vp, _i64, _vp, _vp, _vp, _i, _i, _c_rows, _c_rows, ctypes.c_uint, _vp, _sz, _vp]),
   "bz_search_score_peers": (_i, [_vp, _vp, _i64, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _c_rows, _c_rows, ctypes.c_uint, _vp, _sz, _vp]),
 }
+# the same for include/byzagg_coordinate.h (the coordinate-wise rules up to MAX_N_COORDINATE rows)
+COORDINATE_SIGNATURES = {
+  "bz_coordinate": (_i, [_i, _c_rows, _i, _i, _i64, _vp, _vp]),
+}
 SEARCH_STATE_BYTES = 64                     # BZ_SEARCH_STATE_BYTES
 CANDIDATE_FIRST, CANDIDATE_NEXT, CANDIDATE_FINAL = 0, 1, 2
 
@@ -125,7 +131,8 @@ def lib():
         handle = ctypes.CDLL(str(path))
       except OSError as err:
         raise LibraryError(f"unable to load {path}: {err}") from err
-      tables = (SIGNATURES, SHARD_SIGNATURES, ATTACK_SIGNATURES, SEARCH_SHARD_SIGNATURES, SEARCH_PEER_SIGNATURES)
+      tables = (SIGNATURES, SHARD_SIGNATURES, ATTACK_SIGNATURES, SEARCH_SHARD_SIGNATURES, SEARCH_PEER_SIGNATURES,
+                COORDINATE_SIGNATURES)
       for name, (restype, argtypes) in [item for table in tables for item in table.items()]:
         try:
           fn = getattr(handle, name)

@@ -51,10 +51,11 @@ Geom make_geom(const float* const* rows, int n, const void* out, const void* ext
   return g;
 }
 
-static int check_rows(const float* const* rows, int n, int64_t d, const void* out, const char* who) {
+// max_n: kMaxN, or kMaxNCoordinate for bz_coordinate (the limit's name goes into the message)
+static int check_rows(const float* const* rows, int n, int64_t d, const void* out, const char* who, int max_n = kMaxN) {
   if (rows == nullptr) return fail(BZ_EINVAL, "%s: rows is NULL", who);
   if (n < 1) return fail(BZ_EINVAL, "%s: n = %d, expected n >= 1", who, n);
-  if (n > kMaxN) return fail(BZ_EUNSUPPORTED, "%s: n = %d exceeds BZ_MAX_N = %d", who, n, kMaxN);
+  if (n > max_n) return fail(BZ_EUNSUPPORTED, "%s: n = %d exceeds %s = %d", who, n, max_n == kMaxN ? "BZ_MAX_N" : "BZ_MAX_N_COORDINATE", max_n);
   if (d < 0) return fail(BZ_EINVAL, "%s: d = %lld < 0", who, (long long)d);
   if (d > 0) {
     if (out == nullptr) return fail(BZ_EINVAL, "%s: output pointer is NULL", who);
@@ -67,9 +68,11 @@ static int check_rows(const float* const* rows, int n, int64_t d, const void* ou
   return BZ_OK;
 }
 
-static void fill_table(RowTable& t, const float* const* rows, int n) {
+template <class Rows>
+static void fill_table(Rows& t, const float* const* rows, int n) {
+  constexpr int slots = sizeof(t.p) / sizeof(t.p[0]);
   for (int r = 0; r < n; ++r) t.p[r] = rows[r];
-  for (int r = n; r < kMaxN; ++r) t.p[r] = rows[0];
+  for (int r = n; r < slots; ++r) t.p[r] = rows[0];
 }
 
 // Unique rows by pointer equality: uniq[k] = first row with that address, to_unique[i] = its k.
@@ -127,6 +130,38 @@ static int check_f_trim(int n, int f, const char* who) {
   // executable range (the reference's check(), trmean.py:52-64, is the caller's job)
   if (f < 0 || n - 2 * f < 1) return fail(BZ_EINVAL, "%s: f = %d not executable with n = %d (need n - 2f >= 1)", who, f, n);
   return BZ_OK;
+}
+
+// kMaxN < n <= kMaxNCoordinate: the WideRowTable kernels, VEC = 1 for K1 (a column of up to 128
+// values per thread), the widest common vector for K3.
+static bool launch_median_wide(int n, const WideRowTable& t, const Geom& g, float* out, cudaStream_t st) {
+  return launch_median_wide_part11(n, t, g, out, st) || launch_median_wide_part12(n, t, g, out, st) ||
+         launch_median_wide_part13(n, t, g, out, st) || launch_median_wide_part14(n, t, g, out, st) ||
+         launch_median_wide_part15(n, t, g, out, st) || launch_median_wide_part16(n, t, g, out, st) ||
+         launch_median_wide_part17(n, t, g, out, st) || launch_median_wide_part18(n, t, g, out, st);
+}
+static bool launch_sorted_wide(int n, const WideRowTable& t, const Geom& g, int mode, int f, float* out, cudaStream_t st) {
+  return launch_sorted_wide_part19(n, t, g, mode, f, out, st) || launch_sorted_wide_part20(n, t, g, mode, f, out, st) ||
+         launch_sorted_wide_part21(n, t, g, mode, f, out, st) || launch_sorted_wide_part22(n, t, g, mode, f, out, st) ||
+         launch_sorted_wide_part23(n, t, g, mode, f, out, st) || launch_sorted_wide_part24(n, t, g, mode, f, out, st) ||
+         launch_sorted_wide_part25(n, t, g, mode, f, out, st) || launch_sorted_wide_part26(n, t, g, mode, f, out, st);
+}
+
+static int run_coordinate_wide(int rule, const float* const* rows, int n, int f, int64_t d, float* out, cudaStream_t st) {
+  WideRowTable t;
+  fill_table(t, rows, n);
+  if (rule == BZ_RULE_AVERAGE) {
+    launch_average(t, make_geom(rows, n, out, nullptr, d, 4), nullptr, n, 1, (float)n, nullptr, out, st);
+    return check_launch("k3_average");
+  }
+  const Geom g = make_geom(rows, n, out, nullptr, d, 1);
+  if (rule == BZ_RULE_MEDIAN) {
+    launch_median_wide(n, t, g, out, st);
+    return check_launch("k1_median");
+  }
+  const int mode = (rule == BZ_RULE_TRMEAN) ? kModeTrmean : (rule == BZ_RULE_PHOCAS) ? kModePhocas : kModeMeamed;
+  launch_sorted_wide(n, t, g, mode, f, out, st);
+  return check_launch("k1_sorted");
 }
 
 }  // namespace bz
@@ -276,6 +311,21 @@ int bz_coordinate_host(int rule, const float* const* host_rows, int n, int f, in
   for (int k = 0; k < nev; ++k) cudaEventDestroy(ev[k]);      // released by the runtime once they have completed
   if (rc != BZ_OK) return rc;
   return check_launch("bz_coordinate_host");
+}
+
+int bz_coordinate(int rule, const float* const* rows, int n, int f, int64_t d, float* out, void* stream) {
+  if (rule < BZ_RULE_AVERAGE || rule > BZ_RULE_MEAMED) return fail(BZ_EINVAL, "bz_coordinate: unknown rule %d", rule);
+  if (int rc = check_rows(rows, n, d, out, "bz_coordinate", kMaxNCoordinate)) return rc;
+  if (rule >= BZ_RULE_TRMEAN) if (int rc = check_f_trim(n, f, "bz_coordinate")) return rc;
+  if (d == 0) return BZ_OK;
+  if (n > kMaxN) return run_coordinate_wide(rule, rows, n, f, d, out, (cudaStream_t)stream);
+  switch (rule) {
+    case BZ_RULE_AVERAGE: return bz_average(rows, n, d, out, stream);
+    case BZ_RULE_MEDIAN:  return bz_median(rows, n, d, out, stream);
+    case BZ_RULE_TRMEAN:  return bz_trmean(rows, n, f, d, out, stream);
+    case BZ_RULE_PHOCAS:  return bz_phocas(rows, n, f, d, out, stream);
+    default:              return bz_meamed(rows, n, f, d, out, stream);
+  }
 }
 
 }  // extern "C"

@@ -4,6 +4,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stddef.h>
+#include <type_traits>
 
 #include "../../include/byzagg.h"
 
@@ -20,6 +21,14 @@ constexpr int kMaxN = BZ_MAX_N;
 struct RowTable {
   const float* p[kMaxN];
 };
+
+// The same for the coordinate-wise rules above kMaxN rows (bz_coordinate): 1 KB, well inside the
+// 4 KB of kernel parameters.  The kernels that exist for n <= kMaxN keep the 512-byte table.
+constexpr int kMaxNCoordinate = BZ_MAX_N_COORDINATE;
+struct WideRowTable {
+  const float* p[kMaxNCoordinate];
+};
+template <int N> using RowsOf = typename std::conditional<(N <= kMaxN), RowTable, WideRowTable>::type;
 
 // Geometry of a launch over d coordinates with VEC per thread.  All rows (and the output)
 // share the same misalignment, so shifting the element index by `shift` (0..VEC-1) makes every
@@ -80,7 +89,7 @@ template <> struct VecLoad<1> {
 // common (full) case stay back to back in the instruction stream (one branch, N independent
 // LDG in flight).  Partial vectors (e0 < 0 or e0 + VEC > d) read out-of-range lanes as 0.
 template <int N, int VEC>
-__device__ __forceinline__ void load_rows(const RowTable& rows, int64_t e0, int64_t d, bool full, float (&x)[VEC][N]) {
+__device__ __forceinline__ void load_rows(const RowsOf<N>& rows, int64_t e0, int64_t d, bool full, float (&x)[VEC][N]) {
   if (full) {
 #pragma unroll
     for (int r = 0; r < N; ++r) {

@@ -12,6 +12,10 @@
 //   k1_median<N, VEC>            median.py:31-39        FMNMX.NAN network, pruned to one rank
 //   k1_sorted<N, VEC, F, MODE>   trmean.py:24-50,69-109 sort, then trmean / phocas / meamed
 //
+// Up to N = kMaxN the kernels take the 64-pointer RowTable; above, up to kMaxNCoordinate
+// (bz_coordinate, VEC = 1 only), an overload of the same kernel takes the 128-pointer WideRowTable.
+// RowsOf<N> picks the table; the bodies are shared.
+//
 // F / MODE = -1 mean "run-time value": one generic kernel per (N, VEC) serves every f and the
 // three epilogues after a full sort.  For n = 11, 25, 51 (BASELINE.json's configs and the
 // reference's experiment grids) the trimmed mean is also instantiated for every f with F and
@@ -56,7 +60,7 @@ __device__ __forceinline__ unsigned nsm() {
 // `body(x, e0, full)` consumes the N x VEC values of one logical vector (sorting them in place is
 // fine) and stores its result.
 template <int N, int VEC, class Body>
-__device__ __forceinline__ void k1_walk(const RowTable& rows, const Geom& g, Body body) {
+__device__ __forceinline__ void k1_walk(const RowsOf<N>& rows, const Geom& g, Body body) {
   const int64_t stride = (int64_t)gridDim.x * kK1Threads;
   int64_t v = (int64_t)blockIdx.x * kK1Threads + threadIdx.x;
   // Programmatic dependent launch on both sides: the NEXT kernel of the stream may be scheduled while this
@@ -94,15 +98,17 @@ __device__ __forceinline__ void k1_walk(const RowTable& rows, const Geom& g, Bod
 // ---- median ---------------------------------------------------------------------------
 
 // Register cap: 512 resident threads per SM (<= 128 registers) whenever the N x VEC values leave room.
+// Above kMaxN rows (VEC = 1): two CTAs per SM, i.e. up to 255 registers for the column and the network.
 #ifndef BZ_K1_CAP
 #define BZ_K1_CAP 104
 #endif
-__host__ __device__ constexpr int k1_min_blocks(int n, int vec) { return (n * vec <= BZ_K1_CAP) ? 512 / kK1Threads : 1; }
+__host__ __device__ constexpr int k1_min_blocks(int n, int vec) {
+  return (n > kMaxN) ? 256 / kK1Threads : (n * vec <= BZ_K1_CAP) ? 512 / kK1Threads : 1;
+}
 
 template <int N, int VEC>
-__global__ void __launch_bounds__(kK1Threads, k1_min_blocks(N, VEC))
-k1_median(const __grid_constant__ RowTable rows, const Geom g, float* __restrict__ out) {
-  k1_walk<N, VEC>(rows, g, [&](float (&x)[VEC][N], int64_t e0, bool full) {
+__device__ __forceinline__ void k1_median_body(const RowsOf<N>& rows, const Geom& g, float* __restrict__ out) {
+  k1_walk<N, VEC>(rows, g, [&](float (&x)[VEC][N], int64_t e0, bool full) __attribute__((always_inline)) {
     float chk = 0.f;
 #pragma unroll
     for (int r = 0; r < N; ++r)
@@ -126,6 +132,17 @@ k1_median(const __grid_constant__ RowTable rows, const Geom g, float* __restrict
     }
     store_vec<VEC>(out, e0, g.d, full, res);
   });
+}
+
+template <int N, int VEC>
+__global__ void __launch_bounds__(kK1Threads, k1_min_blocks(N, VEC))
+k1_median(const __grid_constant__ RowTable rows, const Geom g, float* __restrict__ out) {
+  k1_median_body<N, VEC>(rows, g, out);
+}
+template <int N, int VEC>
+__global__ void __launch_bounds__(kK1Threads, k1_min_blocks(N, VEC))
+k1_median(const __grid_constant__ WideRowTable rows, const Geom g, float* __restrict__ out) {
+  k1_median_body<N, VEC>(rows, g, out);
 }
 
 // ---- trimmed mean of a sorted column (trmean.py:33) -----------------------------------------
@@ -197,14 +214,13 @@ template <int N, int F, int MODE> struct MixFor { typedef MixFull<N> mask; typed
 template <int N, int F> struct MixFor<N, F, kModeTrmean> { typedef MixTrim<N, F> mask; typedef OpsMix<mask> type; };
 
 template <int N, int VEC, int F, int MODE>
-__global__ void __launch_bounds__(kK1Threads, k1_min_blocks(N, VEC))
-k1_sorted(const __grid_constant__ RowTable rows, const Geom g, const int mode_rt, const int f_rt,
-          float* __restrict__ out) {
+__device__ __forceinline__ void k1_sorted_body(const RowsOf<N>& rows, const Geom& g, const int mode_rt, const int f_rt,
+                                               float* __restrict__ out) {
   extern __shared__ __align__(16) float smem[];   // sorted columns for the closest modes
   const int mode = (MODE >= 0) ? MODE : mode_rt;
   const int f = (F >= 0) ? F : f_rt;
   float* sorted_cols = smem;
-  k1_walk<N, VEC>(rows, g, [&](float (&x)[VEC][N], int64_t e0, bool full) {
+  k1_walk<N, VEC>(rows, g, [&](float (&x)[VEC][N], int64_t e0, bool full) __attribute__((always_inline)) {
     float chk = 0.f;
 #pragma unroll
     for (int r = 0; r < N; ++r)
@@ -255,5 +271,24 @@ k1_sorted(const __grid_constant__ RowTable rows, const Geom g, const int mode_rt
     store_vec<VEC>(out, e0, g.d, full, res);
   });
 }
+
+template <int N, int VEC, int F, int MODE>
+__global__ void __launch_bounds__(kK1Threads, k1_min_blocks(N, VEC))
+k1_sorted(const __grid_constant__ RowTable rows, const Geom g, const int mode_rt, const int f_rt,
+          float* __restrict__ out) {
+  k1_sorted_body<N, VEC, F, MODE>(rows, g, mode_rt, f_rt, out);
+}
+template <int N, int VEC, int F, int MODE>
+__global__ void __launch_bounds__(kK1Threads, k1_min_blocks(N, VEC))
+k1_sorted(const __grid_constant__ WideRowTable rows, const Geom g, const int mode_rt, const int f_rt,
+          float* __restrict__ out) {
+  k1_sorted_body<N, VEC, F, MODE>(rows, g, mode_rt, f_rt, out);
+}
+
+// The kernel of an N-row launch: the overload that takes RowsOf<N>.
+template <int N, int VEC>
+inline auto k1_median_fn() -> void (*)(RowsOf<N>, Geom, float*) { return k1_median<N, VEC>; }
+template <int N, int VEC, int F, int MODE>
+inline auto k1_sorted_fn() -> void (*)(RowsOf<N>, Geom, int, int, float*) { return k1_sorted<N, VEC, F, MODE>; }
 
 }  // namespace bz

@@ -6,6 +6,8 @@
 // The selection is read from DEVICE memory (written by the K5 scoring kernel), so the
 // distance pass, the scoring and this pass chain on one stream with no host round trip.
 // Roofline: HBM, (count + 1)·4 B per coordinate.
+// bz_coordinate's average above kMaxN rows runs the same body over the 128-pointer WideRowTable
+// (an overload of the kernel; the 64-pointer kernels are unchanged).
 #include "launch.cuh"
 
 namespace bz {
@@ -15,8 +17,8 @@ constexpr int kK3Unroll = 8;
 
 // FULL: the whole vector lies inside [0, d) and is naturally aligned (the common case, kept
 // free of per-load branches so that kK3Unroll loads stay in flight); otherwise element-wise.
-template <int VEC, bool FULL>
-__device__ __forceinline__ void average_body(const RowTable& rows, const int64_t e0, const int64_t d,
+template <int VEC, bool FULL, class Rows>
+__device__ __forceinline__ void average_body(const Rows& rows, const int64_t e0, const int64_t d,
                                              const int32_t* __restrict__ sel, const int count, const int zero_init,
                                              const float divisor, float* __restrict__ out) {
   float acc[VEC];
@@ -52,11 +54,10 @@ __device__ __forceinline__ void average_body(const RowTable& rows, const int64_t
   store_vec<VEC>(out, e0, d, FULL, acc);
 }
 
-template <int VEC>
-__global__ void __launch_bounds__(kK3Threads)
-k3_average(const __grid_constant__ RowTable rows, const Geom g, const int32_t* __restrict__ sel,
-           const int count, const int zero_init, const float divisor,
-           const int32_t* __restrict__ status, float* __restrict__ out) {
+template <int VEC, class Rows>
+__device__ __forceinline__ void k3_average_body(const Rows& rows, const Geom& g, const int32_t* __restrict__ sel,
+                                                const int count, const int zero_init, const float divisor,
+                                                const int32_t* __restrict__ status, float* __restrict__ out) {
   const int64_t blk = g.reverse ? (int64_t)gridDim.x - 1 - blockIdx.x : (int64_t)blockIdx.x;
   const int64_t v = blk * kK3Threads + threadIdx.x;
   if (v >= g.nv) return;
@@ -74,13 +75,38 @@ k3_average(const __grid_constant__ RowTable rows, const Geom g, const int32_t* _
   else      average_body<VEC, false>(rows, e0, g.d, sel, count, zero_init, divisor, out);
 }
 
-void launch_average(const RowTable& rows, const Geom& g, const int32_t* sel, int count,
-                    int zero_init, float divisor, const int32_t* status, float* out, cudaStream_t st) {
+template <int VEC>
+__global__ void __launch_bounds__(kK3Threads)
+k3_average(const __grid_constant__ RowTable rows, const Geom g, const int32_t* __restrict__ sel,
+           const int count, const int zero_init, const float divisor,
+           const int32_t* __restrict__ status, float* __restrict__ out) {
+  k3_average_body<VEC>(rows, g, sel, count, zero_init, divisor, status, out);
+}
+template <int VEC>
+__global__ void __launch_bounds__(kK3Threads)
+k3_average(const __grid_constant__ WideRowTable rows, const Geom g, const int32_t* __restrict__ sel,
+           const int count, const int zero_init, const float divisor,
+           const int32_t* __restrict__ status, float* __restrict__ out) {
+  k3_average_body<VEC>(rows, g, sel, count, zero_init, divisor, status, out);
+}
+
+template <class Rows>
+static void launch_average_rows(const Rows& rows, const Geom& g, const int32_t* sel, int count,
+                                int zero_init, float divisor, const int32_t* status, float* out, cudaStream_t st) {
+  typedef void (*Kernel)(Rows, Geom, const int32_t*, int, int, float, const int32_t*, float*);
   if (g.nv <= 0) return;
   const unsigned blocks = (unsigned)((g.nv + kK3Threads - 1) / kK3Threads);
-  if (g.vec == 4)      launch_after(k3_average<4>, blocks, kK3Threads, 0, st, rows, g, sel, count, zero_init, divisor, status, out);
-  else if (g.vec == 2) launch_after(k3_average<2>, blocks, kK3Threads, 0, st, rows, g, sel, count, zero_init, divisor, status, out);
-  else                 launch_after(k3_average<1>, blocks, kK3Threads, 0, st, rows, g, sel, count, zero_init, divisor, status, out);
+  const Kernel kernel = (g.vec == 4) ? Kernel(k3_average<4>) : (g.vec == 2) ? Kernel(k3_average<2>) : Kernel(k3_average<1>);
+  launch_after(kernel, blocks, kK3Threads, 0, st, rows, g, sel, count, zero_init, divisor, status, out);
+}
+
+void launch_average(const RowTable& rows, const Geom& g, const int32_t* sel, int count,
+                    int zero_init, float divisor, const int32_t* status, float* out, cudaStream_t st) {
+  launch_average_rows(rows, g, sel, count, zero_init, divisor, status, out, st);
+}
+void launch_average(const WideRowTable& rows, const Geom& g, const int32_t* sel, int count,
+                    int zero_init, float divisor, const int32_t* status, float* out, cudaStream_t st) {
+  launch_average_rows(rows, g, sel, count, zero_init, divisor, status, out, st);
 }
 
 }  // namespace bz

@@ -41,7 +41,7 @@ __host__ __device__ constexpr int body_vec(int n) { return n <= 28 ? 4 : 2; }
 // Epilogue of k1_sorted.
 enum SortedMode { kModeTrmean = 0, kModePhocas = 1, kModeMeamed = 2 };
 
-// K1 (k1_inst.cu, 9 parts).  Parts 0-7 return false when n is outside the part's range;
+// K1 (k1_inst.cu, parts 0-10).  Parts 0-7 return false when n is outside the part's range;
 // launch_trmean_special returns false when (n, f) has no compile-time specialisation.
 bool launch_median_part0(int n, const RowTable& rows, const Geom& g, float* out, cudaStream_t st);
 bool launch_median_part1(int n, const RowTable& rows, const Geom& g, float* out, cudaStream_t st);
@@ -55,8 +55,28 @@ bool launch_trmean_special(int n, int f, const RowTable& rows, const Geom& g, fl
 bool launch_phocas_special(int n, int f, const RowTable& rows, const Geom& g, float* out, cudaStream_t st);
 bool launch_meamed_special(int n, int f, const RowTable& rows, const Geom& g, float* out, cudaStream_t st);
 
-// K3 (k3_average.cu): ordered-subset average.
+// K1 above kMaxN rows (k1_inst.cu parts 11-26, VEC = 1, eight n per part): false when n is outside the part's range.
+bool launch_median_wide_part11(int n, const WideRowTable& rows, const Geom& g, float* out, cudaStream_t st);
+bool launch_median_wide_part12(int n, const WideRowTable& rows, const Geom& g, float* out, cudaStream_t st);
+bool launch_median_wide_part13(int n, const WideRowTable& rows, const Geom& g, float* out, cudaStream_t st);
+bool launch_median_wide_part14(int n, const WideRowTable& rows, const Geom& g, float* out, cudaStream_t st);
+bool launch_median_wide_part15(int n, const WideRowTable& rows, const Geom& g, float* out, cudaStream_t st);
+bool launch_median_wide_part16(int n, const WideRowTable& rows, const Geom& g, float* out, cudaStream_t st);
+bool launch_median_wide_part17(int n, const WideRowTable& rows, const Geom& g, float* out, cudaStream_t st);
+bool launch_median_wide_part18(int n, const WideRowTable& rows, const Geom& g, float* out, cudaStream_t st);
+bool launch_sorted_wide_part19(int n, const WideRowTable& rows, const Geom& g, int mode, int f, float* out, cudaStream_t st);
+bool launch_sorted_wide_part20(int n, const WideRowTable& rows, const Geom& g, int mode, int f, float* out, cudaStream_t st);
+bool launch_sorted_wide_part21(int n, const WideRowTable& rows, const Geom& g, int mode, int f, float* out, cudaStream_t st);
+bool launch_sorted_wide_part22(int n, const WideRowTable& rows, const Geom& g, int mode, int f, float* out, cudaStream_t st);
+bool launch_sorted_wide_part23(int n, const WideRowTable& rows, const Geom& g, int mode, int f, float* out, cudaStream_t st);
+bool launch_sorted_wide_part24(int n, const WideRowTable& rows, const Geom& g, int mode, int f, float* out, cudaStream_t st);
+bool launch_sorted_wide_part25(int n, const WideRowTable& rows, const Geom& g, int mode, int f, float* out, cudaStream_t st);
+bool launch_sorted_wide_part26(int n, const WideRowTable& rows, const Geom& g, int mode, int f, float* out, cudaStream_t st);
+
+// K3 (k3_average.cu): ordered-subset average (the 128-pointer table: bz_coordinate's average above kMaxN rows).
 void launch_average(const RowTable& rows, const Geom& g, const int32_t* sel, int count,
+                    int zero_init, float divisor, const int32_t* status, float* out, cudaStream_t st);
+void launch_average(const WideRowTable& rows, const Geom& g, const int32_t* sel, int count,
                     int zero_init, float divisor, const int32_t* status, float* out, cudaStream_t st);
 
 }  // namespace bz

@@ -152,15 +152,17 @@ def _copy_streams(device):
     lanes = _copy_lanes[device.index] = [torch.cuda.Stream(device) for _ in range(_COPY_LANES)]
   return lanes
 
-def _validate(gradients):
-  """ One pass over the list: types, dtype, rank, length; returns (first, all_contiguous). """
+def _validate(gradients, limit=_lib.MAX_N):
+  """ One pass over the list: types, dtype, rank, length (at most `limit` rows: MAX_N, or
+  MAX_N_COORDINATE for the coordinate-wise rules); returns (first, all_contiguous). """
   if not isinstance(gradients, (list, tuple)) or len(gradients) < 1:
     raise ValueError(f"expected a non-empty list of gradients, got {type(gradients).__name__} of length {len(gradients) if hasattr(gradients, '__len__') else '?'}")
   first = gradients[0]
   if not isinstance(first, torch.Tensor):
     raise TypeError(f"gradients must be torch tensors, got {type(first).__name__}")
-  if len(gradients) > _lib.MAX_N:
-    raise ValueError(f"{len(gradients)} gradients exceed the supported maximum of {_lib.MAX_N}")
+  if len(gradients) > limit:
+    wider = f" (the coordinate-wise rules accept up to {_lib.MAX_N_COORDINATE})" if limit < _lib.MAX_N_COORDINATE else ""
+    raise ValueError(f"{len(gradients)} gradients exceed the supported maximum of {limit}{wider}")
   if first.dim() != 1:
     raise ValueError("gradients must be 1-D tensors")
   d = first.numel()
@@ -207,12 +209,12 @@ class _CallCache:
 
 _call_cache = _CallCache()
 
-def _prepare(gradients, single_pass=False):
+def _prepare(gradients, single_pass=False, limit=_lib.MAX_N):
   prep = _call_cache.lookup(gradients)
-  if prep is not None:
+  if prep is not None and prep.n <= limit:
     prep.stream = torch.cuda.current_stream(prep.device).cuda_stream
     return prep
-  first, contiguous = _validate(gradients)
+  first, contiguous = _validate(gradients, limit)
   if not torch.cuda.is_available():
     raise _lib.LibraryError("no CUDA device available: byzantinemomentum_b200 runs on H100 (sm_90a) GPUs only (no CPU fallback)")
   _lib.lib()
@@ -231,8 +233,11 @@ def _prepare(gradients, single_pass=False):
     for g in gradients:
       uniq.setdefault(id(g), g)
     pinned = False          # never asked: Tensor.is_pinned() is a slow driver query on some boxes
-    mode = _host_path(device).choose(single_pass, pinned)
-    prep.host_mode = (single_pass, pinned, mode)
+    if n <= _lib.MAX_N:
+      mode = _host_path(device).choose(single_pass, pinned)
+      prep.host_mode = (single_pass, pinned, mode)
+    else:
+      mode = "lanes"        # above MAX_N rows (bz_stage_rows stops there): per-row copies, kept out of the measured choice
     torch.cuda.current_stream(device).synchronize()        # the clock below times this call only
     prep.host_t0 = time.perf_counter()
     buf = _staging_buffer(device, len(uniq), d)
@@ -350,20 +355,23 @@ def _coordinate_pipeline(name, gradients, f, path, device):
   return result
 
 def _coordinate_call(name, prep, f, out):
-  """ (fn, args) of the coordinate-wise rule `name` writing to the address `out`. """
+  """ (fn, args) of the coordinate-wise rule `name` writing to the address `out`: `bz_<name>` up to
+  MAX_N rows, `bz_coordinate` above. """
+  if prep.n > _lib.MAX_N:
+    return _lib.lib().bz_coordinate, (_RULE_CODES[name], prep.ptrs, prep.n, 0 if f is None else int(f), prep.d, out, prep.stream)
   head = (prep.ptrs, prep.n, int(f)) if name in ("trmean", "phocas", "meamed") else (prep.ptrs, prep.n)
   return getattr(_lib.lib(), "bz_" + name), head + (prep.d, out, prep.stream)
 
 def _coordinate(name, gradients, f=None):
   if type(gradients) in (list, tuple) and len(gradients) > 0 and isinstance(gradients[0], torch.Tensor) and gradients[0].device.type == "cpu" and torch.cuda.is_available():
-    _validate(gradients)
+    _validate(gradients, _lib.MAX_N_COORDINATE)
     _lib.lib()
     device = torch.device("cuda", torch.cuda.current_device())
     path = _host_path(device)
-    if path.choose(True, False) == "pipeline":
+    if len(gradients) <= _lib.MAX_N and path.choose(True, False) == "pipeline":
       torch.cuda.current_stream(device).synchronize()        # the clock times this call only
       return _coordinate_pipeline(name, gradients, f, path, device)
-  prep = _prepare(gradients, single_pass=True)
+  prep = _prepare(gradients, single_pass=True, limit=_lib.MAX_N_COORDINATE)
   out = torch.empty(prep.d, dtype=torch.float32, device=prep.device)
   _run(prep.device, *_coordinate_call(name, prep, f, out.data_ptr()))
   return _finish(prep, out)
@@ -1136,7 +1144,7 @@ class Plan:
   read `plan.status` when needed: non-zero means the rule is undefined on this data and `out`
   is NaN. """
   def __init__(self, gar, gradients, f=None, m=None, mode="mid", out=None):
-    prep = _prepare(list(gradients))
+    prep = _prepare(list(gradients), limit=_lib.MAX_N_COORDINATE if gar in _RULE_CODES else _lib.MAX_N)
     if prep.to_cpu:
       raise ValueError("Plan takes CUDA tensors (host tensors go through the plain call, which stages them)")
     n, d = prep.n, prep.d

@@ -13,7 +13,9 @@ Differences with the reference, all deliberate:
   * `influence(honests, attacks, ...)` right after an aggregation over the same tensors
     reuses the selection computed on the device instead of recomputing all distances
     (attack.py:822 always follows attack.py:821);
-  * with more than 64 gradients the rules raise (`BZ_MAX_N`).
+  * the coordinate-wise rules (average, median, trmean, phocas, meamed) take up to 128 gradients
+    (`BZ_MAX_N_COORDINATE`); with more than 64 gradients the distance-based rules raise
+    (`BZ_MAX_N`), with a message saying so.
 """
 
 import math

@@ -27,7 +27,8 @@
  *     filled with NaN.
  *   - Return value: 0 on success, a negative BZ_E* code otherwise; bz_last_error() returns
  *     a thread-local message for the last failure.
- *   - 1 <= n <= bz_max_n() (= 64), d >= 0 (d = 0 is a no-op).
+ *   - 1 <= n <= bz_max_n() (= 64), d >= 0 (d = 0 is a no-op).  The coordinate-wise rules take up
+ *     to 128 rows through bz_coordinate (byzagg_coordinate.h, included at the end).
  *   - Parameter validity (f, m ranges) is the caller's job, exactly like the reference's
  *     `check()` functions; the library only rejects what it cannot execute.
  */
@@ -284,5 +285,9 @@ BZ_API int bz_gradient_row(const float* grad, int64_t d, double clip, float* sam
 
 /* The same search with every exchange over peer memory inside the kernel that needs it: no collective. */
 #include "byzagg_search_peers.h"
+
+/* The coordinate-wise rules (average, median, trimmed mean, Phocas, MeaMed) for up to
+ * BZ_MAX_N_COORDINATE = 128 rows: bz_coordinate. */
+#include "byzagg_coordinate.h"
 
 #endif /* BYZAGG_H */
