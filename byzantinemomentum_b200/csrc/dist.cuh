@@ -134,8 +134,10 @@ int launch_search_step(const double* partials, int nparts, const SearchTail& tai
 // ---- K6: study metrics in one pass (k6_study.cu) -------------------------------------------------
 // avg = (rows[0] + rows[1] + ...)/n; stats[0] = sum avg^2, stats[1] = max |avg|,
 // stats[2+i] = sum_k (rows[i][k] - avg[k])^2.  `parts` needs kMaxParts*(n+1) doubles (n >= 2) and
-// `bits`: two device scratch words.
+// `bits`: two device scratch words.  The 128-pointer table: kMaxN < n <= kMaxNCoordinate.
 void launch_study(const RowTable& rows, int n, const float* const* host_rows, int64_t d, float* avg,
+                  double* stats, double* parts, unsigned* bits, cudaStream_t st);
+void launch_study(const WideRowTable& rows, int n, const float* const* host_rows, int64_t d, float* avg,
                   double* stats, double* parts, unsigned* bits, cudaStream_t st);
 
 // Sum `nparts` blocks of `len` doubles in index order into `block` (fixed order: deterministic).

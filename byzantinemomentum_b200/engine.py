@@ -561,6 +561,12 @@ def cge(gradients, f):
 _SEARCH_RULES = dict(_RULE_CODES, krum=5, bulyan=6, brute=7, aksel=8, cge=9)      # BZ_RULE_*
 _SEARCH_KINDS = {"identical": 0, "empire-strict": 1}                             # BZ_ATTACK_*
 
+def search_max_rows(gar):
+  """ The most rows (honest + f_real) the line search takes against the rule `gar`: MAX_N_COORDINATE for
+  the coordinate-wise rules, MAX_N for the distance rules (`bz_line_search`'s limits).  `LineSearch`,
+  `sharded.ShardedLineSearch` and `plugin.install_attacks` all ask here. """
+  return _lib.MAX_N_COORDINATE if gar in _RULE_CODES else _lib.MAX_N
+
 class LineSearch:
   """ A prepared `bz_line_search`: `line_maximize(eval_factor, evals)` of the identical-family attacks
   (kind "identical": candidate `grad_avg + s * grad_att`, s = -x when `negative`) or of empire-strict
@@ -576,7 +582,8 @@ class LineSearch:
     if kind not in _SEARCH_KINDS:
       raise ValueError(f"unknown attack kind {kind!r}, expected one of {sorted(_SEARCH_KINDS)}")
     honest = list(grad_honests)
-    prep = _prepare(honest)
+    limit = search_max_rows(gar)
+    prep = _prepare(honest, limit=limit)
     if prep.to_cpu:
       raise ValueError("the line search takes CUDA tensors")
     if not all(g.is_contiguous() for g in honest):
@@ -590,7 +597,7 @@ class LineSearch:
     self._out = torch.empty(prep.d, dtype=torch.float32, device=prep.device)
     self.record = torch.empty(2 * max(self.evals, 0) + 2, dtype=torch.float64, device=prep.device)
     n = prep.n + int(f_real)
-    self._ws = torch.empty(int(_lib.lib().bz_line_search_workspace_bytes(min(max(n, 1), _lib.MAX_N))), dtype=torch.uint8, device=prep.device)
+    self._ws = torch.empty(int(_lib.lib().bz_line_search_workspace_bytes(min(max(n, 1), limit))), dtype=torch.uint8, device=prep.device)
     status = self.record.data_ptr() + 8 * (self.record.numel() - 1)
     self._fn = _lib.lib().bz_line_search
     self._args = (_SEARCH_RULES[gar], prep.ptrs, prep.n, int(f_real), int(f_decl), _SEARCH_KINDS[kind], int(bool(negative)),
@@ -649,8 +656,10 @@ def line_search(gar, grad_honests, f_real, f_decl, grad_avg, grad_att, evals, ne
 
 def avg_dev_max_async(samples):
   """ (avg, stats): the average of the rows and a DEVICE fp64 vector [2 + n]:
-  stats[0] = ||avg||^2, stats[1] = max |avg|, stats[2 + i] = ||samples[i] - avg||^2.  No sync. """
-  prep = _prepare_device(samples, "the study metrics take CUDA tensors (tools.compute_avg_dev_max handles CPU samples)")
+  stats[0] = ||avg||^2, stats[1] = max |avg|, stats[2 + i] = ||samples[i] - avg||^2.  No sync.
+  Up to MAX_N_COORDINATE rows. """
+  prep = _prepare_device(samples, "the study metrics take CUDA tensors (tools.compute_avg_dev_max handles CPU samples)",
+                         limit=_lib.MAX_N_COORDINATE)
   avg = torch.empty(prep.d, dtype=torch.float32, device=prep.device)
   stats = torch.empty(2 + prep.n, dtype=torch.float64, device=prep.device)
   ws = _workspace(prep.device, prep.stream)
@@ -891,8 +900,8 @@ def study_step(grad_sampleds, grad_honests, grad_attacks, grad_defense, pasts, m
 # ---------------------------------------------------------------------------- #
 # Phases of the d-sharded multi-GPU path (device tensors only)
 
-def _prepare_device(gradients, message="the sharded phases take CUDA tensors"):
-  prep = _prepare(gradients)
+def _prepare_device(gradients, message="the sharded phases take CUDA tensors", limit=_lib.MAX_N):
+  prep = _prepare(gradients, limit=limit)
   if prep.to_cpu:
     raise ValueError(message)
   return prep

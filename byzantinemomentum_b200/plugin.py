@@ -71,7 +71,7 @@ def install_tools(tools):
   from . import engine, _lib
   stock = tools.compute_avg_dev_max
   def compute_avg_dev_max(samples):
-    if len(samples) > 0 and samples[0].is_cuda and len(samples) <= _lib.MAX_N:
+    if len(samples) > 0 and samples[0].is_cuda and len(samples) <= _lib.MAX_N_COORDINATE:
       return engine.compute_avg_dev_max(samples)
     return stock(samples)
   compute_avg_dev_max.__doc__ = stock.__doc__
@@ -87,17 +87,19 @@ def _is_cuda(tensors):
 def _device_rule(defense, grad_honests, f_real, f_decl, model):
   """ The name of the rule here that `defense` is, when the attack's search can run on the device:
   `defense` is an entry `install` registered, there are Byzantine rows to generate, every honest
-  gradient is a float32 CUDA vector, the rule's input fits BZ_MAX_N rows, and the rule accepts its
-  parameters.  None otherwise: the stock attack then runs (and fails, if it must, as it always did). """
+  gradient is a float32 CUDA vector, the rule's input fits the search's row limit for that rule
+  (`engine.search_max_rows`: 128 rows for the coordinate-wise rules, 64 for the distance rules), and the
+  rule accepts its parameters.  None otherwise: the stock attack then runs (and fails, if it must, as it
+  always did). """
   import torch
-  from . import _lib
+  from . import engine
   try:
     name = _installed.get(defense)
   except TypeError:                            # unhashable: not one of ours
     return None
   if name is None or not isinstance(f_real, int) or f_real < 1 or not isinstance(grad_honests, list) or not grad_honests:
     return None
-  if len(grad_honests) + f_real > _lib.MAX_N or not _is_cuda(grad_honests):
+  if len(grad_honests) + f_real > engine.search_max_rows(name) or not _is_cuda(grad_honests):
     return None
   if any(g.dtype != torch.float32 or g.dim() != 1 for g in grad_honests):
     return None
@@ -157,7 +159,7 @@ def install_attacks(attacks, backend=None):
   and `defense` is a rule `install` registered, run the whole `line_maximize` search on the device and
   read its outcome once (`engine.line_search`).  The attack direction is computed with the reference's
   torch statements.  Every other call — positive factors, a `--gars` mixture, a stock rule, CPU tensors,
-  more than BZ_MAX_N rows — runs the stock attack unchanged.  The reference's `register` builds the
+  more rows than the search takes for the rule (`engine.search_max_rows`) — runs the stock attack unchanged.  The reference's `register` builds the
   checked wrappers, with the stock checks.
   Args:
     attacks  The imported reference `attacks` package

@@ -518,9 +518,10 @@ class _SearchShard:
     honest = list(grad_honests)
     f_real = int(f_real)
     n = len(honest) + f_real
-    if f_real < 1 or n > _lib.MAX_N:
-      raise ValueError(f"f_real = {f_real} with {len(honest)} honest rows: expected f_real >= 1 and at most {_lib.MAX_N} rows")
-    prep = _engine._prepare_device(honest, "the line search takes CUDA tensors")
+    limit = _engine.search_max_rows(gar)
+    if f_real < 1 or n > limit:
+      raise ValueError(f"f_real = {f_real} with {len(honest)} honest rows: expected f_real >= 1 and at most {limit} rows")
+    prep = _engine._prepare_device(honest, "the line search takes CUDA tensors", limit=limit)
     if not all(g.is_contiguous() for g in honest):
       raise ValueError("the line search takes contiguous honest gradients")
     for vector in [grad_avg] if grad_att is None else [grad_avg, grad_att]:
@@ -534,7 +535,7 @@ class _SearchShard:
     self.scores = torch.zeros(world, dtype=torch.float64, device=device)
     self.score = self.scores[:1] if world == 1 else torch.zeros(1, dtype=torch.float64, device=device)
     inputs = honest + [self.byz] * f_real
-    rows = self._rows = _engine._prepare_device(inputs)
+    rows = self._rows = _engine._prepare_device(inputs, limit=limit)
     ws = self._ws = _engine._workspace(device, stream)
     lib = _lib.lib()
     state, out, avg = self._state.data_ptr(), self.out.data_ptr(), grad_avg.data_ptr()

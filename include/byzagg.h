@@ -28,7 +28,8 @@
  *   - Return value: 0 on success, a negative BZ_E* code otherwise; bz_last_error() returns
  *     a thread-local message for the last failure.
  *   - 1 <= n <= bz_max_n() (= 64), d >= 0 (d = 0 is a no-op).  The coordinate-wise rules take up
- *     to 128 rows through bz_coordinate (byzagg_coordinate.h, included at the end).
+ *     to 128 rows through bz_coordinate (byzagg_coordinate.h, included at the end), and so do
+ *     bz_avg_dev_max and bz_line_search with a coordinate-wise rule.
  *   - Parameter validity (f, m ranges) is the caller's job, exactly like the reference's
  *     `check()` functions; the library only rejects what it cannot execute.
  */
@@ -238,7 +239,8 @@ BZ_API int bz_bulyan_reduce(const float* const* rows, int n, int f, int m, const
  * stats[0] = sum_k avg[k]^2, stats[1] = max_k |avg[k]|, stats[2+i] = sum_k (g_i[k] - avg[k])^2.
  * avg: device fp32[d]; stats: device double[2+n].  One pass over the rows instead of n+2 with
  * n+2 host syncs; the caller derives norm_avg = sqrt(stats[0]) and
- * norm_dev = sqrt(sum_i stats[2+i] / (n-1)). */
+ * norm_dev = sqrt(sum_i stats[2+i] / (n-1)).  1 <= n <= BZ_MAX_N_COORDINATE (128); above 128,
+ * BZ_EUNSUPPORTED.  ws: bz_workspace_bytes(n) bytes, which is the same for every n >= 64. */
 BZ_API int bz_avg_dev_max(const float* const* rows, int n, int64_t d, float* avg, double* stats,
                           void* ws, size_t ws_bytes, void* stream);
 

@@ -28,7 +28,8 @@ extern "C" {
 #define BZ_ATTACK_IDENTICAL     0   /* byz = fl32(avg + fl32(fl32(s) * att)), s = -x when negative, else x */
 #define BZ_ATTACK_EMPIRE_STRICT 1   /* byz = fl32(avg * fl32(-x)); att is not read */
 
-/* Bytes of device scratch bz_line_search needs for n = nh + f_real rows (multiple of 256). */
+/* Bytes of device scratch bz_line_search needs for n = nh + f_real rows (multiple of 256); n up to
+ * BZ_MAX_N_COORDINATE, the same for every n >= 64. */
 BZ_API size_t bz_line_search_workspace_bytes(int n);
 
 /* `line_maximize(scape, evals, start=0., delta=1., ratio=0.8)` over the rule `rule` (defaults: Multi-Krum
@@ -38,7 +39,9 @@ BZ_API size_t bz_line_search_workspace_bytes(int n);
  * The search state is fp64 and follows tools/misc.py:468-513 operation for operation (NaN scores never
  * win a comparison), so the same y values give the same x sequence, bit for bit.  The score is K2''s
  * deterministic fp32-then-fp64 sum, not ATen's `dot` order.
- *   honest      HOST array of nh DEVICE pointers (fp32[d], 4-byte aligned), 1 <= nh, nh + f_real <= BZ_MAX_N
+ *   honest      HOST array of nh DEVICE pointers (fp32[d], 4-byte aligned), 1 <= nh, and nh + f_real at most
+ *               BZ_MAX_N_COORDINATE (128) for BZ_RULE_AVERAGE .. BZ_RULE_MEAMED, BZ_MAX_N (64) for the
+ *               distance rules (BZ_EUNSUPPORTED above)
  *   f_real      copies of the candidate row in the rule's input, >= 1
  *   kind        BZ_ATTACK_*; negative applies to BZ_ATTACK_IDENTICAL only
  *   avg, att    DEVICE fp32[d]: honest average and attack direction (att unused by empire-strict)
