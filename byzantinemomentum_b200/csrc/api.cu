@@ -5,6 +5,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <type_traits>
+#include <utility>
 
 #include "launch.cuh"
 #include "dist.cuh"
@@ -89,40 +90,69 @@ static int dedupe_rows(const float* const* rows, int n, const float** uniq, int*
   return u;
 }
 
-static bool launch_median(int n, const RowTable& t, const Geom& g, float* out, cudaStream_t st) {
-  return launch_median_part0(n, t, g, out, st) || launch_median_part1(n, t, g, out, st) ||
-         launch_median_part2(n, t, g, out, st) || launch_median_part3(n, t, g, out, st);
-}
-static bool launch_sorted(int n, const RowTable& t, const Geom& g, int mode, int f, float* out, cudaStream_t st) {
-  return launch_sorted_part4(n, t, g, mode, f, out, st) || launch_sorted_part5(n, t, g, mode, f, out, st) ||
-         launch_sorted_part6(n, t, g, mode, f, out, st) || launch_sorted_part7(n, t, g, mode, f, out, st);
+// The pointer table the kernels of n rows take, RowTable up to kMaxN rows and WideRowTable above, handed to `fn`.
+template <class Fn>
+static void with_table(const float* const* rows, int n, Fn fn) {
+  if (n > kMaxN) {
+    WideRowTable t;
+    fill_table(t, rows, n);
+    fn(t);
+  } else {
+    RowTable t;
+    fill_table(t, rows, n);
+    fn(t);
+  }
 }
 
+// First n of every range of K1's kernels: each has a median and a sorted object in the Makefile (K1FIRST).
+using K1Ranges = std::integer_sequence<int, 1, 17, 33, 49, 65, 73, 81, 89, 97, 105, 113, 121>;
+
+// The launcher of the range that holds n.  A range whose kernels take the other table never does.
+template <int FIRST, class Rows>
+static bool median_range(int n, const Rows& t, const Geom& g, float* out, cudaStream_t st) {
+  if constexpr (std::is_same<Rows, RowsOf<FIRST>>::value) return launch_median_range<FIRST>(n, t, g, out, st);
+  else return false;
+}
+template <int FIRST, class Rows>
+static bool sorted_range(int n, const Rows& t, const Geom& g, int mode, int f, float* out, cudaStream_t st) {
+  if constexpr (std::is_same<Rows, RowsOf<FIRST>>::value) return launch_sorted_range<FIRST>(n, t, g, mode, f, out, st);
+  else return false;
+}
+template <class Rows, int... FIRST>
+static bool launch_median(std::integer_sequence<int, FIRST...>, int n, const Rows& t, const Geom& g, float* out, cudaStream_t st) {
+  return (median_range<FIRST>(n, t, g, out, st) || ...);
+}
+template <class Rows, int... FIRST>
+static bool launch_sorted(std::integer_sequence<int, FIRST...>, int n, const Rows& t, const Geom& g, int mode, int f, float* out, cudaStream_t st) {
+  return (sorted_range<FIRST>(n, t, g, mode, f, out, st) || ...);
+}
+// The (n, f) specialisations exist up to kMaxN rows only.
+static bool launch_special(int n, const RowTable& t, const Geom& g, int mode, int f, float* out, cudaStream_t st) {
+  return (mode == kModeTrmean) ? launch_trmean_special(n, f, t, g, out, st)
+       : (mode == kModePhocas) ? launch_phocas_special(n, f, t, g, out, st)
+                               : launch_meamed_special(n, f, t, g, out, st);
+}
+static bool launch_special(int, const WideRowTable&, const Geom&, int, int, float*, cudaStream_t) { return false; }
+
 int run_median(const float* const* rows, int n, int64_t d, float* out, cudaStream_t st) {
-  RowTable t;
-  fill_table(t, rows, n);
-  launch_median(n, t, make_geom(rows, n, out, nullptr, d, body_vec(n)), out, st);
+  const Geom g = make_geom(rows, n, out, nullptr, d, body_vec(n));
+  with_table(rows, n, [&](const auto& t) { launch_median(K1Ranges{}, n, t, g, out, st); });
   return check_launch("k1_median");
 }
 
 int run_sorted(const float* const* rows, int n, int mode, int f, int64_t d, float* out, cudaStream_t st) {
-  RowTable t;
-  fill_table(t, rows, n);
   const Geom g = make_geom(rows, n, out, nullptr, d, body_vec(n));
-  const bool special = (mode == kModeTrmean) ? launch_trmean_special(n, f, t, g, out, st)
-                     : (mode == kModePhocas) ? launch_phocas_special(n, f, t, g, out, st)
-                                             : launch_meamed_special(n, f, t, g, out, st);
-  if (!special) launch_sorted(n, t, g, mode, f, out, st);
+  with_table(rows, n, [&](const auto& t) {
+    if (!launch_special(n, t, g, mode, f, out, st)) launch_sorted(K1Ranges{}, n, t, g, mode, f, out, st);
+  });
   return check_launch("k1_sorted");
 }
 
 int run_average_selected(const float* const* rows, int n, const int32_t* sel, int count, int zero_init,
                          float divisor, const int32_t* status, int64_t d, float* out, cudaStream_t st, int reverse = 0) {
-  RowTable t;
-  fill_table(t, rows, n);
   Geom g = make_geom(rows, n, out, nullptr, d, 4);
   g.reverse = reverse;
-  launch_average(t, g, sel, count, zero_init, divisor, status, out, st);
+  with_table(rows, n, [&](const auto& t) { launch_average(t, g, sel, count, zero_init, divisor, status, out, st); });
   return check_launch("k3_average");
 }
 
@@ -132,36 +162,23 @@ static int check_f_trim(int n, int f, const char* who) {
   return BZ_OK;
 }
 
-// kMaxN < n <= kMaxNCoordinate: the WideRowTable kernels, VEC = 1 for K1 (a column of up to 128
-// values per thread), the widest common vector for K3.
-static bool launch_median_wide(int n, const WideRowTable& t, const Geom& g, float* out, cudaStream_t st) {
-  return launch_median_wide_part11(n, t, g, out, st) || launch_median_wide_part12(n, t, g, out, st) ||
-         launch_median_wide_part13(n, t, g, out, st) || launch_median_wide_part14(n, t, g, out, st) ||
-         launch_median_wide_part15(n, t, g, out, st) || launch_median_wide_part16(n, t, g, out, st) ||
-         launch_median_wide_part17(n, t, g, out, st) || launch_median_wide_part18(n, t, g, out, st);
-}
-static bool launch_sorted_wide(int n, const WideRowTable& t, const Geom& g, int mode, int f, float* out, cudaStream_t st) {
-  return launch_sorted_wide_part19(n, t, g, mode, f, out, st) || launch_sorted_wide_part20(n, t, g, mode, f, out, st) ||
-         launch_sorted_wide_part21(n, t, g, mode, f, out, st) || launch_sorted_wide_part22(n, t, g, mode, f, out, st) ||
-         launch_sorted_wide_part23(n, t, g, mode, f, out, st) || launch_sorted_wide_part24(n, t, g, mode, f, out, st) ||
-         launch_sorted_wide_part25(n, t, g, mode, f, out, st) || launch_sorted_wide_part26(n, t, g, mode, f, out, st);
+// The launches of coordinate-wise rule `rule` over checked rows, d >= 1.
+static int run_coordinate(int rule, const float* const* rows, int n, int f, int64_t d, float* out, cudaStream_t st) {
+  switch (rule) {
+    case BZ_RULE_AVERAGE: return run_average_selected(rows, n, nullptr, n, 1, (float)n, nullptr, d, out, st);
+    case BZ_RULE_MEDIAN:  return run_median(rows, n, d, out, st);
+    case BZ_RULE_TRMEAN:  return run_sorted(rows, n, kModeTrmean, f, d, out, st);
+    case BZ_RULE_PHOCAS:  return run_sorted(rows, n, kModePhocas, f, d, out, st);
+    default:              return run_sorted(rows, n, kModeMeamed, f, d, out, st);
+  }
 }
 
-static int run_coordinate_wide(int rule, const float* const* rows, int n, int f, int64_t d, float* out, cudaStream_t st) {
-  WideRowTable t;
-  fill_table(t, rows, n);
-  if (rule == BZ_RULE_AVERAGE) {
-    launch_average(t, make_geom(rows, n, out, nullptr, d, 4), nullptr, n, 1, (float)n, nullptr, out, st);
-    return check_launch("k3_average");
-  }
-  const Geom g = make_geom(rows, n, out, nullptr, d, 1);
-  if (rule == BZ_RULE_MEDIAN) {
-    launch_median_wide(n, t, g, out, st);
-    return check_launch("k1_median");
-  }
-  const int mode = (rule == BZ_RULE_TRMEAN) ? kModeTrmean : (rule == BZ_RULE_PHOCAS) ? kModePhocas : kModeMeamed;
-  launch_sorted_wide(n, t, g, mode, f, out, st);
-  return check_launch("k1_sorted");
+// Entry point `who` of a coordinate-wise rule, for up to max_n rows.
+static int coordinate_entry(const char* who, int max_n, int rule, const float* const* rows, int n, int f, int64_t d, float* out, void* stream) {
+  if (int rc = check_rows(rows, n, d, out, who, max_n)) return rc;
+  if (rule >= BZ_RULE_TRMEAN) if (int rc = check_f_trim(n, f, who)) return rc;
+  if (d == 0) return BZ_OK;
+  return run_coordinate(rule, rows, n, f, d, out, (cudaStream_t)stream);
 }
 
 }  // namespace bz
@@ -175,36 +192,19 @@ int bz_max_n(void) { return kMaxN; }
 const char* bz_last_error(void) { return g_error; }
 
 int bz_average(const float* const* rows, int n, int64_t d, float* out, void* stream) {
-  if (int rc = check_rows(rows, n, d, out, "bz_average")) return rc;
-  if (d == 0) return BZ_OK;
-  return run_average_selected(rows, n, nullptr, n, 1, (float)n, nullptr, d, out, (cudaStream_t)stream);
+  return coordinate_entry("bz_average", kMaxN, BZ_RULE_AVERAGE, rows, n, 0, d, out, stream);
 }
-
 int bz_median(const float* const* rows, int n, int64_t d, float* out, void* stream) {
-  if (int rc = check_rows(rows, n, d, out, "bz_median")) return rc;
-  if (d == 0) return BZ_OK;
-  return run_median(rows, n, d, out, (cudaStream_t)stream);
+  return coordinate_entry("bz_median", kMaxN, BZ_RULE_MEDIAN, rows, n, 0, d, out, stream);
 }
-
 int bz_trmean(const float* const* rows, int n, int f, int64_t d, float* out, void* stream) {
-  if (int rc = check_rows(rows, n, d, out, "bz_trmean")) return rc;
-  if (int rc = check_f_trim(n, f, "bz_trmean")) return rc;
-  if (d == 0) return BZ_OK;
-  return run_sorted(rows, n, kModeTrmean, f, d, out, (cudaStream_t)stream);
+  return coordinate_entry("bz_trmean", kMaxN, BZ_RULE_TRMEAN, rows, n, f, d, out, stream);
 }
-
 int bz_phocas(const float* const* rows, int n, int f, int64_t d, float* out, void* stream) {
-  if (int rc = check_rows(rows, n, d, out, "bz_phocas")) return rc;
-  if (int rc = check_f_trim(n, f, "bz_phocas")) return rc;
-  if (d == 0) return BZ_OK;
-  return run_sorted(rows, n, kModePhocas, f, d, out, (cudaStream_t)stream);
+  return coordinate_entry("bz_phocas", kMaxN, BZ_RULE_PHOCAS, rows, n, f, d, out, stream);
 }
-
 int bz_meamed(const float* const* rows, int n, int f, int64_t d, float* out, void* stream) {
-  if (int rc = check_rows(rows, n, d, out, "bz_meamed")) return rc;
-  if (int rc = check_f_trim(n, f, "bz_meamed")) return rc;
-  if (d == 0) return BZ_OK;
-  return run_sorted(rows, n, kModeMeamed, f, d, out, (cudaStream_t)stream);
+  return coordinate_entry("bz_meamed", kMaxN, BZ_RULE_MEAMED, rows, n, f, d, out, stream);
 }
 
 int bz_average_selected(const float* const* rows, int n, const int32_t* sel, int count, int zero_init,
@@ -262,6 +262,7 @@ int bz_coordinate_host(int rule, const float* const* host_rows, int n, int f, in
   if (rule >= BZ_RULE_TRMEAN) if (int rc = check_f_trim(n, f, "bz_coordinate_host")) return rc;
   if (d == 0) return BZ_OK;
   if (staging == nullptr || dev_out == nullptr) return fail(BZ_EINVAL, "bz_coordinate_host: staging / dev_out is NULL");
+  if ((((uintptr_t)staging | (uintptr_t)dev_out) % sizeof(float)) != 0) return fail(BZ_EINVAL, "bz_coordinate_host: staging / dev_out is not 4-byte aligned");
   if (pitch < d || pitch % 4 != 0) return fail(BZ_EINVAL, "bz_coordinate_host: pitch = %lld must be >= d and a multiple of 4 floats", (long long)pitch);
   if (chunks < 1 || chunks > BZ_MAX_HOST_CHUNKS) return fail(BZ_EINVAL, "bz_coordinate_host: chunks = %d outside 1..%d", chunks, BZ_MAX_HOST_CHUNKS);
   cudaStream_t st = (cudaStream_t)stream, sin = (cudaStream_t)in_stream, sout = (cudaStream_t)out_stream;
@@ -295,13 +296,7 @@ int bz_coordinate_host(int rule, const float* const* host_rows, int n, int f, in
     h2d_rows(dsts, srcs, u, (size_t)cnt * sizeof(float), sin);
     if (sin != st) cudaStreamWaitEvent(st, event_on(sin), 0);
     for (int i = 0; i < n; ++i) dev_rows[i] = staging + (size_t)slot[i] * pitch + c0;
-    switch (rule) {
-      case BZ_RULE_AVERAGE: rc = bz_average(dev_rows, n, cnt, dev_out + c0, stream); break;
-      case BZ_RULE_MEDIAN:  rc = bz_median(dev_rows, n, cnt, dev_out + c0, stream); break;
-      case BZ_RULE_TRMEAN:  rc = bz_trmean(dev_rows, n, f, cnt, dev_out + c0, stream); break;
-      case BZ_RULE_PHOCAS:  rc = bz_phocas(dev_rows, n, f, cnt, dev_out + c0, stream); break;
-      default:              rc = bz_meamed(dev_rows, n, f, cnt, dev_out + c0, stream); break;
-    }
+    rc = run_coordinate(rule, dev_rows, n, f, cnt, dev_out + c0, st);
     if (rc != BZ_OK) break;
     if (sout != st) cudaStreamWaitEvent(sout, event_on(st), 0);
     cudaMemcpyAsync(host_out + c0, dev_out + c0, (size_t)cnt * sizeof(float), cudaMemcpyDeviceToHost, sout);
@@ -315,17 +310,7 @@ int bz_coordinate_host(int rule, const float* const* host_rows, int n, int f, in
 
 int bz_coordinate(int rule, const float* const* rows, int n, int f, int64_t d, float* out, void* stream) {
   if (rule < BZ_RULE_AVERAGE || rule > BZ_RULE_MEAMED) return fail(BZ_EINVAL, "bz_coordinate: unknown rule %d", rule);
-  if (int rc = check_rows(rows, n, d, out, "bz_coordinate", kMaxNCoordinate)) return rc;
-  if (rule >= BZ_RULE_TRMEAN) if (int rc = check_f_trim(n, f, "bz_coordinate")) return rc;
-  if (d == 0) return BZ_OK;
-  if (n > kMaxN) return run_coordinate_wide(rule, rows, n, f, d, out, (cudaStream_t)stream);
-  switch (rule) {
-    case BZ_RULE_AVERAGE: return bz_average(rows, n, d, out, stream);
-    case BZ_RULE_MEDIAN:  return bz_median(rows, n, d, out, stream);
-    case BZ_RULE_TRMEAN:  return bz_trmean(rows, n, f, d, out, stream);
-    case BZ_RULE_PHOCAS:  return bz_phocas(rows, n, f, d, out, stream);
-    default:              return bz_meamed(rows, n, f, d, out, stream);
-  }
+  return coordinate_entry("bz_coordinate", kMaxNCoordinate, rule, rows, n, f, d, out, stream);
 }
 
 }  // extern "C"

@@ -28,7 +28,9 @@ constexpr int kMaxNCoordinate = BZ_MAX_N_COORDINATE;
 struct WideRowTable {
   const float* p[kMaxNCoordinate];
 };
-template <int N> using RowsOf = typename std::conditional<(N <= kMaxN), RowTable, WideRowTable>::type;
+// BZ_MAX_N rather than kMaxN: RowsOf appears in the signatures of launch.cuh's function templates, and a
+// signature that names a constant of internal linkage would make their instantiations internal as well.
+template <int N> using RowsOf = typename std::conditional<(N <= BZ_MAX_N), RowTable, WideRowTable>::type;
 
 // Geometry of a launch over d coordinates with VEC per thread.  All rows (and the output)
 // share the same misalignment, so shifting the element index by `shift` (0..VEC-1) makes every

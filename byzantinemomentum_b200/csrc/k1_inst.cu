@@ -1,28 +1,27 @@
-// k1_inst.cu — instantiations of the K1 kernels for a range of n, compiled once per part
-// (`-DBZ_PART=<0..26>`) so that the kernels build in parallel.  Parts 0-3: k1_median for n in
-// 1-16 / 17-32 / 33-48 / 49-64; parts 4-7: generic k1_sorted for the same ranges; parts 8-10:
-// trimmed mean / phocas / meamed with (n, f) fixed at compile time for n = 11, 25, 51.
-// Parts 11-26 (bz_coordinate above 64 rows, VEC = 1): k1_median (11-18) and generic k1_sorted
-// (19-26) for n in 65-72 / 73-80 / ... / 121-128.
+// k1_inst.cu — instantiations of the K1 kernels, compiled once per family and range of n so that
+// the kernels build in parallel (the Makefile names each object after what it holds):
+//   -DBZ_MEDIAN_FROM=<first n>   k1_median for every n of the range
+//   -DBZ_SORTED_FROM=<first n>   generic k1_sorted for every n of the range
+//   -DBZ_SPECIAL=<0..2>          trimmed mean / phocas / meamed with (n, f) fixed at compile time for n = 11, 25, 51
+// A range is 16 sizes up to kMaxN rows and 8 above (VEC = 1, networks_wide_gen.cuh).
 #include "k1_select.cuh"
 
-#ifndef BZ_PART
-#error "compile with -DBZ_PART=<0..26>"
+#if defined(BZ_MEDIAN_FROM)
+#define BZ_FIRST BZ_MEDIAN_FROM
+#elif defined(BZ_SORTED_FROM)
+#define BZ_FIRST BZ_SORTED_FROM
+#elif !defined(BZ_SPECIAL)
+#error "compile with -DBZ_MEDIAN_FROM=<first n>, -DBZ_SORTED_FROM=<first n> or -DBZ_SPECIAL=<0..2>"
 #endif
 
-#if BZ_PART >= 11
+#ifdef BZ_FIRST
+#define BZ_N8(b) X((b)) X((b) + 1) X((b) + 2) X((b) + 3) X((b) + 4) X((b) + 5) X((b) + 6) X((b) + 7)
+#if BZ_FIRST > BZ_MAX_N
 #include "networks_wide_gen.cuh"
-#define BZ_WIDE_BASE (65 + 8 * ((BZ_PART - 11) % 8))
-#define BZ_N_LIST X(BZ_WIDE_BASE) X(BZ_WIDE_BASE + 1) X(BZ_WIDE_BASE + 2) X(BZ_WIDE_BASE + 3) \
-                  X(BZ_WIDE_BASE + 4) X(BZ_WIDE_BASE + 5) X(BZ_WIDE_BASE + 6) X(BZ_WIDE_BASE + 7)
-#elif (BZ_PART % 4) == 0
-#define BZ_N_LIST X(1) X(2) X(3) X(4) X(5) X(6) X(7) X(8) X(9) X(10) X(11) X(12) X(13) X(14) X(15) X(16)
-#elif (BZ_PART % 4) == 1
-#define BZ_N_LIST X(17) X(18) X(19) X(20) X(21) X(22) X(23) X(24) X(25) X(26) X(27) X(28) X(29) X(30) X(31) X(32)
-#elif (BZ_PART % 4) == 2
-#define BZ_N_LIST X(33) X(34) X(35) X(36) X(37) X(38) X(39) X(40) X(41) X(42) X(43) X(44) X(45) X(46) X(47) X(48)
+#define BZ_N_LIST BZ_N8(BZ_FIRST)
 #else
-#define BZ_N_LIST X(49) X(50) X(51) X(52) X(53) X(54) X(55) X(56) X(57) X(58) X(59) X(60) X(61) X(62) X(63) X(64)
+#define BZ_N_LIST BZ_N8(BZ_FIRST) BZ_N8(BZ_FIRST + 8)
+#endif
 #endif
 
 namespace bz {
@@ -41,54 +40,10 @@ static unsigned tile_grid(K kernel, size_t smem, int64_t nv, unsigned long long&
   return (unsigned)((nv + kK1Threads - 1) / kK1Threads);
 }
 
-#if BZ_PART >= 19
+#if defined(BZ_MEDIAN_FROM)
 
 template <int N>
-static void launch_sorted_wide_n(const WideRowTable& rows, const Geom& g, int mode, int f, float* out, cudaStream_t st) {
-  if (g.nv <= 0) return;
-  // the closest modes stage the sorted columns in shared memory (64 KB per CTA at n = 128)
-  static unsigned long long opted = 0;
-  const size_t smem = (mode == kModeTrmean) ? 0 : Stage<N, 1>::kColumnFloats * sizeof(float);
-  const auto kernel = k1_sorted_fn<N, 1, -1, -1>();
-  launch_after(kernel, tile_grid(kernel, smem, g.nv, opted), kK1Threads, smem, st, rows, g, mode, f, out);
-}
-
-#define BZ_FN2(p) launch_sorted_wide_part##p
-#define BZ_FN(p) BZ_FN2(p)
-bool BZ_FN(BZ_PART)(int n, const WideRowTable& rows, const Geom& g, int mode, int f, float* out, cudaStream_t st) {
-  switch (n) {
-#define X(N) case N: launch_sorted_wide_n<N>(rows, g, mode, f, out, st); return true;
-    BZ_N_LIST
-#undef X
-    default: return false;
-  }
-}
-
-#elif BZ_PART >= 11
-
-template <int N>
-static void launch_median_wide_n(const WideRowTable& rows, const Geom& g, float* out, cudaStream_t st) {
-  if (g.nv <= 0) return;
-  static unsigned long long opted = 0;
-  const auto kernel = k1_median_fn<N, 1>();
-  launch_after(kernel, tile_grid(kernel, 0, g.nv, opted), kK1Threads, 0, st, rows, g, out);
-}
-
-#define BZ_FN2(p) launch_median_wide_part##p
-#define BZ_FN(p) BZ_FN2(p)
-bool BZ_FN(BZ_PART)(int n, const WideRowTable& rows, const Geom& g, float* out, cudaStream_t st) {
-  switch (n) {
-#define X(N) case N: launch_median_wide_n<N>(rows, g, out, st); return true;
-    BZ_N_LIST
-#undef X
-    default: return false;
-  }
-}
-
-#elif BZ_PART < 4
-
-template <int N>
-static void launch_median_n(const RowTable& rows, const Geom& g, float* out, cudaStream_t st) {
+static void launch_median_n(const RowsOf<N>& rows, const Geom& g, float* out, cudaStream_t st) {
   if (g.nv <= 0) return;
   static unsigned long long opted = 0;
   if (g.vec == 1)
@@ -97,9 +52,8 @@ static void launch_median_n(const RowTable& rows, const Geom& g, float* out, cud
     launch_after(k1_median_fn<N, body_vec(N)>(), tile_grid(k1_median_fn<N, body_vec(N)>(), 0, g.nv, opted), kK1Threads, 0, st, rows, g, out);
 }
 
-#define BZ_FN2(p) launch_median_part##p
-#define BZ_FN(p) BZ_FN2(p)
-bool BZ_FN(BZ_PART)(int n, const RowTable& rows, const Geom& g, float* out, cudaStream_t st) {
+template <int FIRST>
+bool launch_median_range(int n, const RowsOf<FIRST>& rows, const Geom& g, float* out, cudaStream_t st) {
   switch (n) {
 #define X(N) case N: launch_median_n<N>(rows, g, out, st); return true;
     BZ_N_LIST
@@ -107,27 +61,27 @@ bool BZ_FN(BZ_PART)(int n, const RowTable& rows, const Geom& g, float* out, cuda
     default: return false;
   }
 }
+template bool launch_median_range<BZ_FIRST>(int, const RowsOf<BZ_FIRST>&, const Geom&, float*, cudaStream_t);
 
-#elif BZ_PART < 8
+#elif defined(BZ_SORTED_FROM)
 
 template <int N, int VEC>
-static void launch_sorted_nv(const RowTable& rows, const Geom& g, int mode, int f, float* out, cudaStream_t st) {
+static void launch_sorted_nv(const RowsOf<N>& rows, const Geom& g, int mode, int f, float* out, cudaStream_t st) {
   if (g.nv <= 0) return;
-  // the closest modes stage the sorted columns in shared memory
+  // the closest modes stage the sorted columns in shared memory (64 KB per CTA at n = 128)
   static unsigned long long opted = 0;
   const size_t smem = (mode == kModeTrmean) ? 0 : Stage<N, VEC>::kColumnFloats * sizeof(float);
   launch_after(k1_sorted_fn<N, VEC, -1, -1>(), tile_grid(k1_sorted_fn<N, VEC, -1, -1>(), smem, g.nv, opted), kK1Threads, smem, st, rows, g, mode, f, out);
 }
 
 template <int N>
-static void launch_sorted_n(const RowTable& rows, const Geom& g, int mode, int f, float* out, cudaStream_t st) {
+static void launch_sorted_n(const RowsOf<N>& rows, const Geom& g, int mode, int f, float* out, cudaStream_t st) {
   if (g.vec == 1) launch_sorted_nv<N, 1>(rows, g, mode, f, out, st);
   else            launch_sorted_nv<N, body_vec(N)>(rows, g, mode, f, out, st);
 }
 
-#define BZ_FN2(p) launch_sorted_part##p
-#define BZ_FN(p) BZ_FN2(p)
-bool BZ_FN(BZ_PART)(int n, const RowTable& rows, const Geom& g, int mode, int f, float* out, cudaStream_t st) {
+template <int FIRST>
+bool launch_sorted_range(int n, const RowsOf<FIRST>& rows, const Geom& g, int mode, int f, float* out, cudaStream_t st) {
   switch (n) {
 #define X(N) case N: launch_sorted_n<N>(rows, g, mode, f, out, st); return true;
     BZ_N_LIST
@@ -135,6 +89,7 @@ bool BZ_FN(BZ_PART)(int n, const RowTable& rows, const Geom& g, int mode, int f,
     default: return false;
   }
 }
+template bool launch_sorted_range<BZ_FIRST>(int, const RowsOf<BZ_FIRST>&, const Geom&, int, int, float*, cudaStream_t);
 
 #else
 
@@ -146,10 +101,10 @@ bool BZ_FN(BZ_PART)(int n, const RowTable& rows, const Geom& g, int mode, int f,
   Y(51, 1) Y(51, 2) Y(51, 3) Y(51, 4) Y(51, 5) Y(51, 6) Y(51, 7) Y(51, 8) Y(51, 9) Y(51, 10) Y(51, 11) Y(51, 12) Y(51, 13) \
   Y(51, 14) Y(51, 15) Y(51, 16) Y(51, 17) Y(51, 18) Y(51, 19) Y(51, 20) Y(51, 21) Y(51, 22) Y(51, 23) Y(51, 24) Y(51, 25)
 
-#if BZ_PART == 8
+#if BZ_SPECIAL == 0
 #define BZ_SPECIAL_MODE kModeTrmean
 #define BZ_SPECIAL_FN launch_trmean_special
-#elif BZ_PART == 9
+#elif BZ_SPECIAL == 1
 #define BZ_SPECIAL_MODE kModePhocas
 #define BZ_SPECIAL_FN launch_phocas_special
 #else

@@ -13,8 +13,8 @@
 //   k1_sorted<N, VEC, F, MODE>   trmean.py:24-50,69-109 sort, then trmean / phocas / meamed
 //
 // Up to N = kMaxN the kernels take the 64-pointer RowTable; above, up to kMaxNCoordinate
-// (bz_coordinate, VEC = 1 only), an overload of the same kernel takes the 128-pointer WideRowTable.
-// RowsOf<N> picks the table; the bodies are shared.
+// (VEC = 1 only), an overload of the same kernel takes the 128-pointer WideRowTable.
+// RowsOf<N> picks the table; the bodies, and the launchers of k1_inst.cu, are shared.
 //
 // F / MODE = -1 mean "run-time value": one generic kernel per (N, VEC) serves every f and the
 // three epilogues after a full sort.  For n = 11, 25, 51 (BASELINE.json's configs and the

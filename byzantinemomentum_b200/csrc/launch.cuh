@@ -34,44 +34,25 @@ inline cudaError_t launch_after(void (*kernel)(Params...), dim3 grid, dim3 block
 }
 
 // Elements per thread in the aligned body of a K1 launch: 4 (LDG.128) while 4n values fit
-// the register file comfortably, else 2 (LDG.64).  The scalar variant (1) serves the
-// unaligned head/tail and rows whose alignments disagree.
-__host__ __device__ constexpr int body_vec(int n) { return n <= 28 ? 4 : 2; }
+// the register file comfortably, else 2 (LDG.64); above kMaxN rows a column alone takes the
+// registers, so 1.  The scalar variant (1) also serves the unaligned head/tail and rows whose
+// alignments disagree.
+__host__ __device__ constexpr int body_vec(int n) { return n <= 28 ? 4 : n <= kMaxN ? 2 : 1; }
 
 // Epilogue of k1_sorted.
 enum SortedMode { kModeTrmean = 0, kModePhocas = 1, kModeMeamed = 2 };
 
-// K1 (k1_inst.cu, parts 0-10).  Parts 0-7 return false when n is outside the part's range;
-// launch_trmean_special returns false when (n, f) has no compile-time specialisation.
-bool launch_median_part0(int n, const RowTable& rows, const Geom& g, float* out, cudaStream_t st);
-bool launch_median_part1(int n, const RowTable& rows, const Geom& g, float* out, cudaStream_t st);
-bool launch_median_part2(int n, const RowTable& rows, const Geom& g, float* out, cudaStream_t st);
-bool launch_median_part3(int n, const RowTable& rows, const Geom& g, float* out, cudaStream_t st);
-bool launch_sorted_part4(int n, const RowTable& rows, const Geom& g, int mode, int f, float* out, cudaStream_t st);
-bool launch_sorted_part5(int n, const RowTable& rows, const Geom& g, int mode, int f, float* out, cudaStream_t st);
-bool launch_sorted_part6(int n, const RowTable& rows, const Geom& g, int mode, int f, float* out, cudaStream_t st);
-bool launch_sorted_part7(int n, const RowTable& rows, const Geom& g, int mode, int f, float* out, cudaStream_t st);
+// K1 (k1_inst.cu).  The kernels of each family are built in ranges of n, one object per range:
+// launch_*_range<FIRST> is instantiated by the object whose range starts at n = FIRST, takes the
+// table of those n and returns false when n is outside the range.  launch_*_special returns false
+// when (n, f) has no compile-time specialisation.
+template <int FIRST>
+bool launch_median_range(int n, const RowsOf<FIRST>& rows, const Geom& g, float* out, cudaStream_t st);
+template <int FIRST>
+bool launch_sorted_range(int n, const RowsOf<FIRST>& rows, const Geom& g, int mode, int f, float* out, cudaStream_t st);
 bool launch_trmean_special(int n, int f, const RowTable& rows, const Geom& g, float* out, cudaStream_t st);
 bool launch_phocas_special(int n, int f, const RowTable& rows, const Geom& g, float* out, cudaStream_t st);
 bool launch_meamed_special(int n, int f, const RowTable& rows, const Geom& g, float* out, cudaStream_t st);
-
-// K1 above kMaxN rows (k1_inst.cu parts 11-26, VEC = 1, eight n per part): false when n is outside the part's range.
-bool launch_median_wide_part11(int n, const WideRowTable& rows, const Geom& g, float* out, cudaStream_t st);
-bool launch_median_wide_part12(int n, const WideRowTable& rows, const Geom& g, float* out, cudaStream_t st);
-bool launch_median_wide_part13(int n, const WideRowTable& rows, const Geom& g, float* out, cudaStream_t st);
-bool launch_median_wide_part14(int n, const WideRowTable& rows, const Geom& g, float* out, cudaStream_t st);
-bool launch_median_wide_part15(int n, const WideRowTable& rows, const Geom& g, float* out, cudaStream_t st);
-bool launch_median_wide_part16(int n, const WideRowTable& rows, const Geom& g, float* out, cudaStream_t st);
-bool launch_median_wide_part17(int n, const WideRowTable& rows, const Geom& g, float* out, cudaStream_t st);
-bool launch_median_wide_part18(int n, const WideRowTable& rows, const Geom& g, float* out, cudaStream_t st);
-bool launch_sorted_wide_part19(int n, const WideRowTable& rows, const Geom& g, int mode, int f, float* out, cudaStream_t st);
-bool launch_sorted_wide_part20(int n, const WideRowTable& rows, const Geom& g, int mode, int f, float* out, cudaStream_t st);
-bool launch_sorted_wide_part21(int n, const WideRowTable& rows, const Geom& g, int mode, int f, float* out, cudaStream_t st);
-bool launch_sorted_wide_part22(int n, const WideRowTable& rows, const Geom& g, int mode, int f, float* out, cudaStream_t st);
-bool launch_sorted_wide_part23(int n, const WideRowTable& rows, const Geom& g, int mode, int f, float* out, cudaStream_t st);
-bool launch_sorted_wide_part24(int n, const WideRowTable& rows, const Geom& g, int mode, int f, float* out, cudaStream_t st);
-bool launch_sorted_wide_part25(int n, const WideRowTable& rows, const Geom& g, int mode, int f, float* out, cudaStream_t st);
-bool launch_sorted_wide_part26(int n, const WideRowTable& rows, const Geom& g, int mode, int f, float* out, cudaStream_t st);
 
 // K3 (k3_average.cu): ordered-subset average (the 128-pointer table: bz_coordinate's average above kMaxN rows).
 void launch_average(const RowTable& rows, const Geom& g, const int32_t* sel, int count,

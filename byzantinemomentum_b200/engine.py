@@ -355,12 +355,8 @@ def _coordinate_pipeline(name, gradients, f, path, device):
   return result
 
 def _coordinate_call(name, prep, f, out):
-  """ (fn, args) of the coordinate-wise rule `name` writing to the address `out`: `bz_<name>` up to
-  MAX_N rows, `bz_coordinate` above. """
-  if prep.n > _lib.MAX_N:
-    return _lib.lib().bz_coordinate, (_RULE_CODES[name], prep.ptrs, prep.n, 0 if f is None else int(f), prep.d, out, prep.stream)
-  head = (prep.ptrs, prep.n, int(f)) if name in ("trmean", "phocas", "meamed") else (prep.ptrs, prep.n)
-  return getattr(_lib.lib(), "bz_" + name), head + (prep.d, out, prep.stream)
+  """ (fn, args) of the coordinate-wise rule `name` writing to the address `out`. """
+  return _lib.lib().bz_coordinate, (_RULE_CODES[name], prep.ptrs, prep.n, 0 if f is None else int(f), prep.d, out, prep.stream)
 
 def _coordinate(name, gradients, f=None):
   if type(gradients) in (list, tuple) and len(gradients) > 0 and isinstance(gradients[0], torch.Tensor) and gradients[0].device.type == "cpu" and torch.cuda.is_available():
