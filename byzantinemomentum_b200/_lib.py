@@ -1,7 +1,7 @@
 # coding: utf-8
 """ctypes binding of `libbyzagg.so` (C ABI: `include/byzagg.h`, `include/byzagg_shards.h`,
-`include/byzagg_attack.h`, `include/byzagg_search_shards.h`, `include/byzagg_search_peers.h` and
-`include/byzagg_coordinate.h`).
+`include/byzagg_attack.h`, `include/byzagg_search_shards.h`, `include/byzagg_search_peers.h`,
+`include/byzagg_coordinate.h` and `include/byzagg_peers_next.h`).
 
 The library is loaded lazily, on the first call that needs it, and the load FAILS LOUDLY:
 there is no CPU or PyTorch fallback anywhere in this package.  Build it in-tree with
@@ -106,6 +106,15 @@ SEARCH_PEER_SIGNATURES = {
   "bz_rowdist_peers": (_i, [_i, _c_rows, _i, _i, _i, _vp, _i64, _vp, _vp, _vp, _i, _i, _c_rows, _c_rows, ctypes.c_uint, _vp, _sz, _vp]),
   "bz_search_score_peers": (_i, [_vp, _vp, _i64, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _c_rows, _c_rows, ctypes.c_uint, _vp, _sz, _vp]),
 }
+# the same for include/byzagg_peers_next.h (the exchanges over peer memory with the epoch taken from the buffer)
+PEER_NEXT_SIGNATURES = {
+  "bz_krum_peers_next": (_i, [_c_rows, _i, _i, _i, _i64, _vp, _vp, _vp, _i, _i, _c_rows, _c_rows, _vp, _sz, _vp]),
+  "bz_bulyan_peers_next": (_i, [_c_rows, _i, _i, _i, _i64, _vp, _vp, _vp, _i, _i, _c_rows, _c_rows, _vp, _sz, _vp]),
+  "bz_pairdist_reuse_peers_next": (_i, [_i, _c_rows, _i, _i, _i, _i64, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _i, _i, _c_rows,
+                                        _c_rows, _vp, _sz, _vp]),
+  "bz_rowdist_peers_next": (_i, [_i, _c_rows, _i, _i, _i, _vp, _i64, _vp, _vp, _vp, _i, _i, _c_rows, _c_rows, _vp, _sz, _vp]),
+  "bz_search_score_peers_next": (_i, [_vp, _vp, _i64, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _c_rows, _c_rows, _vp, _sz, _vp]),
+}
 # the same for include/byzagg_coordinate.h (the coordinate-wise rules up to MAX_N_COORDINATE rows)
 COORDINATE_SIGNATURES = {
   "bz_coordinate": (_i, [_i, _c_rows, _i, _i, _i64, _vp, _vp]),
@@ -132,7 +141,7 @@ def lib():
       except OSError as err:
         raise LibraryError(f"unable to load {path}: {err}") from err
       tables = (SIGNATURES, SHARD_SIGNATURES, ATTACK_SIGNATURES, SEARCH_SHARD_SIGNATURES, SEARCH_PEER_SIGNATURES,
-                COORDINATE_SIGNATURES)
+                COORDINATE_SIGNATURES, PEER_NEXT_SIGNATURES)
       for name, (restype, argtypes) in [item for table in tables for item in table.items()]:
         try:
           fn = getattr(handle, name)

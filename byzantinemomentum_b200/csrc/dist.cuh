@@ -59,9 +59,12 @@ struct SelectTail {
   int u_old;
   double* cache_out;
   int reused;
-  // fused exchange over peer memory (bz_*_peers): nranks > 0
+  // fused exchange over peer memory (bz_*_peers): nranks > 0.  By value: the tables hold nranks pointers
+  // (this step's slot); `next` (bz_*_peers_next): 2 * nranks, slot 0's then slot 1's, and the kernel takes
+  // the epoch and the slot from the flags (peers.cuh, next_epoch); `epoch` is unused
   int nranks, rank;
   unsigned epoch;
+  int next;
   double* const* peer_blocks;
   unsigned* const* peer_flags;
 };
@@ -88,10 +91,12 @@ int launch_rowdist(const RowTable& rows, int n, const float* const* host_rows, c
 struct PeerTail {
   int nranks, rank;
   unsigned epoch;
+  int next;                        // 1 (bz_*_peers_next): epoch and slot from the flags (next_epoch), `epoch` unused
   int32_t* status;                 // rowdist: 0, or BZ_STATUS_PEER_TIMEOUT; search: the search's status word,
                                    // set to BZ_STATUS_PEER_TIMEOUT on a timeout after the transition
-  double* block[BZ_MAX_PEERS];     // this step's slot on every rank ([rank] is local)
-  unsigned* flag[BZ_MAX_PEERS];    // this step's flag array (nranks words) on every rank
+  double* block[2][BZ_MAX_PEERS];  // [slot][rank]: the slot on every rank ([rank] is local); by value, [0] is
+                                   // this step's slot and [1] is unused
+  unsigned* flag[2][BZ_MAX_PEERS]; // the same for the flag arrays (nranks words each)
 };
 // K2' over the rows against `center` (NULL: the origin) in bz_rowdist_partial's geometry, its last CTA
 // summing the blocks in k_reduce_parts's order (the block the collective path all-gathers), exchanging

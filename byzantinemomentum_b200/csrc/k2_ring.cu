@@ -88,8 +88,10 @@ struct RingTail {
   // table on every rank) and scores.
   int nranks, rank;                       // nranks == 0: single GPU
   unsigned epoch;                         // step number, > the previous step's
-  double* peer_block[BZ_MAX_PEERS];       // this step's slot on every rank ([rank] is local)
-  unsigned* peer_flag[BZ_MAX_PEERS];      // this step's flag array (nranks words) on every rank
+  int next;                               // 1 (bz_*_peers_next): epoch and slot from the flags (next_epoch)
+  double* peer_block[2][BZ_MAX_PEERS];    // [slot][rank]: the slot on every rank ([rank] is local); by value,
+                                          // [0] is this step's slot and [1] is unused
+  unsigned* peer_flag[2][BZ_MAX_PEERS];   // the same for the flag arrays (nranks words each)
 };
 
 // New rows of a reuse call: star task = one new row against 25 consecutive rows.
@@ -612,8 +614,18 @@ k2_ring(const __grid_constant__ RowTable rows, const __grid_constant__ SelfList 
               local[e] = v;
               if (tail.cache_out != nullptr) tail.cache_out[e] = v;
             }
+            // the epoch and the slot: by value, or (`next`) from this rank's own flags, read by every thread
+            // before the barrier that precedes the signal
+            unsigned epoch = tail.epoch;
+            int slot = 0;
+            if (tail.next) {
+              epoch = next_epoch(tail.peer_flag[0][tail.rank] + tail.rank, tail.peer_flag[1][tail.rank] + tail.rank);
+              slot = (int)(epoch & 1u);
+            }
+            double* const* blocks = tail.peer_block[slot];
+            unsigned* const* flags = tail.peer_flag[slot];
             __syncthreads();
-            double* mine = tail.peer_block[tail.rank];
+            double* mine = blocks[tail.rank];
             for (int e = threadIdx.x; e < NN; e += kThreads) {
               const int i = e / N, j = e - i * N;
               double v = 0.;
@@ -628,14 +640,14 @@ k2_ring(const __grid_constant__ RowTable rows, const __grid_constant__ SelfList 
             __syncthreads();
             // flag, bounded wait (peers.cuh): a peer that never shows up sets the status word
             if ((int)threadIdx.x < tail.nranks &&
-                peer_signal_wait(tail.peer_flag[threadIdx.x] + tail.rank, tail.peer_flag[tail.rank] + threadIdx.x, tail.epoch))
+                peer_signal_wait(flags[threadIdx.x] + tail.rank, flags[tail.rank] + threadIdx.x, epoch))
               peer_timeout = 1;
             __syncthreads();
             asm volatile("" ::: "memory");      // the block loads below stay below the flag wait
             for (int e = threadIdx.x; e < NN; e += kThreads) {
               double part[BZ_MAX_PEERS];
 #pragma unroll
-              for (int r = 0; r < BZ_MAX_PEERS; ++r) part[r] = (r < tail.nranks) ? ld_relaxed_sys_f64(tail.peer_block[r] + e) : 0.;
+              for (int r = 0; r < BZ_MAX_PEERS; ++r) part[r] = (r < tail.nranks) ? ld_relaxed_sys_f64(blocks[r] + e) : 0.;
               double v = part[0];
 #pragma unroll
               for (int r = 1; r < BZ_MAX_PEERS; ++r) v += part[r];      // rank order; + 0.0 past nranks is exact
@@ -797,11 +809,12 @@ int launch_pairdist_ring(const RowTable& rows, int n, int64_t d, double* parts, 
     tail.u_old = select->u_old;
     select->reused = 0;
     if (select->nranks > 0) {
-      tail.nranks = select->nranks; tail.rank = select->rank; tail.epoch = select->epoch;
-      for (int r = 0; r < BZ_MAX_PEERS; ++r) {
-        tail.peer_block[r] = select->peer_blocks[r < select->nranks ? r : 0];
-        tail.peer_flag[r] = select->peer_flags[r < select->nranks ? r : 0];
-      }
+      tail.nranks = select->nranks; tail.rank = select->rank; tail.epoch = select->epoch; tail.next = select->next;
+      for (int s = 0; s < (select->next ? 2 : 1); ++s)
+        for (int r = 0; r < BZ_MAX_PEERS; ++r) {
+          tail.peer_block[s][r] = select->peer_blocks[s * select->nranks + (r < select->nranks ? r : 0)];
+          tail.peer_flag[s][r] = select->peer_flags[s * select->nranks + (r < select->nranks ? r : 0)];
+        }
     }
     // Distance reuse: unique row k was row old_index[k] of the table in `cache_in`.  A star pass is
     // taken when 1..kStarMax unique rows are new, every other one is in the table, and that table

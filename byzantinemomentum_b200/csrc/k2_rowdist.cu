@@ -166,19 +166,29 @@ rowdist_body(const RowTable& rows, const int n, const float* __restrict__ center
       for (int k = 0; k < S; ++k) sum += partial[k * n + threadIdx.x];
   }
   if (PEERS) {
-    // publish, flag, wait (peers.cuh), then ((p0 + p1) + p2) + ... over the R ranks
+    // the epoch and the slot: by value, or (`next`) from this rank's own flags, read by every thread that
+    // needs them before the barrier below (SEARCH: after this kernel's pdl_wait); then publish, flag, wait
+    // (peers.cuh), and ((p0 + p1) + p2) + ... over the R ranks
+    unsigned epoch = peers.epoch;
+    int slot = 0;
+    if (peers.next && ((int)threadIdx.x < n || (int)threadIdx.x < peers.nranks)) {
+      epoch = next_epoch(peers.flag[0][peers.rank] + peers.rank, peers.flag[1][peers.rank] + peers.rank);
+      slot = (int)(epoch & 1u);
+    }
+    double* const* blocks = peers.block[slot];
+    unsigned* const* flags = peers.flag[slot];
     if (threadIdx.x == 0) peer_timeout = 0;
-    if (threadIdx.x < n) peers.block[peers.rank][threadIdx.x] = sum;
+    if (threadIdx.x < n) blocks[peers.rank][threadIdx.x] = sum;
     __threadfence_system();
     __syncthreads();
     if ((int)threadIdx.x < peers.nranks &&
-        peer_signal_wait(peers.flag[threadIdx.x] + peers.rank, peers.flag[peers.rank] + threadIdx.x, peers.epoch))
+        peer_signal_wait(flags[threadIdx.x] + peers.rank, flags[peers.rank] + threadIdx.x, epoch))
       peer_timeout = 1;
     __syncthreads();
     asm volatile("" ::: "memory");      // the block loads below stay below the flag wait
     if (threadIdx.x < n) {
-      sum = ld_relaxed_sys_f64(peers.block[0] + threadIdx.x);
-      for (int r = 1; r < peers.nranks; ++r) sum += ld_relaxed_sys_f64(peers.block[r] + threadIdx.x);
+      sum = ld_relaxed_sys_f64(blocks[0] + threadIdx.x);
+      for (int r = 1; r < peers.nranks; ++r) sum += ld_relaxed_sys_f64(blocks[r] + threadIdx.x);
     }
   }
   if (threadIdx.x < n) {

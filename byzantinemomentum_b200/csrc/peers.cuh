@@ -26,6 +26,16 @@ __device__ __forceinline__ double ld_relaxed_sys_f64(const double* p) {
   return v;
 }
 
+// The epoch of an exchange that takes it from the buffer (bz_*_peers_next): one past the last epoch this rank
+// raised, i.e. the later, compared wrap-aware as below, of its own entries in its own flag arrays of the two
+// slots (`own0`, `own1`: flag[s][rank] + rank).  A zeroed buffer gives 1; the slot is the epoch modulo 2.
+// Only this rank writes those entries, and only in the signal below: read them before the barrier that
+// precedes it, once every earlier exchanging kernel has completed (stream order, or pdl_wait).
+__device__ __forceinline__ unsigned next_epoch(const unsigned* own0, const unsigned* own1) {
+  const unsigned e0 = ld_acquire_sys(own0), e1 = ld_acquire_sys(own1);
+  return ((int)(e1 - e0) > 0 ? e1 : e0) + 1u;
+}
+
 // One thread per rank t of the exchange: raise this rank's flag for `epoch` in rank t's flag array
 // (`signal`) and wait for rank t's flag in this rank's array (`wait_on`).  The caller has made its block
 // visible (__threadfence_system + __syncthreads) before, and synchronises the block after.  The wait is

@@ -100,7 +100,13 @@ class FusedExchange:
   `ShardedLineSearch(exchange="fused")` runs its exchanges (the rule's block, the score's share) over the
   same buffer: one per call here, each advancing `epoch` by one.  That relies on one condition: the calls
   that share a FusedExchange (the search and the `ShardedPlan` of the same n) are issued on ONE stream, in
-  the same order on every rank. """
+  the same order on every rank.
+  `epoch` is the host's count of the exchanges issued so far; the flags hold the same count on the device
+  (this rank's own entry [rank] of its flag array, in the slot of its last epoch).  The eager calls pass
+  `epoch` by value.  A captured call (`ShardedPlan.graph()`, `ShardedLineSearch.graph()`) cannot: its
+  kernel takes the epoch from the flags instead (one past the later of the two own entries, wrap-aware; 1
+  on a zeroed buffer; the `bz_*_peers_next` calls), and each replay adds the graph's exchanges to `epoch`,
+  so that eager calls and replays can interleave on one buffer. """
   FLAG_WORDS = 16
   def __init__(self, n, device, group=None):
     import torch.distributed._symmetric_memory as symm_mem
@@ -132,11 +138,42 @@ class FusedExchange:
     flags = 2 * self.n * self.n * 8 + slot * self.FLAG_WORDS * 4
     return ((ctypes.c_void_p * self.world)(*[b + block for b in self.peer_base]),
             (ctypes.c_void_p * self.world)(*[b + flags for b in self.peer_base]))
+  def both(self):
+    """ The tables of both slots, as the `bz_*_peers_next` calls take them: (2R block pointers, 2R flag-array
+    pointers), slot 0's then slot 1's. """
+    (b0, f0), (b1, f1) = self.tables(0), self.tables(1)
+    return ((ctypes.c_void_p * (2 * self.world))(*b0, *b1), (ctypes.c_void_p * (2 * self.world))(*f0, *f1))
 
 _fused = {}
 
 def fused_exchange(n, device, group=None):
   return _registered(_fused, FusedExchange, n, device, group)
+
+def _capture(device, issue):
+  """ A CUDA graph of `issue(call)` on `device`: every `call(fn, args)` of a prepared call is made on the
+  capture stream (a prepared call's last argument is the stream current at construction).  The first call
+  that fails ends the issuing; its error is raised once the capture has ended. """
+  failed = []
+  with _engine._on(device):
+    torch.cuda.synchronize(device)
+    graph = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(graph):
+      stream = torch.cuda.current_stream(device).cuda_stream
+      def call(fn, args):
+        if not failed:
+          code = fn(*(args[:-1] + (stream,)))
+          if code != 0:
+            failed.append((code, fn.__name__))
+      issue(call)
+  if failed:
+    _lib.check(*failed[0])
+  return graph
+
+def _capturable(exchange, world, what):
+  """ Raise unless `what` can capture `exchange` on `world` ranks: "fused" anywhere, any exchange on one rank. """
+  if exchange == "p2p" or (exchange == "nccl" and world > 1):
+    raise ValueError(f"{what}.graph() captures the fused exchange on any number of ranks, or any exchange on one rank: "
+                     f"not {exchange!r} on {world} ranks")
 
 def rows_aligned(rows):
   """ Whether the ring kernel takes these rows: every non-empty row 16-byte aligned (an empty shard
@@ -240,7 +277,12 @@ class ShardedPlan:
                     has symmetric memory; else "nccl".  The ranks agree on the choice
                     (`choose_exchange`); a failing symmetric-memory setup raises.
   Both exchanges use the same fixed summation order: bitwise identical selections on every rank.
-  Coordinate-wise rules need no exchange and simply wrap `engine.Plan`. """
+  Coordinate-wise rules need no exchange and simply wrap `engine.Plan`.
+
+  `graph()` captures a step in a CUDA graph, as `engine.Plan.graph()` does: "fused" on any number of ranks
+  (the captured kernel takes its epoch from the exchange buffer, `bz_*_peers_next`), any exchange on one
+  rank; a coordinate-wise plan returns `engine.Plan.graph()`.  Like a call, `graph()` and every replay are
+  collective: every rank issues them at the same point of its stream order. """
   def __init__(self, gar, gradients, f=None, m=None, mode="mid", group=None, exchange="auto"):
     self.gar, self.group = gar, group
     self.rows = list(gradients)
@@ -248,6 +290,7 @@ class ShardedPlan:
     self.world = dist.get_world_size(group) if dist.is_initialized() else 1
     self.selection = None
     self.status = None
+    self._graph = None
     if gar in COORDINATE_WISE:
       self._local = _engine.Plan(gar, self.rows, f=f)
       self.out = self._local.out
@@ -273,6 +316,7 @@ class ShardedPlan:
       self.status = self._meta[n:]                          # krum too: a peer that never signals
       self._fused_fn = getattr(_lib.lib(), f"bz_{gar}_peers")
       self._fused_tables = [fx.tables(0), fx.tables(1)]
+      self._next_fn, self._next_tables = getattr(_lib.lib(), f"bz_{gar}_peers_next"), fx.both()
       self._fused_head = (prep.ptrs, n) + rule.params + (prep.d, out, meta, status, fx.rank, fx.world)
       self._fused_tail = (ws.data_ptr(), ws.numel(), prep.stream)
       return
@@ -294,30 +338,51 @@ class ShardedPlan:
   def __call__(self):
     if self._local is not None:
       return self._local()
-    call = _engine._call
     with _engine._on(self.device):
-      if self.exchange == "fused":
-        fx = self._fx
-        fx.epoch += 1
-        call(self._fused_fn, self._fused_head + self._fused_tables[fx.epoch % 2] + (fx.epoch,) + self._fused_tail)
-        return self.out
-      if self._median is not None:
-        self._median()
-      if self.exchange == "p2p":
-        ex = self._ex
-        a, b = self._ab[ex.step % 2]
-        call(*a)
-        ex.publish()
-      else:
-        a, b = self._ab[0]
-        call(*a)
-        if self.world > 1:
-          dist.all_gather_into_tensor(self._gathered, self._part, group=self.group)
-        else:
-          self._gathered.copy_(self._part.unsqueeze(0))
-      call(*b)
-      call(*self._c)
+      self._issue(_engine._call)
     return self.out
+  def graph(self):
+    """ Capture a step in a CUDA graph (after one eager step, the warm-up) and return `replay`: a callable
+    that launches it and returns `plan.out`.  With "fused", each replay advances the exchange's epoch by one. """
+    if self._local is not None:
+      return self._local.graph()
+    _capturable(self.exchange, self.world, "ShardedPlan")
+    if self._graph is None:
+      self()
+      self._graph = _capture(self.device, lambda call: self._issue(call, captured=True))
+    graph, out, fx = self._graph, self.out, self._fx if self.exchange == "fused" else None
+    def replay():
+      graph.replay()
+      if fx is not None:
+        fx.epoch += 1
+      return out
+    return replay
+  def _issue(self, call, captured=False):
+    """ One step's calls through `call(fn, args)`; `captured`: the fused exchange takes its epoch from the buffer. """
+    if self.exchange == "fused":
+      if captured:
+        call(self._next_fn, self._fused_head + self._next_tables + self._fused_tail)
+        return
+      fx = self._fx
+      fx.epoch += 1
+      call(self._fused_fn, self._fused_head + self._fused_tables[fx.epoch % 2] + (fx.epoch,) + self._fused_tail)
+      return
+    if self._median is not None:
+      call(self._median._fn, self._median._args)
+    if self.exchange == "p2p":
+      ex = self._ex
+      a, b = self._ab[ex.step % 2]
+      call(*a)
+      ex.publish()
+    else:
+      a, b = self._ab[0]
+      call(*a)
+      if self.world > 1:
+        dist.all_gather_into_tensor(self._gathered, self._part, group=self.group)
+      else:
+        self._gathered.copy_(self._part.unsqueeze(0))
+    call(*b)
+    call(*self._c)
 
 SEARCH_EXCHANGES = ("auto", "fused", "nccl")
 
@@ -546,6 +611,7 @@ class _SearchShard:
                         for which in (_lib.CANDIDATE_FIRST, _lib.CANDIDATE_NEXT, _lib.CANDIDATE_FINAL)]
     self._score = (lib.bz_search_score_partial, (out, avg, d, state, self.score.data_ptr(), ws.data_ptr(), ws.numel(), stream))
     self._stream = stream
+    self.call = _engine._call           # every stage's calls go through it (`ShardedLineSearch.graph()` swaps it)
     self.distance = gar in DISTANCE_BASED
     eval_status = None
     self._pair = False
@@ -592,12 +658,14 @@ class _SearchShard:
   def fuse(self, fx):
     """ Prepare the stages of the fused exchange over `fx` (a `FusedExchange` of n rows): per evaluation the
     rule's `*_peers` call (distance rules) and `bz_search_score_peers`, every argument but the slot's
-    tables and the epoch resolved here.  Every distance rule then reports a status word (0, or a peer that
-    did not show up), which the score's transition folds into the search's. """
+    tables and the epoch resolved here (and of their `bz_*_peers_next` twins, which take both slots' tables
+    and no epoch).  Every distance rule then reports a status word (0, or a peer that did not show up), which
+    the score's transition folds into the search's. """
     lib = _lib.lib()
     rows, ws, stream = self._rows, self._ws, self._stream
     n, d, state, out, record = rows.n, rows.d, self._state.data_ptr(), self.out.data_ptr(), self.record.data_ptr()
     self._slots = [fx.tables(0), fx.tables(1)]
+    self._both = fx.both()
     self._tail = (ws.data_ptr(), ws.numel(), stream)
     peers = (fx.rank, fx.world)
     eval_status = None
@@ -607,35 +675,41 @@ class _SearchShard:
       eval_status = meta + 4 * n
       if self._pair:
         head = (code, rows.ptrs, n, rule.f, rule.m, d, out, meta, eval_status)
-        self._rule_peers = [[(lib.bz_pairdist_reuse_peers, head + reuse + peers) for reuse in self._reuse[s]] for s in (0, 1)]
+        self._rule_peers = [[(lib.bz_pairdist_reuse_peers, lib.bz_pairdist_reuse_peers_next, head + reuse + peers)
+                             for reuse in self._reuse[s]] for s in (0, 1)]
       else:
         mode = _lib.AKSEL_MODES["mid"] if rule.center else 0
-        self._rule_peers = (lib.bz_rowdist_peers, (code, rows.ptrs, n, rule.f, mode, out if rule.center else None, d, out, meta,
-                                                   eval_status) + peers)
-    self._score_peers = [(lib.bz_search_score_peers, (out, self._avg, d, state, record, eval_status, record + 8 * (2 * self.evals + 1),
-                                                      k, self.evals) + peers) for k in range(self.evals)]
-  def _with_slot(self, fn, head, epoch):
-    blocks, flags = self._slots[epoch % 2]
-    _engine._call(fn, head + (blocks, flags, epoch) + self._tail)
+        self._rule_peers = (lib.bz_rowdist_peers, lib.bz_rowdist_peers_next,
+                            (code, rows.ptrs, n, rule.f, mode, out if rule.center else None, d, out, meta, eval_status) + peers)
+    self._score_peers = [(lib.bz_search_score_peers, lib.bz_search_score_peers_next,
+                          (out, self._avg, d, state, record, eval_status, record + 8 * (2 * self.evals + 1), k, self.evals) + peers)
+                         for k in range(self.evals)]
+  def _with_slot(self, fn, fn_next, head, epoch):
+    """ An exchanging call: by value at `epoch`, or (None) its `_next` twin, which takes the epoch from the flags. """
+    if epoch is None:
+      self.call(fn_next, head + self._both + self._tail)
+    else:
+      blocks, flags = self._slots[epoch % 2]
+      self.call(fn, head + (blocks, flags, epoch) + self._tail)
   def evaluate_fused(self, k, epoch):
     """ Evaluation k up to its score with the fused exchange: the candidate row, then the rule (distance
-    rules: its exchange at `epoch`; coordinate-wise rules: no exchange, `epoch` is None). """
+    rules: its exchange at `epoch`, or None: at the epoch the flags give; coordinate-wise rules: no exchange). """
     with _engine._on(self.device):
-      _engine._call(*self._candidates[_lib.CANDIDATE_FIRST if k == 0 else _lib.CANDIDATE_NEXT])
+      self.call(*self._candidates[_lib.CANDIDATE_FIRST if k == 0 else _lib.CANDIDATE_NEXT])
       if not self.distance:
-        _engine._call(*self._coordinate)
+        self.call(*self._coordinate)
       elif self._pair:
         self._with_slot(*self._rule_peers[k % 2][int(k > 0 and self._mode.value >= 0)], epoch)
       else:
         if self._median is not None:
-          _engine._call(*self._median)
+          self.call(*self._median)
         self._with_slot(*self._rule_peers, epoch)
   def score_fused(self, k, epoch):
-    """ The score of evaluation k, its exchange at `epoch` and the transition. """
+    """ The score of evaluation k, its exchange at `epoch` (None: at the epoch the flags give) and the transition. """
     with _engine._on(self.device):
       self._with_slot(*self._score_peers[k], epoch)
   def evaluate(self, k):
-    call = _engine._call
+    call = self.call
     with _engine._on(self.device):
       call(*self._candidates[_lib.CANDIDATE_FIRST if k == 0 else _lib.CANDIDATE_NEXT])
       if not self.distance:
@@ -652,17 +726,19 @@ class _SearchShard:
   def conclude(self, blocks):
     select = self._select if blocks is self.blocks else _engine._select_call(self._rule, blocks, self._meta.data_ptr(), self._stream)
     with _engine._on(self.device):
-      _engine._call(*select)
-      _engine._call(*self._reduce)
-      _engine._call(*self._score)
+      self.call(*select)
+      self.call(*self._reduce)
+      self.call(*self._score)
     return self.score
   def step(self, k, scores):
     fn, args = self._steps[k]
     if scores is not self.scores:
       args = (scores.data_ptr(), scores.numel()) + args[2:]
-    _engine._run(self.device, fn, args)
+    with _engine._on(self.device):
+      self.call(fn, args)
   def finish(self):
-    _engine._run(self.device, *self._candidates[_lib.CANDIDATE_FINAL])
+    with _engine._on(self.device):
+      self.call(*self._candidates[_lib.CANDIDATE_FINAL])
     return self.byz
 
 class ShardedLineSearch:
@@ -703,10 +779,14 @@ class ShardedLineSearch:
                      (the share's exchange and the transition): 2 exchanges per evaluation for a distance
                      rule, 1 for the others, each advancing the buffer's epoch by one.  The same bits as
                      "nccl".  The calls that share the buffer must be issued on one stream, in the same
-                     order on every rank.  Not for CUDA-graph capture: the epoch is passed by value;
+                     order on every rank.  The eager calls pass the epoch by value; `graph()` captures
+                     the `_next` calls, which take it from the buffer;
             "auto"   "fused" on 2..16 ranks with symmetric memory, the CUDA engine and (Multi-Krum, Bulyan,
                      brute) 16-byte aligned rows on every rank, else "nccl"; the ranks agree on it
-                     (`choose_search_exchange`). """
+                     (`choose_search_exchange`).
+  `graph()` captures the whole search in a CUDA graph, as `engine.LineSearch.graph()` does: "fused" on any
+  number of ranks, "nccl" on one rank (no collective).  Like a search, `graph()` and every replay are
+  collective: every rank issues them at the same point of its stream order. """
   def __init__(self, gar, grad_honests, f_real, f_decl, grad_avg, grad_att, evals, negative=False, kind="identical",
                group=None, backend=None, exchange="auto"):
     if gar not in _engine._SEARCH_RULES:
@@ -722,6 +802,7 @@ class ShardedLineSearch:
     self.exchange = choose_search_exchange(exchange, not pair or rows_aligned(honest), _symmetric_memory_importable(),
                                            backend is None, group)
     make = _SearchShard if backend is None else backend.search_shard
+    self._backend, self._graph = backend, None
     self._shard = make(gar, honest, f_real, f_decl, grad_avg, grad_att, self.evals, negative, kind, self.world)
     self.byz, self.record = self._shard.byz, self._shard.record
     if self.exchange == "fused":
@@ -751,12 +832,43 @@ class ShardedLineSearch:
     """ The epoch of the next exchange over the shared buffer. """
     self._fx.epoch += 1
     return self._fx.epoch
+  def graph(self):
+    """ Capture the whole search (every evaluation and the last candidate) in a CUDA graph, after one eager
+    search (the warm-up), and return `replay`: a callable that launches it and returns `byz`.  With "fused",
+    each replay advances the exchange's epoch by the graph's exchanges: 2 per evaluation for a distance rule,
+    1 for the others.  CUDA engine only. """
+    if self._backend is not None:
+      raise ValueError("ShardedLineSearch.graph() needs the CUDA engine, not a stand-in backend")
+    _capturable(self.exchange, self.world, "ShardedLineSearch")
+    shard = self._shard
+    if self._graph is None:
+      self()
+      def issue(call):
+        shard.call = call
+        try:
+          self._issue(captured=True)
+        finally:
+          shard.call = _engine._call
+      self._graph = _capture(shard.device, issue)
+    graph, byz = self._graph, self.byz
+    fx = self._fx if self.exchange == "fused" else None
+    exchanges = (2 if shard.distance else 1) * self.evals
+    def replay():
+      graph.replay()
+      if fx is not None:
+        fx.epoch += exchanges
+      return byz
+    return replay
   def __call__(self):
+    return self._issue()
+  def _issue(self, captured=False):
+    """ The search's stages and exchanges; `captured`: the fused exchanges take their epochs from the buffer. """
     shard = self._shard
     if self.exchange == "fused":
+      epoch = (lambda: None) if captured else self._epoch
       for k in range(self.evals):
-        shard.evaluate_fused(k, self._epoch() if shard.distance else None)
-        shard.score_fused(k, self._epoch())
+        shard.evaluate_fused(k, epoch() if shard.distance else None)
+        shard.score_fused(k, epoch())
       return self.finish()
     for k in range(self.evals):
       part = self.evaluate(k)

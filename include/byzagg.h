@@ -292,4 +292,8 @@ BZ_API int bz_gradient_row(const float* grad, int64_t d, double clip, float* sam
  * BZ_MAX_N_COORDINATE = 128 rows: bz_coordinate. */
 #include "byzagg_coordinate.h"
 
+/* The exchanges over peer memory (bz_krum_peers ... bz_search_score_peers) with the epoch taken from the
+ * exchange buffer instead of an argument, so that a CUDA graph can capture them: the _next calls. */
+#include "byzagg_peers_next.h"
+
 #endif /* BYZAGG_H */

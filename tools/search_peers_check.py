@@ -7,8 +7,11 @@ pitched (16-byte aligned) rows, runs both searches for every rule and checks tha
 the status word, its shard of the Byzantine gradient and of the rule's last output are bit-identical
 between the exchanges and across the ranks; it also prints the per-search time of both (slowest rank),
 with the card's name and power limit.
+--graph: the fused search is also captured (`ShardedLineSearch.graph()`, whose exchanges take their epoch
+from the buffer) and replayed around an eager search on the same buffer; the replays must give the eager
+fused search's bits on every rank, and their time (slowest rank) is printed too.
 
-  torchrun --nproc-per-node 8 tools/search_peers_check.py
+  torchrun --nproc-per-node 8 tools/search_peers_check.py [--graph]
 """
 import datetime, os, subprocess, sys, pathlib
 sys.path.insert(0, str(pathlib.Path(__file__).resolve().parent.parent))
@@ -20,6 +23,7 @@ GARS = ["average", "median", "trmean", "phocas", "meamed", "krum", "bulyan", "br
 CASES = [(25, 1_310_922), (25, 7)]          # (n, d): a real shard, and d < R (empty shards) at R = 8
 F = {"brute": 2}                            # f = 5 otherwise; brute: C(n, n - f) <= 2^31
 EVALS = 16
+GRAPH = "--graph" in sys.argv                # also replay the fused search from `ShardedLineSearch.graph()`
 
 def card():
   name = torch.cuda.get_device_name()
@@ -71,6 +75,24 @@ def main():
         search()
         torch.cuda.synchronize()
         runs[exchange] = (search.record.clone(), search.byz.clone(), search._shard.out.clone(), timeit(search) if d > 1000 else 0.)
+        if exchange == "fused" and GRAPH:
+          # the captured search (after graph()'s own eager warm-up), then an eager one between two replays
+          replay = search.graph()
+          replay()
+          search()
+          replay()
+          torch.cuda.synchronize()
+          runs["graph"] = (search.record.clone(), search.byz.clone(), search._shard.out.clone(), timeit(replay) if d > 1000 else 0.)
+      if GRAPH:
+        (rec_g, byz_g, out_g, t_g), (rec_f, byz_f, out_f, _) = runs["graph"], runs["fused"]
+        same_g = (torch.equal(rec_g.view(torch.int64), rec_f.view(torch.int64)) and torch.equal(byz_g.view(torch.int32), byz_f.view(torch.int32))
+                  and torch.equal(out_g.view(torch.int32), out_f.view(torch.int32)))
+        ok = ok and same_g
+        worst_g = torch.tensor([t_g], device=dev)
+        dist.all_reduce(worst_g, op=dist.ReduceOp.MAX)
+        if rank == 0:
+          print(f"n={n} d={d} {gar:7s}: fused graph replay == eager fused on every rank: {same_g}; per replay (slowest rank) "
+                f"{worst_g[0]:9.1f} us", flush=True)
       (rec_c, byz_c, out_c, t_c), (rec_f, byz_f, out_f, t_f) = runs["nccl"], runs["fused"]
       same = (torch.equal(rec_c.view(torch.int64), rec_f.view(torch.int64)) and torch.equal(byz_c.view(torch.int32), byz_f.view(torch.int32))
               and torch.equal(out_c.view(torch.int32), out_f.view(torch.int32)))
