@@ -1,7 +1,7 @@
 # coding: utf-8
 """ctypes binding of `libbyzagg.so` (C ABI: `include/byzagg.h`, `include/byzagg_shards.h`,
 `include/byzagg_attack.h`, `include/byzagg_search_shards.h`, `include/byzagg_search_peers.h`,
-`include/byzagg_coordinate.h` and `include/byzagg_peers_next.h`).
+`include/byzagg_coordinate.h`, `include/byzagg_peers_next.h` and `include/byzagg_distance.h`).
 
 The library is loaded lazily, on the first call that needs it, and the load FAILS LOUDLY:
 there is no CPU or PyTorch fallback anywhere in this package.  Build it in-tree with
@@ -13,11 +13,12 @@ import os
 import pathlib
 import threading
 
-__all__ = ["lib", "LibraryError", "library_path", "check", "MAX_N", "MAX_N_COORDINATE", "STATUS_MESSAGES",
+__all__ = ["lib", "LibraryError", "library_path", "check", "MAX_N", "MAX_N_COORDINATE", "MAX_N_DISTANCE", "STATUS_MESSAGES",
            "AKSEL_MODES", "STATUS_NO_FINITE_SET", "STATUS_DEGENERATE"]
 
 MAX_N = 64
 MAX_N_COORDINATE = 128      # BZ_MAX_N_COORDINATE: the coordinate-wise rules through bz_coordinate
+MAX_N_DISTANCE = 128        # BZ_MAX_N_DISTANCE: Multi-Krum, Bulyan, Aksel and CGE through bz_distance
 MAX_PEERS = 16
 STATUS_NO_FINITE_SET = 1
 STATUS_DEGENERATE = 2
@@ -119,6 +120,11 @@ PEER_NEXT_SIGNATURES = {
 COORDINATE_SIGNATURES = {
   "bz_coordinate": (_i, [_i, _c_rows, _i, _i, _i64, _vp, _vp]),
 }
+# the same for include/byzagg_distance.h (Multi-Krum, Bulyan, Aksel and CGE up to MAX_N_DISTANCE rows)
+DISTANCE_SIGNATURES = {
+  "bz_distance_workspace_bytes": (_sz, [_i]),
+  "bz_distance": (_i, [_i, _c_rows, _i, _i, _i, _i, _i64, _vp, _vp, _vp, _vp, _sz, _vp]),
+}
 SEARCH_STATE_BYTES = 64                     # BZ_SEARCH_STATE_BYTES
 CANDIDATE_FIRST, CANDIDATE_NEXT, CANDIDATE_FINAL = 0, 1, 2
 
@@ -141,7 +147,7 @@ def lib():
       except OSError as err:
         raise LibraryError(f"unable to load {path}: {err}") from err
       tables = (SIGNATURES, SHARD_SIGNATURES, ATTACK_SIGNATURES, SEARCH_SHARD_SIGNATURES, SEARCH_PEER_SIGNATURES,
-                COORDINATE_SIGNATURES, PEER_NEXT_SIGNATURES)
+                COORDINATE_SIGNATURES, PEER_NEXT_SIGNATURES, DISTANCE_SIGNATURES)
       for name, (restype, argtypes) in [item for table in tables for item in table.items()]:
         try:
           fn = getattr(handle, name)

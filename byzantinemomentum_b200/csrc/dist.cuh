@@ -184,4 +184,38 @@ bool launch_bulyan_reduce(const RowTable& rows, int n, int f, int m, const int32
 bool launch_bulyan_reduce_static(const RowTable& rows, int n, int f, int m, const int32_t* order, const int32_t* status,
                                  const Geom& g, float* out, cudaStream_t st);
 
+// ---- Above kMaxN rows (bz_distance, api_distance.inc) ----------------------------------------------
+// The pairwise distances of u <= kMaxNDistance unique rows come from passes of the 64-row K2: up to kMaxN
+// rows one pass over all of them, above that the rows are cut into K = ceil(u / 32) blocks of consecutive
+// unique rows (3 or 4, sizes differing by at most one) and every block pair I < J gets one pass over the
+// rows of I then J.  A pair across blocks comes from its pass; a pair inside block I, and the self distance
+// of an aliased row of I, from the pass (0, 1) for I = 0 and (0, I) otherwise.
+constexpr int kMaxNDistance = BZ_MAX_N_DISTANCE;
+constexpr int kMaxBlocks = 4;
+constexpr int kMaxPasses = kMaxBlocks * (kMaxBlocks - 1) / 2;
+constexpr size_t kPassTable = (size_t)kMaxN * kMaxN;     // doubles between two pass tables
+struct PassTables {
+  const double* table;                        // pass p: size[p] x size[p] squared distances at table + p * kPassTable
+  int nblocks, npasses;
+  int start[kMaxBlocks + 1];                  // block b: unique rows [start[b], start[b + 1])
+  int first[kMaxPasses], size[kMaxPasses];    // pass p: its first block (rows 0 ..) and its row count
+  signed char pass[kMaxBlocks][kMaxBlocks];   // the pass that holds the pairs of blocks (a, b)
+  unsigned char to_unique[kMaxNDistance];     // original row -> unique row
+};
+size_t distance_workspace_bytes(int n);
+
+// K2 over `u` rows as given, the diagonal entries (self distance) of the rows in self_rows[0, nself) included:
+// the ring, or the cp.async kernel when the ring cannot run.  Returns the number of blocks written.
+int launch_pairdist_rows(const RowTable& rows, int u, int64_t d, double* parts, cudaStream_t st,
+                         const unsigned char* self_rows, int nself, SelectTail* select = nullptr);
+// K5 of Multi-Krum (bulyan = 0) or Bulyan on n <= kMaxNDistance rows, reading the pass tables.
+void launch_select_wide(const PassTables& t, int n, int count, int32_t* order, int32_t* status, int f, int m, int bulyan,
+                        cudaStream_t st);
+// K2' over the 128-pointer table with the selection of launch_rowdist (order and ticket required).
+int launch_rowdist(const WideRowTable& rows, int n, const float* const* host_rows, const float* center, int64_t d,
+                   double* parts, cudaStream_t st, int reverse, int32_t* order, unsigned* ticket, int sqrt_norm);
+// K4 over the 128-pointer table, kMaxN < n <= kMaxNDistance; false when theta is outside 33..128.
+bool launch_bulyan_reduce_wide(const WideRowTable& rows, int n, int f, int m, const int32_t* order, const int32_t* status,
+                               int64_t d, float* out, cudaStream_t st);
+
 }  // namespace bz

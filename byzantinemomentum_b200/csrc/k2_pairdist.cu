@@ -256,14 +256,19 @@ int aliased_rows(const int* to_unique, int u, int n_orig, unsigned char* self_ro
   return nself;
 }
 
-int launch_pairdist_auto(const RowTable& rows, int u, int64_t d, double* parts, cudaStream_t st,
-                         const int* to_unique, int n_orig, SelectTail* select) {
-  unsigned char self_rows[kMaxN];
-  const int nself = aliased_rows(to_unique, u, n_orig, self_rows);
+int launch_pairdist_rows(const RowTable& rows, int u, int64_t d, double* parts, cudaStream_t st,
+                         const unsigned char* self_rows, int nself, SelectTail* select) {
   const int nparts = launch_pairdist_ring(rows, u, d, parts, st, self_rows, nself, select);
   if (nparts > 0) return nparts;
   if (select != nullptr) select->fused = 0;
   return launch_pairdist(rows, u, d, parts, st, nself > 0 ? 1 : 0);
+}
+
+int launch_pairdist_auto(const RowTable& rows, int u, int64_t d, double* parts, cudaStream_t st,
+                         const int* to_unique, int n_orig, SelectTail* select) {
+  unsigned char self_rows[kMaxN];
+  const int nself = aliased_rows(to_unique, u, n_orig, self_rows);
+  return launch_pairdist_rows(rows, u, d, parts, st, self_rows, nself, select);
 }
 
 void launch_reduce_parts(const double* parts, int nparts, int len, int pair_n, double* block, cudaStream_t st) {

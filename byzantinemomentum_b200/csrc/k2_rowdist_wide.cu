@@ -1,0 +1,127 @@
+// k2_rowdist_wide.cu — K2' above 64 rows (bz_distance's Aksel and CGE): the squared distance of every row to
+// the coordinate-wise median (aksel.py:41) or to the origin (cge.py:36) over the 128-pointer table, with the
+// selection in the last CTA, as k2_rowdist does up to 64 rows.
+//
+// One fp32 accumulator per row and per thread, as k2_rowdist keeps, would take 128 registers; instead, as
+// K6 does over the wide table (k6_study.cu), a thread takes one coordinate (VEC = 1) and folds its rows 32 at
+// a time: the 32 squares of a chunk go through the transposed warp reduction (an fp32 sum over the warp's 32
+// coordinates) and into fp64, so that lane L ends with rows L, L + 32, L + 64 and L + 96.  Warps are combined
+// through shared memory in fixed order, one fp64 block per CTA; the last CTA (ticket) sums the blocks in S
+// interleaved classes, the class sums in class order, and writes the stable order of the n keys.
+// Deterministic; identical rows give identical sums.  Roofline: HBM, n·4 B per coordinate (+4 B for the centre).
+#include "dist.cuh"
+#include "k5_device.cuh"
+#include "reduce.cuh"
+
+namespace bz {
+
+constexpr int kRwThreads = 256;
+constexpr int kRwWarps = kRwThreads / 32;
+constexpr int kRwChunks = kMaxNDistance / 32;
+
+template <bool CENTER>
+__global__ void __launch_bounds__(kRwThreads, 2)
+k2_rowdist_wide(const __grid_constant__ WideRowTable rows, const int n, const float* __restrict__ center, const Geom g,
+                double* __restrict__ parts, int32_t* __restrict__ order, unsigned* __restrict__ ticket, const int sqrt_norm) {
+  __shared__ double warp_tot[kRwWarps][kMaxNDistance];
+  __shared__ bool last;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  double dr[kRwChunks];
+#pragma unroll
+  for (int c = 0; c < kRwChunks; ++c) dr[c] = 0.;
+  const int64_t stride = (int64_t)gridDim.x * kRwThreads;
+  // warp-uniform trip count: lanes past the end contribute zeros and still join the shuffles
+  const int64_t first = (int64_t)blockIdx.x * kRwThreads + warp * 32;
+  for (int64_t vf = first; vf < g.nv; vf += stride) {
+    // reversed walk (Geom::reverse): same warp-uniform trip count, mirrored base; VEC = 1: no shift
+    const int64_t e = (g.reverse ? ((g.nv - 1) / 32) * 32 - vf : vf) + lane;
+    const bool live = e < g.d;
+    // out-of-range lanes and rows past n add exactly 0: they take the centre itself
+    const float c = (CENTER && live) ? __ldcs(center + e) : 0.f;
+#pragma unroll
+    for (int ch = 0; ch < kRwChunks; ++ch) {
+      if (ch * 32 >= n) break;                              // warp-uniform
+      float v[32];
+#pragma unroll
+      for (int j = 0; j < 32; ++j) {
+        const int r = ch * 32 + j;
+        v[j] = (live && r < n) ? __ldcs(rows.p[r] + e) : c;
+      }
+#pragma unroll
+      for (int j = 0; j < 32; ++j) {
+        if (CENTER) {
+          const float df = __fsub_rn(v[j], c);
+          v[j] = __fmul_rn(df, df);                        // aksel.py:41: the square is rounded to fp32
+        } else {
+          v[j] = __fmul_rn(v[j], v[j]);
+        }
+      }
+      dr[ch] += (double)transpose_reduce(v, lane);
+    }
+  }
+#pragma unroll
+  for (int c = 0; c < kRwChunks; ++c) warp_tot[warp][c * 32 + lane] = dr[c];
+  __syncthreads();
+  if (threadIdx.x < n) {
+    double s = 0.;
+#pragma unroll
+    for (int w = 0; w < kRwWarps; ++w) s += warp_tot[w][threadIdx.x];
+    parts[(size_t)blockIdx.x * n + threadIdx.x] = s;
+  }
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0) last = atomicAdd(ticket, 1u) == gridDim.x - 1;
+  __syncthreads();
+  if (!last) return;
+  __threadfence();
+  double* partial = &warp_tot[0][0];                // S * n <= kRwThreads doubles
+  double* key = partial + kRwThreads;               // n doubles behind them
+  const int S = kRwThreads / n;                     // >= 2
+  const int c = threadIdx.x % n, cls = threadIdx.x / n;
+  if (cls < S) {
+    double s = 0.;
+    int p = cls;
+    for (; p + 7 * S < (int)gridDim.x; p += 8 * S) {
+      double t[8];
+#pragma unroll
+      for (int u = 0; u < 8; ++u) t[u] = __ldcg(parts + (size_t)(p + u * S) * n + c);
+#pragma unroll
+      for (int u = 0; u < 8; ++u) s += t[u];
+    }
+    for (; p < (int)gridDim.x; p += S) s += __ldcg(parts + (size_t)p * n + c);
+    partial[cls * n + c] = s;
+  }
+  __syncthreads();
+  if (threadIdx.x < n) {
+    double sum = 0.;
+    for (int k = 0; k < S; ++k) sum += partial[k * n + threadIdx.x];
+    double v;
+    if (sqrt_norm) {
+      v = (double)fp32_norm(sum);                    // cge.py:36-37: fp32 norm, non-finite -> +inf
+      if (!finite_d(v)) v = CUDART_INF;
+    } else {
+      v = (double)(float)sum;                        // aksel.py:41: fp32 sum of squares
+    }
+    key[threadIdx.x] = v;
+  }
+  __syncthreads();
+  stable_order(key, n, order);
+  if (threadIdx.x == 0) *ticket = 0u;
+}
+
+int launch_rowdist(const WideRowTable& rows, int n, const float* const* host_rows, const float* center, int64_t d,
+                   double* parts, cudaStream_t st, int reverse, int32_t* order, unsigned* ticket, int sqrt_norm) {
+  Geom g = make_geom(host_rows, n, center, nullptr, d, 1);
+  g.reverse = reverse;
+  int64_t grid = (g.nv + kRwThreads - 1) / kRwThreads;
+  const int64_t cap = (int64_t)sm_count() * 2;
+  if (grid > cap) grid = cap;
+  if (grid > kMaxParts) grid = kMaxParts;
+  if (grid < 1) grid = 1;
+  cudaMemsetAsync(ticket, 0, sizeof(unsigned), st);
+  if (center) k2_rowdist_wide<true><<<(unsigned)grid, kRwThreads, 0, st>>>(rows, n, center, g, parts, order, ticket, sqrt_norm);
+  else        k2_rowdist_wide<false><<<(unsigned)grid, kRwThreads, 0, st>>>(rows, n, center, g, parts, order, ticket, sqrt_norm);
+  return (int)grid;
+}
+
+}  // namespace bz

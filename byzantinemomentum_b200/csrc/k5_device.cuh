@@ -103,7 +103,9 @@ __device__ inline void finish_distances(const double* sq, int n, bool map_nonfin
 
 // CPython >= 3.12 `sum()` over floats (Objects/bltinmodule.c: Neumaier's compensated sum;
 // the compensation is dropped when it is not finite).
-__device__ inline double py_sum(const double* v, int count) {
+// T = float: fp32 values (the 128-row scoring keeps its distances so), each widened to double.
+template <class T>
+__device__ inline double py_sum(const T* v, int count) {
   if (count <= 0) return 0.;
   double f = v[0], c = 0.;
   for (int k = 1; k < count; ++k) {
@@ -118,13 +120,14 @@ __device__ inline double py_sum(const double* v, int count) {
 }
 
 // Row-wise ascending sort by ranking: sorted[i][rank] = dist[i][j] (ties by column index).
-__device__ inline void sort_rows(const double* dist, double* sorted, int n) {
+template <class T>
+__device__ inline void sort_rows(const T* dist, T* sorted, int n) {
   for (int e = threadIdx.x; e < n * n; e += blockDim.x) {
     const int i = e / n, j = e - i * n;
-    const double v = dist[e];
+    const T v = dist[e];
     int rank = 0;
     for (int k = 0; k < n; ++k) {
-      const double w = dist[i * n + k];
+      const T w = dist[i * n + k];
       rank += (w < v || (w == v && k < j)) ? 1 : 0;
     }
     sorted[i * n + rank] = v;
@@ -149,6 +152,21 @@ __device__ inline void stable_order(const double* key, int n, int32_t* __restric
   }
 }
 
+// bulyan.py:65-73: from the second iteration on, pruned `(inf, None)` entries precede every +inf score
+// (stable sort), so fewer than m_i finite scores left means gradients[None].  One thread.
+__device__ inline int bulyan_status(const double* score, int n, int f, int m) {
+  int st = BZ_STATUS_OK;
+  int finite = 0;
+  for (int i = 0; i < n; ++i) finite += finite_d(score[i]) ? 1 : 0;
+  const int m_max = n - f - 2, theta = n - 2 * f - 2;
+  int mi = m;
+  for (int i = 0; i < theta; ++i) {
+    mi = min(mi, m_max - i);
+    if (i >= 1 && finite - i < mi) st = BZ_STATUS_DEGENERATE;
+  }
+  return st;
+}
+
 // krum.py:52-62 (count = n-f-1, diagonal excluded) and bulyan.py:56-62 (count = m over the
 // row INCLUDING its +inf diagonal).  Putting +inf on the diagonal serves both: the extra +inf
 // can only be reached after every finite distance, where the sum is +inf either way.
@@ -165,22 +183,7 @@ __device__ inline void score_from_table(const RowMap& map, int n, int count, int
   for (int i = threadIdx.x; i < n; i += blockDim.x) score[i] = py_sum(sorted + i * n, count);
   __syncthreads();
   stable_order(score, n, order);
-  if (threadIdx.x == 0 && status != nullptr) {
-    int st = BZ_STATUS_OK;
-    if (bulyan) {
-      // bulyan.py:65-73: from the second iteration on, pruned `(inf, None)` entries precede every
-      // +inf score (stable sort), so fewer than m_i finite scores left means gradients[None]
-      int finite = 0;
-      for (int i = 0; i < n; ++i) finite += finite_d(score[i]) ? 1 : 0;
-      const int m_max = n - f - 2, theta = n - 2 * f - 2;
-      int mi = m;
-      for (int i = 0; i < theta; ++i) {
-        mi = min(mi, m_max - i);
-        if (i >= 1 && finite - i < mi) st = BZ_STATUS_DEGENERATE;
-      }
-    }
-    *status = st;
-  }
+  if (threadIdx.x == 0 && status != nullptr) *status = bulyan ? bulyan_status(score, n, f, m) : BZ_STATUS_OK;
 }
 
 template <class Parts>

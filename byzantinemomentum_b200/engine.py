@@ -473,6 +473,7 @@ def pair_cache_stats(device_index=None):
 # phases of the d-sharded path
 
 DISTANCE_BASED = ("krum", "bulyan", "brute", "aksel", "cge")
+WIDE_DISTANCE = ("krum", "bulyan", "aksel", "cge")        # `Plan` takes them up to MAX_N_DISTANCE rows (bz_distance)
 
 class _Rule:
   """ The facts of a distance-based rule for (gar, n, f, m, mode):
@@ -507,6 +508,14 @@ class _Rule:
       self.count = m if gar == "krum" else n - f
     self.select = gar if self.pair else "rowdist"
     self.select_params = (f, m) if gar == "bulyan" else (f,) if self.pair else (int(gar == "cge"),)
+  def wide_entry(self, ptrs, d, out, meta, ws, stream):
+    """ (fn, args) of `bz_distance`, which takes krum, bulyan, aksel and cge up to MAX_N_DISTANCE rows, writing to
+    the addresses `out` and `meta` (order[n] + status). """
+    m = self.m if self.gar in ("krum", "bulyan") else 0
+    mode = self.params[1] if self.gar == "aksel" else 0
+    status = meta + 4 * self.n if self.status else None
+    return _lib.lib().bz_distance, (_SEARCH_RULES[self.gar], ptrs, self.n, self.f, m, mode, d, out, meta, status,
+                                    ws.data_ptr(), ws.numel(), stream)
   def entry(self, ptrs, d, out, meta, ws, stream, reuse=()):
     """ (fn, args) of the single-GPU call `bz_<gar>` writing to the addresses `out` and `meta`
     (order[n] + status), or of `bz_<gar>_reuse` given the distance cache's `reuse` arguments. """
@@ -1145,11 +1154,14 @@ class Plan:
       plan = engine.Plan("krum", gradients, f=5)
       aggregated = plan()          # same tensor every time: plan.out
       plan.selection               # device int32 (distance-based rules)
+  Up to MAX_N_COORDINATE rows for the coordinate-wise rules, MAX_N_DISTANCE for krum, bulyan, aksel and cge
+  (above MAX_N through `bz_distance`, with a workspace of its own), MAX_N for brute.
   For brute / bulyan the device status word is NOT checked here (that would synchronise);
   read `plan.status` when needed: non-zero means the rule is undefined on this data and `out`
   is NaN. """
   def __init__(self, gar, gradients, f=None, m=None, mode="mid", out=None):
-    prep = _prepare(list(gradients), limit=_lib.MAX_N_COORDINATE if gar in _RULE_CODES else _lib.MAX_N)
+    limit = _lib.MAX_N_COORDINATE if gar in _RULE_CODES else _lib.MAX_N_DISTANCE if gar in WIDE_DISTANCE else _lib.MAX_N
+    prep = _prepare(list(gradients), limit=limit)
     if prep.to_cpu:
       raise ValueError("Plan takes CUDA tensors (host tensors go through the plain call, which stages them)")
     n, d = prep.n, prep.d
@@ -1166,12 +1178,17 @@ class Plan:
       fn, args = _coordinate_call(gar, prep, f, self.out.data_ptr())
     else:
       rule = _rule(gar, n, f, m, mode)
-      self._ws = _workspace(prep.device, prep.stream)
       self._meta = torch.empty(n + 1, dtype=torch.int32, device=prep.device)
       self.selection = self._meta[:rule.length]
       if rule.status:
         self.status = self._meta[n:]
-      fn, args = rule.entry(prep.ptrs, d, self.out.data_ptr(), self._meta.data_ptr(), self._ws, prep.stream)
+      if n > _lib.MAX_N:
+        # the pass tables of bz_distance, held by the plan: the per-stream workspace stays at its 64-row size
+        self._ws = torch.empty(int(_lib.lib().bz_distance_workspace_bytes(n)), dtype=torch.uint8, device=prep.device)
+        fn, args = rule.wide_entry(prep.ptrs, d, self.out.data_ptr(), self._meta.data_ptr(), self._ws, prep.stream)
+      else:
+        self._ws = _workspace(prep.device, prep.stream)
+        fn, args = rule.entry(prep.ptrs, d, self.out.data_ptr(), self._meta.data_ptr(), self._ws, prep.stream)
     self._fn, self._args = fn, args
     self._graph = None
   def graph(self):

@@ -29,7 +29,8 @@
  *     a thread-local message for the last failure.
  *   - 1 <= n <= bz_max_n() (= 64), d >= 0 (d = 0 is a no-op).  The coordinate-wise rules take up
  *     to 128 rows through bz_coordinate (byzagg_coordinate.h, included at the end), and so do
- *     bz_avg_dev_max and bz_line_search with a coordinate-wise rule.
+ *     bz_avg_dev_max and bz_line_search with a coordinate-wise rule.  Multi-Krum, Bulyan, Aksel
+ *     and CGE take up to 128 rows through bz_distance (byzagg_distance.h, included at the end).
  *   - Parameter validity (f, m ranges) is the caller's job, exactly like the reference's
  *     `check()` functions; the library only rejects what it cannot execute.
  */
@@ -295,5 +296,8 @@ BZ_API int bz_gradient_row(const float* grad, int64_t d, double clip, float* sam
 /* The exchanges over peer memory (bz_krum_peers ... bz_search_score_peers) with the epoch taken from the
  * exchange buffer instead of an argument, so that a CUDA graph can capture them: the _next calls. */
 #include "byzagg_peers_next.h"
+
+/* Multi-Krum, Bulyan, Aksel and CGE for up to BZ_MAX_N_DISTANCE = 128 rows on one GPU: bz_distance. */
+#include "byzagg_distance.h"
 
 #endif /* BYZAGG_H */
