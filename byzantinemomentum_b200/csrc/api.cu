@@ -321,3 +321,4 @@ int bz_coordinate(int rule, const float* const* rows, int n, int f, int64_t d, f
 #include "api_search_peers.inc"
 #include "api_peers_next.inc"
 #include "api_distance.inc"
+#include "api_distance_shards.inc"

@@ -204,6 +204,19 @@ struct PassTables {
 };
 size_t distance_workspace_bytes(int n);
 
+// The squared distance of unique rows a <= b (the self distance when a == b) from the pass that holds it.
+__device__ __forceinline__ double pass_sq(const PassTables& t, int a, int b) {
+  int ba = 0;
+  while (a >= t.start[ba + 1]) ++ba;
+  int bb = ba;
+  while (b >= t.start[bb + 1]) ++bb;
+  const int p = t.pass[ba][bb], f = t.first[p], s = t.size[p];
+  const int s0 = t.start[f + 1] - t.start[f];
+  const int la = ba == f ? a - t.start[f] : s0 + a - t.start[ba];
+  const int lb = bb == f ? b - t.start[f] : s0 + b - t.start[bb];
+  return __ldcg(t.table + (size_t)p * kPassTable + (size_t)la * s + lb);
+}
+
 // K2 over `u` rows as given, the diagonal entries (self distance) of the rows in self_rows[0, nself) included:
 // the ring, or the cp.async kernel when the ring cannot run.  Returns the number of blocks written.
 int launch_pairdist_rows(const RowTable& rows, int u, int64_t d, double* parts, cudaStream_t st,
@@ -217,5 +230,20 @@ int launch_rowdist(const WideRowTable& rows, int n, const float* const* host_row
 // K4 over the 128-pointer table, kMaxN < n <= kMaxNDistance; false when theta is outside 33..128.
 bool launch_bulyan_reduce_wide(const WideRowTable& rows, int n, int f, int m, const int32_t* order, const int32_t* status,
                                int64_t d, float* out, cudaStream_t st);
+
+// ---- The d-sharded phases above kMaxN rows (bz_distance_partial / _select, api_distance_shards.inc) ----------------
+// K2-share: the n x n block of the original rows from the pass tables (entries i < j, the self distance for an
+// aliased pair, 0 elsewhere).
+void launch_pairshare_wide(const PassTables& t, int n, double* block, cudaStream_t st);
+// K2'-share: K2' over the 128-pointer table in launch_rowdist's geometry, its last CTA writing the n sums to `sums`
+// (the sums K2' forms its keys from) instead of the order.
+int launch_rowshare(const WideRowTable& rows, int n, const float* const* host_rows, const float* center, int64_t d,
+                    double* parts, cudaStream_t st, int reverse, unsigned* ticket, double* sums);
+// K5 of Multi-Krum (bulyan = 0) or Bulyan from `nparts` gathered n x n blocks, added in rank order.
+void launch_blocks_select_wide(const double* parts, int nparts, int n, int count, int32_t* order, int32_t* status, int f,
+                               int m, int bulyan, cudaStream_t st);
+// The stable order of the n row keys from `nparts` gathered blocks of n sums, added in rank order (sqrt_norm as in
+// bz_rowdist_select).
+void launch_rowkeys_select_wide(const double* parts, int nparts, int n, int sqrt_norm, int32_t* order, cudaStream_t st);
 
 }  // namespace bz

@@ -1,6 +1,7 @@
 // k2_rowdist_wide.cu — K2' above 64 rows (bz_distance's Aksel and CGE): the squared distance of every row to
 // the coordinate-wise median (aksel.py:41) or to the origin (cge.py:36) over the 128-pointer table, with the
-// selection in the last CTA, as k2_rowdist does up to 64 rows.
+// selection in the last CTA, as k2_rowdist does up to 64 rows.  K2'-share (k2_rowshare_wide, phase A of the
+// d-sharded path, bz_distance_partial) is the same kernel with the last CTA writing the n sums instead.
 //
 // One fp32 accumulator per row and per thread, as k2_rowdist keeps, would take 128 registers; instead, as
 // K6 does over the wide table (k6_study.cu), a thread takes one coordinate (VEC = 1) and folds its rows 32 at
@@ -19,10 +20,12 @@ constexpr int kRwThreads = 256;
 constexpr int kRwWarps = kRwThreads / 32;
 constexpr int kRwChunks = kMaxNDistance / 32;
 
-template <bool CENTER>
-__global__ void __launch_bounds__(kRwThreads, 2)
-k2_rowdist_wide(const __grid_constant__ WideRowTable rows, const int n, const float* __restrict__ center, const Geom g,
-                double* __restrict__ parts, int32_t* __restrict__ order, unsigned* __restrict__ ticket, const int sqrt_norm) {
+// SUMS: the last CTA writes the n sums to `sums` (K2'-share); otherwise the stable order of their keys to `order`.
+template <bool CENTER, bool SUMS>
+__device__ __forceinline__ void rowdist_wide_body(const WideRowTable& rows, const int n, const float* __restrict__ center,
+                                                  const Geom& g, double* __restrict__ parts, int32_t* __restrict__ order,
+                                                  unsigned* __restrict__ ticket, const int sqrt_norm,
+                                                  double* __restrict__ sums) {
   __shared__ double warp_tot[kRwWarps][kMaxNDistance];
   __shared__ bool last;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -95,23 +98,44 @@ k2_rowdist_wide(const __grid_constant__ WideRowTable rows, const int n, const fl
   if (threadIdx.x < n) {
     double sum = 0.;
     for (int k = 0; k < S; ++k) sum += partial[k * n + threadIdx.x];
-    double v;
-    if (sqrt_norm) {
-      v = (double)fp32_norm(sum);                    // cge.py:36-37: fp32 norm, non-finite -> +inf
-      if (!finite_d(v)) v = CUDART_INF;
+    if (SUMS) {
+      sums[threadIdx.x] = sum;
     } else {
-      v = (double)(float)sum;                        // aksel.py:41: fp32 sum of squares
+      double v;
+      if (sqrt_norm) {
+        v = (double)fp32_norm(sum);                  // cge.py:36-37: fp32 norm, non-finite -> +inf
+        if (!finite_d(v)) v = CUDART_INF;
+      } else {
+        v = (double)(float)sum;                      // aksel.py:41: fp32 sum of squares
+      }
+      key[threadIdx.x] = v;
     }
-    key[threadIdx.x] = v;
   }
-  __syncthreads();
-  stable_order(key, n, order);
+  if (!SUMS) {
+    __syncthreads();
+    stable_order(key, n, order);
+  }
   if (threadIdx.x == 0) *ticket = 0u;
 }
 
-int launch_rowdist(const WideRowTable& rows, int n, const float* const* host_rows, const float* center, int64_t d,
-                   double* parts, cudaStream_t st, int reverse, int32_t* order, unsigned* ticket, int sqrt_norm) {
-  Geom g = make_geom(host_rows, n, center, nullptr, d, 1);
+template <bool CENTER>
+__global__ void __launch_bounds__(kRwThreads, 2)
+k2_rowdist_wide(const __grid_constant__ WideRowTable rows, const int n, const float* __restrict__ center, const Geom g,
+                double* __restrict__ parts, int32_t* __restrict__ order, unsigned* __restrict__ ticket, const int sqrt_norm) {
+  rowdist_wide_body<CENTER, false>(rows, n, center, g, parts, order, ticket, sqrt_norm, nullptr);
+}
+
+template <bool CENTER>
+__global__ void __launch_bounds__(kRwThreads, 2)
+k2_rowshare_wide(const __grid_constant__ WideRowTable rows, const int n, const float* __restrict__ center, const Geom g,
+                 double* __restrict__ parts, unsigned* __restrict__ ticket, double* __restrict__ sums) {
+  rowdist_wide_body<CENTER, true>(rows, n, center, g, parts, nullptr, ticket, 0, sums);
+}
+
+// The geometry of both kernels: at most two CTAs per SM and kMaxParts blocks; the ticket is zeroed first.
+static unsigned rowdist_wide_grid(const float* const* host_rows, int n, const float* center, int64_t d, int reverse,
+                                  unsigned* ticket, cudaStream_t st, Geom& g) {
+  g = make_geom(host_rows, n, center, nullptr, d, 1);
   g.reverse = reverse;
   int64_t grid = (g.nv + kRwThreads - 1) / kRwThreads;
   const int64_t cap = (int64_t)sm_count() * 2;
@@ -119,8 +143,24 @@ int launch_rowdist(const WideRowTable& rows, int n, const float* const* host_row
   if (grid > kMaxParts) grid = kMaxParts;
   if (grid < 1) grid = 1;
   cudaMemsetAsync(ticket, 0, sizeof(unsigned), st);
-  if (center) k2_rowdist_wide<true><<<(unsigned)grid, kRwThreads, 0, st>>>(rows, n, center, g, parts, order, ticket, sqrt_norm);
-  else        k2_rowdist_wide<false><<<(unsigned)grid, kRwThreads, 0, st>>>(rows, n, center, g, parts, order, ticket, sqrt_norm);
+  return (unsigned)grid;
+}
+
+int launch_rowdist(const WideRowTable& rows, int n, const float* const* host_rows, const float* center, int64_t d,
+                   double* parts, cudaStream_t st, int reverse, int32_t* order, unsigned* ticket, int sqrt_norm) {
+  Geom g;
+  const unsigned grid = rowdist_wide_grid(host_rows, n, center, d, reverse, ticket, st, g);
+  if (center) k2_rowdist_wide<true><<<grid, kRwThreads, 0, st>>>(rows, n, center, g, parts, order, ticket, sqrt_norm);
+  else        k2_rowdist_wide<false><<<grid, kRwThreads, 0, st>>>(rows, n, center, g, parts, order, ticket, sqrt_norm);
+  return (int)grid;
+}
+
+int launch_rowshare(const WideRowTable& rows, int n, const float* const* host_rows, const float* center, int64_t d,
+                    double* parts, cudaStream_t st, int reverse, unsigned* ticket, double* sums) {
+  Geom g;
+  const unsigned grid = rowdist_wide_grid(host_rows, n, center, d, reverse, ticket, st, g);
+  if (center) k2_rowshare_wide<true><<<grid, kRwThreads, 0, st>>>(rows, n, center, g, parts, ticket, sums);
+  else        k2_rowshare_wide<false><<<grid, kRwThreads, 0, st>>>(rows, n, center, g, parts, ticket, sums);
   return (int)grid;
 }
 

@@ -135,6 +135,20 @@ __device__ inline void sort_rows(const T* dist, T* sorted, int n) {
   __syncthreads();
 }
 
+// The key of a row from its summed squared distance: cge.py:36-37's fp32 norm with every non-finite norm mapped
+// to +inf (sqrt_norm), or aksel.py:41's fp32 sum of squares.  The same statements as K2''s last CTA and
+// k5_rowdist_select, which keep their own copy so that their code stays as it was built.
+__device__ __forceinline__ double row_key(double sum, int sqrt_norm) {
+  double v;
+  if (sqrt_norm) {
+    v = (double)fp32_norm(sum);
+    if (!finite_d(v)) v = CUDART_INF;
+  } else {
+    v = (double)(float)sum;
+  }
+  return v;
+}
+
 // Stable ascending argsort of key[0..n): order[rank] = index.  NaN keys sort last.
 __device__ inline void stable_order(const double* key, int n, int32_t* __restrict__ order) {
   for (int i = threadIdx.x; i < n; i += blockDim.x) {

@@ -511,11 +511,24 @@ class _Rule:
   def wide_entry(self, ptrs, d, out, meta, ws, stream):
     """ (fn, args) of `bz_distance`, which takes krum, bulyan, aksel and cge up to MAX_N_DISTANCE rows, writing to
     the addresses `out` and `meta` (order[n] + status). """
-    m = self.m if self.gar in ("krum", "bulyan") else 0
-    mode = self.params[1] if self.gar == "aksel" else 0
+    m, mode = self._m_mode()
     status = meta + 4 * self.n if self.status else None
     return _lib.lib().bz_distance, (_SEARCH_RULES[self.gar], ptrs, self.n, self.f, m, mode, d, out, meta, status,
                                     ws.data_ptr(), ws.numel(), stream)
+  def phase_entries(self, ptrs, d, center, part, blocks, nparts, out, meta, ws, stream):
+    """ The three (fn, args) of the d-sharded phases through `bz_distance_partial`, `bz_distance_select` and
+    `bz_distance_reduce`, which take every rule up to MAX_N_DISTANCE rows (brute: MAX_N): phase A of this
+    shard into the address `part` (aksel: against the address `center`), phase B on the `nparts` gathered
+    blocks at `blocks`, writing to `meta` (order[n] + status), and phase C into `out`. """
+    lib = _lib.lib()
+    code, (m, mode) = _SEARCH_RULES[self.gar], self._m_mode()
+    status = meta + 4 * self.n if self.status else None
+    return ((lib.bz_distance_partial, (code, ptrs, self.n, center, d, part, ws.data_ptr(), ws.numel(), stream)),
+            (lib.bz_distance_select, (code, blocks, nparts, self.n, self.f, m, mode, meta, status, stream)),
+            (lib.bz_distance_reduce, (code, ptrs, self.n, self.f, m, mode, meta, status, d, out, stream)))
+  def _m_mode(self):
+    """ The m and mode arguments of the bz_distance calls (0 where the rule ignores them). """
+    return (self.m if self.gar in ("krum", "bulyan") else 0), (self.params[1] if self.gar == "aksel" else 0)
   def entry(self, ptrs, d, out, meta, ws, stream, reuse=()):
     """ (fn, args) of the single-GPU call `bz_<gar>` writing to the addresses `out` and `meta`
     (order[n] + status), or of `bz_<gar>_reuse` given the distance cache's `reuse` arguments. """

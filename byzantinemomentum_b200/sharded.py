@@ -31,7 +31,7 @@ import torch.distributed as dist
 from . import _lib
 from . import engine as _engine
 
-__all__ = ["aggregate", "aggregate_p2p", "compute_avg_dev_max", "study_step", "replicate", "apply_update", "shard_bounds", "rows_aligned", "choose_exchange", "choose_search_exchange", "PeerExchange", "FusedExchange", "ShardedPlan", "GradientShards", "choose_delivery", "ShardedLineSearch", "line_search", "COORDINATE_WISE", "DISTANCE_BASED"]
+__all__ = ["aggregate", "aggregate_p2p", "compute_avg_dev_max", "study_step", "replicate", "apply_update", "shard_bounds", "rows_aligned", "choose_exchange", "rows_exchange", "choose_search_exchange", "PeerExchange", "FusedExchange", "ShardedPlan", "GradientShards", "choose_delivery", "ShardedLineSearch", "line_search", "COORDINATE_WISE", "DISTANCE_BASED"]
 
 COORDINATE_WISE = ("average", "median", "trmean", "phocas", "meamed")
 DISTANCE_BASED = _engine.DISTANCE_BASED
@@ -222,6 +222,17 @@ def choose_exchange(gar, exchange, aligned, symmetric, group=None):
     raise ValueError("the p2p exchange needs symmetric memory on every rank")
   return exchange
 
+def rows_exchange(exchange, n):
+  """ The exchange `ShardedPlan` of n rows asks `choose_exchange` for.  The "p2p" and "fused" exchanges
+  serve up to MAX_N rows; above, "auto" is "nccl" and an explicit "p2p" or "fused" raises.  Every rank has
+  the same n, so every rank resolves the same way, before any collective. """
+  if exchange not in EXCHANGES:
+    raise ValueError(f"unknown exchange {exchange!r}")
+  if n <= _lib.MAX_N or exchange in ("auto", "nccl"):
+    return "nccl" if n > _lib.MAX_N else exchange
+  raise ValueError(f"the {exchange} exchange serves at most MAX_N = {_lib.MAX_N} rows, not n = {n}: "
+                   f"above, ShardedPlan exchanges through \"nccl\"")
+
 def _phases(be, gar, gradients, f, m, mode, group, p2p):
   """ (this rank's shard of the result, the selection) of a distance-based rule.  Phase A computes
   this rank's partial block; the R blocks are all-gathered into [R, ...] in rank order, or (`p2p`)
@@ -278,6 +289,10 @@ class ShardedPlan:
                     (`choose_exchange`); a failing symmetric-memory setup raises.
   Both exchanges use the same fixed summation order: bitwise identical selections on every rank.
   Coordinate-wise rules need no exchange and simply wrap `engine.Plan`.
+  Rows: up to MAX_N_DISTANCE for krum, bulyan, aksel and cge, MAX_N for brute.  Above MAX_N the exchange is
+  "nccl" (`rows_exchange`: "auto" resolves to it, "p2p" and "fused" raise), whose phases are
+  `bz_distance_partial`, `bz_distance_select` and `bz_distance_reduce` at every n: the n x n block of 128 rows
+  is 131 KB per rank.  One rank gives `engine.Plan`'s output, selection and status bit for bit.
 
   `graph()` captures a step in a CUDA graph, as `engine.Plan.graph()` does: "fused" on any number of ranks
   (the captured kernel takes its epoch from the exchange buffer, `bz_*_peers_next`), any exchange on one
@@ -298,12 +313,18 @@ class ShardedPlan:
       return
     rule = _engine._rule(gar, n, f, m, mode)
     self._local = None
-    prep = _engine._prepare_device(self.rows)
+    exchange = rows_exchange(exchange, n)
+    limit = _lib.MAX_N_DISTANCE if gar in _engine.WIDE_DISTANCE else _lib.MAX_N
+    prep = _engine._prepare_device(self.rows, limit=limit)
     if not all(g.is_contiguous() for g in self.rows):
       raise ValueError("ShardedPlan takes contiguous rows")
     device = self.device = prep.device
     self.d = prep.d
-    ws = self._ws = _engine._workspace(device, prep.stream)
+    if n > _lib.MAX_N:
+      # the pass tables of bz_distance_partial, held by the plan, as `engine.Plan` holds them
+      ws = self._ws = torch.empty(int(_lib.lib().bz_distance_workspace_bytes(n)), dtype=torch.uint8, device=device)
+    else:
+      ws = self._ws = _engine._workspace(device, prep.stream)
     self.out = torch.empty(prep.d, dtype=torch.float32, device=device)
     self._meta = torch.empty(n + 1, dtype=torch.int32, device=device)
     meta, status, out = self._meta.data_ptr(), self._meta[n:].data_ptr(), self.out.data_ptr()
@@ -323,18 +344,21 @@ class ShardedPlan:
     # aksel: the coordinate-wise median of the local shard is the center of phase A
     self._median = _engine.Plan("median", self.rows) if rule.center else None
     center = None if self._median is None else self._median.out.data_ptr()
-    def phases(part, blocks):
-      return _engine._partial_call(prep, rule.pair, center, part, ws), _engine._select_call(rule, blocks, meta, prep.stream)
     width = n * n if rule.pair else n
     if exchange == "p2p":
+      def phases(part, blocks):
+        return _engine._partial_call(prep, rule.pair, center, part, ws), _engine._select_call(rule, blocks, meta, prep.stream)
       # two slots -> two prepared argument sets; the step counter of the exchange picks one
       self._ex = peer_exchange(n, device, group)
       self._ab = [phases(mine.data_ptr(), peers) for mine, peers in map(self._ex.slot, range(2))]
+      self._c = _engine._reduce_call(prep, rule, meta, status if rule.status else None, out)
     else:
+      # bz_distance_partial / _select / _reduce: one dispatch for 1 to MAX_N_DISTANCE rows
       self._part = torch.empty(width, dtype=torch.float64, device=device)
       self._gathered = torch.empty((self.world, width), dtype=torch.float64, device=device)
-      self._ab = [phases(self._part.data_ptr(), self._gathered)]
-    self._c = _engine._reduce_call(prep, rule, meta, status if rule.status else None, out)
+      a, b, self._c = rule.phase_entries(prep.ptrs, prep.d, center, self._part.data_ptr(), self._gathered.data_ptr(),
+                                         self.world, out, meta, ws, prep.stream)
+      self._ab = [(a, b)]
   def __call__(self):
     if self._local is not None:
       return self._local()

@@ -300,4 +300,8 @@ BZ_API int bz_gradient_row(const float* grad, int64_t d, double clip, float* sam
 /* Multi-Krum, Bulyan, Aksel and CGE for up to BZ_MAX_N_DISTANCE = 128 rows on one GPU: bz_distance. */
 #include "byzagg_distance.h"
 
+/* The phases of the d-sharded path for Multi-Krum, Bulyan, Aksel and CGE up to BZ_MAX_N_DISTANCE rows:
+ * bz_distance_partial, bz_distance_select, bz_distance_reduce. */
+#include "byzagg_distance_shards.h"
+
 #endif /* BYZAGG_H */
