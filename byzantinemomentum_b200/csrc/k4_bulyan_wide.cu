@@ -6,7 +6,8 @@
 // closest values are then read from the sorted shared column at run-time positions.  Everything else is
 // k4_bulyan's: one thread per coordinate, the m_max = n - f - 2 best-scored rows in score order in a shared
 // column of max(m_max, theta) x kK4Threads floats (<= 126 x 512 B), the running means in the reference's
-// order, the lower median, the last strict gain of the closest-beta window.
+// order, the lower median, the last strict gain of the closest-beta window.  Only the window's sum differs: it is
+// accumulated in fp64 and rounded to fp32 once before the division (see below).
 #include "dist.cuh"
 #include "launch.cuh"
 #include "networks_gen.cuh"
@@ -69,9 +70,12 @@ k4_bulyan_wide(const __grid_constant__ WideRowTable rows, const int64_t d, const
     const int dhi = abs_key(__fsub_rn(col[(l + beta) * kK4WideThreads], med));
     lstar = (dlo > dhi) ? l + 1 : lstar;
   }
-  float acc = 0.f;
-  for (int q = 0; q < beta; ++q) acc = __fadd_rn(acc, col[(lstar + q) * kK4WideThreads]);
-  const float r = __fdiv_rn(acc, (float)beta);
+  // The window is added in fp64 and rounded once: beta reaches 124 here, and an ascending fp32 sum of that many
+  // values (aliased rows repeat one value, so its rounding errors add up) drifts past 1e-6 of the exact mean.
+  // The fp32 rounding of the sum keeps the reference's overflow to +-inf, the division stays fp32's.
+  double acc = 0.;
+  for (int q = 0; q < beta; ++q) acc += (double)col[(lstar + q) * kK4WideThreads];
+  const float r = __fdiv_rn(__double2float_rn(acc), (float)beta);
   out[e] = (med != med) ? quiet_nan() : r;
 }
 

@@ -76,11 +76,30 @@ def naive_sum(v):
 def _fp32_sqrt(s):
   return float(orc.fp32_norm(s))
 
-def straddle_split(R, rng, y, key=_fp32_sqrt, alt_slices=None, square=True, tries=200_000):
+def reverse_sum(parts):
+  """ The blocks added in reverse rank order, ((p[R-1] + p[R-2]) + ...) + p0. """
+  return orc.sum_parts(np.asarray(parts)[::-1])
+
+def pairwise_sum(parts):
+  """ The blocks added as a pairwise tree: the sums of the two halves (the first one the larger) added. """
+  parts = np.asarray(parts, dtype=np.float64)
+  if parts.shape[0] == 1:
+    return parts[0].copy()
+  h = (parts.shape[0] + 1) // 2
+  with np.errstate(all="ignore"):
+    return pairwise_sum(parts[:h]) + pairwise_sum(parts[h:])
+
+def other_orders(R):
+  """ The alternative summers that can round R blocks differently from rank order: the reverse from 3 blocks
+  on (two blocks commute), the pairwise tree from 4 on (with 3 it is rank order). """
+  return ([reverse_sum] if R >= 3 else []) + ([pairwise_sum] if R >= 4 else [])
+
+def straddle_split(R, rng, y, key=_fp32_sqrt, alt_slices=None, square=True, tries=200_000, alts=()):
   """ R non-negative fp64 blocks of one entry whose rank-order sum lies within a few ulps of the
   square of the midpoint between y and its upper fp32 neighbour (of the midpoint itself when not
   `square`).  With `alt_slices`, only a split whose rank-order and interleaved sums give different
-  keys is accepted.  Returns (blocks, key of the rank-order sum). """
+  keys is accepted; with `alts` (summers of a [R][1] stack), only a split that every one of them
+  rounds to another key.  Returns (blocks, key of the rank-order sum). """
   y = F32(y)
   mid = (float(y) + float(np.nextafter(y, F32(np.inf)))) / 2.      # exact in fp64
   target = mid * mid if square else mid
@@ -91,13 +110,15 @@ def straddle_split(R, rng, y, key=_fp32_sqrt, alt_slices=None, square=True, trie
     parts[-1] += rng.integers(-4, 5) * math.ulp(target)
     parts = np.maximum(parts, 0.)
     got = key(orc.sum_parts(parts[:, None])[0])
+    if any(got == key(alt(parts[:, None])[0]) for alt in alts):
+      continue
     if alt_slices is None or R == 1:
       return parts, got
     if got != key(interleaved_sum(parts[:, None], alt_slices)[0]):
       return parts, got
   raise RuntimeError(f"no straddling split for R = {R}")
 
-def straddle_table(n, R, seed, alt_slices=None):
+def straddle_table(n, R, seed, alt_slices=None, alts=()):
   """ n x n blocks in which the order of Krum / Bulyan rows 0-3 and brute's best pair hinge on one
   distance: d(0, 1) is the straddled y or its upper neighbour, d(2, 3) is exactly y, every other
   distance 3.0.  Rows 0 and 1 score d(0, 1) + c and rows 2 and 3 y + c (exact sums): a tie kept in
@@ -106,7 +127,7 @@ def straddle_table(n, R, seed, alt_slices=None):
   assert n >= 4
   rng = np.random.default_rng(seed)
   y = F32(rng.uniform(1., 2.))
-  split, d01 = straddle_split(R, rng, y, alt_slices=alt_slices)
+  split, d01 = straddle_split(R, rng, y, alt_slices=alt_slices, alts=alts)
   table = np.full((n, n), 9.)
   table[2, 3] = float(y) * float(y)
   parts = np.zeros((R, n, n))
@@ -116,16 +137,16 @@ def straddle_table(n, R, seed, alt_slices=None):
   parts[:, 0, 1] = split
   return parts.reshape(R, n * n), d01
 
-def straddle_keys(n, R, seed, sqrt_norm, alt_slices=None):
+def straddle_keys(n, R, seed, sqrt_norm, alt_slices=None, alts=()):
   """ [R][n] row keys: key 0 straddles, key 1 is exactly y (its lower neighbour), the rest larger.
   The stable order starts [0, 1] when key 0 rounds to y, [1, 0] otherwise. """
   rng = np.random.default_rng(seed)
   y = F32(rng.uniform(1., 2.))
   if sqrt_norm:
-    split, _ = straddle_split(R, rng, y, alt_slices=alt_slices)
+    split, _ = straddle_split(R, rng, y, alt_slices=alt_slices, alts=alts)
     rest = (float(y) * float(y), 16.)
   else:
-    split, _ = straddle_split(R, rng, y, key=lambda s: float(F32(s)), alt_slices=alt_slices, square=False)
+    split, _ = straddle_split(R, rng, y, key=lambda s: float(F32(s)), alt_slices=alt_slices, square=False, alts=alts)
     rest = (float(y), 4.)
   parts = np.zeros((R, n))
   parts[:, 0] = split
@@ -210,11 +231,47 @@ def neumaier_corpus(count=40, seed=0, max_tries=5_000):
         return out
   raise RuntimeError(f"only {len(out)} discriminating tables")
 
+def neumaier_corpus_wide(count=24, seed=0, max_tries=200):
+  """ (n, f, D) tables of exact fp32 distances, n in 65..128, f in 0..(n-3)//2 (Krum counts n - f - 1 up to 127
+  terms), built rather than sampled: rows 2k and 2k + 1 are at a small integer distance s_k of each other and at
+  one huge power of two B (2^53 or 2^60) of every other row.  A row's score is s_k + (count - 1) B: the naive sum
+  rounds s_k at every power of two the partial sum crosses, the compensated one once, so some pairs the naive sum
+  ties (or inverts) are strictly ordered by sum().  The s_k are drawn within a few ulps of (count - 1) B and put in
+  descending order, so that a tie kept in index order is the inverse of the compensated order.  Only tables whose
+  naive and compensated Krum orders differ are kept. """
+  rng = np.random.default_rng(seed)
+  out = []
+  first = [(128, 0), (127, 0), (65, 31), (96, 1)]          # the longest counts, and the shortest
+  for t in range(max_tries):
+    n = first[t][0] if t < len(first) else int(rng.integers(65, 129))
+    f = first[t][1] if t < len(first) else int(rng.choice([0, 1, int(rng.integers(0, (n - 3) // 2 + 1)), (n - 3) // 2]))
+    big = 2. ** int(rng.choice([53, 60]))
+    ulp = math.ulp((n - f - 2) * big)
+    s = np.sort(rng.integers(1, int(4 * ulp) + 2, n // 2).astype(np.float64))[::-1]
+    D = np.full((n, n), big)
+    for k, v in enumerate(s):
+      D[2 * k, 2 * k + 1] = D[2 * k + 1, 2 * k] = v
+    np.fill_diagonal(D, 0.)
+    if orc._stable_argsort(_krum_scores(D, f, sum)) != orc._stable_argsort(_krum_scores(D, f, naive_sum)):
+      out.append((n, f, D))
+      if len(out) == count:
+        return out
+  raise RuntimeError(f"only {len(out)} discriminating tables")
+
 def square_blocks(D, R=1):
   """ [R][n*n] blocks whose rank-order sum is exactly D**2 above the diagonal (R a power of two:
   equal shares, each exact). """
   sq = np.triu(D * D, 1)
   return np.stack([sq / R] * R).reshape(R, -1)
+
+def tie_table(n, seed, levels=(1., 2.)):
+  """ n x n exact fp32 distances drawn from a few values: rows hold long runs of equal distances (ties in the
+  row sort, broken by column index) and many rows score alike (ties in the stable argsort, kept in index
+  order). """
+  rng = np.random.default_rng(seed)
+  D = np.asarray(levels, dtype=np.float64)[rng.integers(0, len(levels), (n, n))]
+  D = np.triu(D, 1)
+  return D + D.T
 
 # ---------------------------------------------------------------------------------------------- #
 # Brute: planted subsets
@@ -303,6 +360,16 @@ def nonfinite_table(n, R, seed):
     parts[0][big] = sq[big] / 2.
     parts[R - 1][big] = sq[big] / 2.
   return parts.reshape(R, n * n)
+
+def special_keys(n, seed):
+  """ [n] fp64 row sums for Aksel and CGE: NaN, +inf, sums at and just below the fp32 rounding point to +inf,
+  FLT_MAX, 1e300, fp32 ties of different fp64 sums (y^2 and y^2 (1 +- 2^-40)), exact squares and 0, shuffled. """
+  rng = np.random.default_rng(seed)
+  y = float(F32(1.5))
+  special = [math.nan, math.inf, INF_TIE, INF_BELOW, FLT_MAX, 1e300, y * y, y * y * (1 + 2. ** -40),
+             y * y * (1 - 2. ** -40), 0.]
+  rest = rng.integers(1, 6, max(0, n - 3 * len(special))).astype(np.float64) ** 2
+  return rng.permutation(np.concatenate([special * 3, rest])[:n])
 
 # ---------------------------------------------------------------------------------------------- #
 # Bulyan: degenerate boundary

@@ -118,8 +118,7 @@ def test_ranks_select_the_single_gpu_rows(n, nb, d, R):
       want = call(gar, rows, f, m, mode)
       assert np.array_equal(order, want[1]) and status == want[2], what
       assert same_bits(got, want[0]), what
-      if not (gar == "bulyan" and m is not None):      # the oracle's Bulyan bar is set for the default m
-        check_against_oracle(gar, x, nh, got, order, status, f, m, "mid" if mode == 0 else "n-f", what)
+      check_against_oracle(gar, x, nh, got, order, status, f, m, "mid" if mode == 0 else "n-f", what)
 
 @pytest.mark.parametrize("n", [65, 128])
 def test_a_rank_with_an_empty_shard(n):

@@ -10,6 +10,7 @@ import numpy as np
 import pytest
 
 from conftest import Golden, canon_alias
+import bulyan_columns
 import parity
 from oracle import byzoracle as orc
 from test_distance_wide_abi import WD_DIR
@@ -83,7 +84,9 @@ def clear(keys, order, upto, nh):
 
 def check_against_oracle(gar, x, nh, got, order, status, f, m=None, mode="mid", what=""):
   """ The selection (where its margin is clear) and the status bit-exact, the output bit-exact (Multi-Krum,
-  Aksel, CGE) or within the closest-m bar (Bulyan).  Returns whether the selection was compared. """
+  Aksel, CGE) or within the closest-m bar (Bulyan; where the selection is compared, also K4's order bit for bit
+  and within the bar of the exact mean of its window, tests/bulyan_columns.py).  Returns whether the selection
+  was compared. """
   rows = [x[i] for i in range(x.shape[0])]
   n = len(rows)
   if gar == "bulyan":
@@ -98,6 +101,7 @@ def check_against_oracle(gar, x, nh, got, order, status, f, m=None, mode="mid", 
     if not clear(info["scores"], info["order"], n - f - 2, nh):
       return False
     assert canon_alias(order[:n - f - 2], nh) == canon_alias(info["order"][:n - f - 2], nh), what
+    bulyan_columns.check(got, info["stage1"], f, bulyan_columns.uses_wide(n, f), what)
     return True
   if gar == "krum":
     ref, info = orc.krum(rows, f, m, return_info=True)
@@ -120,9 +124,10 @@ def test_every_n_against_the_oracle(n):
   x, nh = stack(n, nb, 67 + 3 * n, seed=n)
   rows = device_rows(x, nh)
   f = (n - 3) // 4                               # the largest f Bulyan takes: theta = n - 2f - 2 down to 33
+  m_max = n - f - 2
   compared = 0
-  for gar, m, mode in (("krum", None, 0), ("krum", 3, 0), ("bulyan", None, 0), ("aksel", None, 0), ("aksel", None, 1),
-                       ("cge", None, 0)):
+  for gar, m, mode in (("krum", None, 0), ("krum", 3, 0), ("bulyan", None, 0), ("bulyan", 1, 0), ("bulyan", m_max // 2, 0),
+                       ("aksel", None, 0), ("aksel", None, 1), ("cge", None, 0)):
     got, order, status = call(gar, rows, f, m, mode)
     compared += check_against_oracle(gar, x, nh, got, order, status, f, m, "mid" if mode == 0 else "n-f", f"{gar} n={n}")
   assert compared >= 2, n
