@@ -1,8 +1,8 @@
 # coding: utf-8
 """ctypes binding of `libbyzagg.so` (C ABI: `include/byzagg.h`, `include/byzagg_shards.h`,
 `include/byzagg_attack.h`, `include/byzagg_search_shards.h`, `include/byzagg_search_peers.h`,
-`include/byzagg_coordinate.h`, `include/byzagg_peers_next.h`, `include/byzagg_distance.h` and
-`include/byzagg_distance_shards.h`).
+`include/byzagg_coordinate.h`, `include/byzagg_peers_next.h`, `include/byzagg_distance.h`,
+`include/byzagg_distance_shards.h` and `include/byzagg_anticge.h`).
 
 The library is loaded lazily, on the first call that needs it, and the load FAILS LOUDLY:
 there is no CPU or PyTorch fallback anywhere in this package.  Build it in-tree with
@@ -132,6 +132,13 @@ DISTANCE_SHARD_SIGNATURES = {
   "bz_distance_select": (_i, [_i, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
   "bz_distance_reduce": (_i, [_i, _c_rows, _i, _i, _i, _i, _vp, _vp, _i64, _vp, _vp]),
 }
+# the same for include/byzagg_anticge.h (the attack against CGE, on one GPU and on the d-sharded path)
+ANTICGE_SIGNATURES = {
+  "bz_anticge_workspace_bytes": (_sz, [_i]),
+  "bz_anticge": (_i, [_c_rows, _i, _i, _i, _i64, _vp, _vp, _sz, _vp]),
+  "bz_anticge_partial": (_i, [_c_rows, _i, _i, _vp, _i64, _vp, _vp, _vp, _sz, _vp]),
+  "bz_anticge_scale": (_i, [_vp, _vp, _vp, _i, _i, _i, _i64, _vp, _vp]),
+}
 SEARCH_STATE_BYTES = 64                     # BZ_SEARCH_STATE_BYTES
 CANDIDATE_FIRST, CANDIDATE_NEXT, CANDIDATE_FINAL = 0, 1, 2
 
@@ -154,7 +161,7 @@ def lib():
       except OSError as err:
         raise LibraryError(f"unable to load {path}: {err}") from err
       tables = (SIGNATURES, SHARD_SIGNATURES, ATTACK_SIGNATURES, SEARCH_SHARD_SIGNATURES, SEARCH_PEER_SIGNATURES,
-                COORDINATE_SIGNATURES, PEER_NEXT_SIGNATURES, DISTANCE_SIGNATURES, DISTANCE_SHARD_SIGNATURES)
+                COORDINATE_SIGNATURES, PEER_NEXT_SIGNATURES, DISTANCE_SIGNATURES, DISTANCE_SHARD_SIGNATURES, ANTICGE_SIGNATURES)
       for name, (restype, argtypes) in [item for table in tables for item in table.items()]:
         try:
           fn = getattr(handle, name)

@@ -322,3 +322,4 @@ int bz_coordinate(int rule, const float* const* rows, int n, int f, int64_t d, f
 #include "api_peers_next.inc"
 #include "api_distance.inc"
 #include "api_distance_shards.inc"
+#include "api_anticge.inc"

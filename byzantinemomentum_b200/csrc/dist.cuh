@@ -246,4 +246,27 @@ void launch_blocks_select_wide(const double* parts, int nparts, int n, int count
 // bz_rowdist_select).
 void launch_rowkeys_select_wide(const double* parts, int nparts, int n, int sqrt_norm, int32_t* order, cudaStream_t st);
 
+// ---- The attack against CGE (bz_anticge, api_anticge.inc; k10_anticge.cu) ----------------------------------------
+// What K11 does to the attack row: multiply by `factor` when `apply` (anticge.py:75-76).
+struct AntiCgeScale {
+  float factor;
+  int apply;
+};
+// K10, chained by PDL: out = σ0 + σ0 + σ1 + ... + σ(maxpos-1) (σ = order, device) and the fp64 Σ out² in one pass;
+// per-CTA blocks in `parts` (kMaxParts doubles), `ticket` zero on entry and left zero.  nparts_k2 > 0: K2''s
+// `nparts_k2` blocks of n sums in `k2_parts` give the key of σ_maxpos and the last CTA writes the decision to `scale`;
+// otherwise it writes the sum to `partial`.  Returns 0, or -1 when the launch fails.
+int launch_anticge_sum(const RowTable& rows, int n, const float* const* host_rows, int maxpos, const int32_t* order, int64_t d,
+                       float* out, double* parts, unsigned* ticket, const double* k2_parts, int nparts_k2,
+                       AntiCgeScale* scale, double* partial, cudaStream_t st);
+int launch_anticge_sum(const WideRowTable& rows, int n, const float* const* host_rows, int maxpos, const int32_t* order,
+                       int64_t d, float* out, double* parts, unsigned* ticket, const double* k2_parts, int nparts_k2,
+                       AntiCgeScale* scale, double* partial, cudaStream_t st);
+// K11, chained by PDL: out *= factor when the decision says so; the decision is `scale`'s, or (blocks != NULL) formed
+// from the `nparts` gathered sums `partials` and the gathered norm blocks `blocks` (nparts x n) by every CTA.
+int launch_anticge_scale(float* out, int64_t d, const AntiCgeScale* scale, const double* blocks, const double* partials,
+                         int nparts, int n, int maxpos, const int32_t* order, cudaStream_t st);
+// out[0, d) = NaN (0x7fc00000).
+int launch_nan_fill(float* out, int64_t d, cudaStream_t st);
+
 }  // namespace bz

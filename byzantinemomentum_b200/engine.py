@@ -26,7 +26,7 @@ __all__ = ["average", "median", "trmean", "phocas", "meamed", "krum", "bulyan", 
            "pairdist_partial", "rowdist_partial", "select", "krum_select", "bulyan_select", "brute_select",
            "rowdist_select", "average_selected", "bulyan_reduce", "avg_dev_max_async", "compute_avg_dev_max", "rowdots_async", "study_step",
            "StudyPartials", "study_partials", "study_finish",
-           "LineSearch", "line_search", "config", "Plan", "pair_cache_stats", "GradientStack", "gradient_scatter", "momentum_rows", "host_path_report"]
+           "LineSearch", "line_search", "AntiCGE", "anticge", "config", "Plan", "pair_cache_stats", "GradientStack", "gradient_scatter", "momentum_rows", "host_path_report"]
 
 class _Config:
   """ strict_status: after brute / bulyan, read the device status word (one 4-byte D2H copy,
@@ -668,6 +668,70 @@ def line_search(gar, grad_honests, f_real, f_decl, grad_avg, grad_att, evals, ne
   byz = search()
   factor, _ = search.result()
   return factor, byz
+
+# ---------------------------------------------------------------------------- #
+# The attack against CGE (attacks/anticge.py)
+
+def anticge_takes(grad_honests, f_decl, f_real):
+  """ Whether `bz_anticge` takes these arguments: 1 to MAX_N_DISTANCE honest rows, integer f_decl with
+  0 <= maxpos = nh - f_decl < nh, integer f_real >= 0.  Outside, the reference indexes from the end or raises. """
+  if not isinstance(grad_honests, (list, tuple)) or not isinstance(f_decl, int) or not isinstance(f_real, int):
+    return False
+  nh = len(grad_honests)
+  return 1 <= nh <= _lib.MAX_N_DISTANCE and 1 <= f_decl <= nh and f_real >= 0
+
+class AntiCGE:
+  """ A prepared `bz_anticge`: the attack of attacks/anticge.py on the honest rows (fp32 CUDA vectors, contiguous),
+  f_decl and f_real — the rows ranked by their norm (CGE's order), the first maxpos = nh - f_decl of them summed
+  with the first counted twice, scaled to just below the norm of the row at maxpos and negated; a row of NaN when
+  f_real > f_decl.  `__call__` only enqueues (no allocation, no synchronisation; `graph()` captures it) and returns
+  the row `byz` f_real times, aliased, as the reference does. """
+  def __init__(self, grad_honests, f_decl, f_real):
+    honest = list(grad_honests)
+    if not anticge_takes(honest, f_decl, f_real):
+      raise ValueError(f"the attack against CGE takes 1..{_lib.MAX_N_DISTANCE} honest rows, 1 <= f_decl <= nh and "
+                       f"f_real >= 0, got nh = {len(honest)}, f_decl = {f_decl!r}, f_real = {f_real!r}")
+    prep = _prepare(honest, limit=_lib.MAX_N_DISTANCE)
+    if prep.to_cpu:
+      raise ValueError("the attack against CGE takes CUDA tensors")
+    if not all(g.is_contiguous() for g in honest):
+      raise ValueError("the attack against CGE takes contiguous honest gradients")
+    self.device, self.f_real, self.rows = prep.device, f_real, honest
+    self.byz = torch.empty(prep.d, dtype=torch.float32, device=prep.device)
+    self._ws = torch.empty(int(_lib.lib().bz_anticge_workspace_bytes(prep.n)), dtype=torch.uint8, device=prep.device)
+    self._fn = _lib.lib().bz_anticge
+    self._args = (prep.ptrs, prep.n, f_decl, f_real, prep.d, self.byz.data_ptr(), self._ws.data_ptr(), self._ws.numel())
+    self._graph = None
+  def _issue(self):
+    return self._fn(*(self._args + (torch.cuda.current_stream(self.device).cuda_stream,)))
+  def __call__(self):
+    """ Enqueue the attack on the current stream of the rows' device; returns [byz] * f_real. """
+    with _on(self.device):
+      code = self._issue()
+    if code != 0:
+      _lib.check(code, self._fn.__name__)
+    return [self.byz] * self.f_real
+  def graph(self):
+    """ Capture the call in a CUDA graph; returns `replay`, which launches it and returns [byz] * f_real. """
+    if self._graph is None:
+      with _on(self.device):
+        self()                                           # warm-up outside the capture
+        torch.cuda.synchronize(self.device)
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph):
+          code = self._issue()
+        if code != 0:
+          _lib.check(code, self._fn.__name__)
+      self._graph = graph
+    graph, byz, count = self._graph, self.byz, self.f_real
+    def replay():
+      graph.replay()
+      return [byz] * count
+    return replay
+
+def anticge(grad_honests, f_decl, f_real):
+  """ attacks/anticge.py's attack on the device (see `AntiCGE`): a new row, returned f_real times. """
+  return AntiCGE(grad_honests, f_decl, f_real)()
 
 # ---------------------------------------------------------------------------- #
 # Study metrics on the same stack (tools/pytorch.py:97-125, attack.py:846-848)

@@ -14,7 +14,8 @@ routes lead there without touching a reference file:
      them (median.py:80-87, krum.py:159-166, bulyan.py:137-144, brute.py:149-156).
 
 `install_attacks(attacks)` then lets the line-searching attacks run their whole search on the device
-(`engine.line_search`) when the rule they attack is one `install` registered.
+(`engine.line_search`) when the rule they attack is one `install` registered, and, asked for by name, the
+attack against CGE run on the device (`engine.anticge`).
 """
 
 import math
@@ -153,7 +154,22 @@ def _empire_strict(stock, backend):
     return [byz] * f_real
   return attack
 
-def install_attacks(attacks, backend=None):
+def _anticge(stock, backend):
+  """ attacks/anticge.py:49-78 on the device (`engine.anticge`) when the honest rows are fp32 CUDA vectors and
+  `bz_anticge` takes the arguments (`engine.anticge_takes`: 1..128 rows, 0 <= nh - f_decl < nh, f_real >= 0);
+  the stock attack, with its arguments unchanged, otherwise. """
+  def attack(grad_honests, f_decl, f_real, **kwargs):
+    import torch
+    from . import engine
+    if (engine.anticge_takes(grad_honests, f_decl, f_real) and _is_cuda(grad_honests)
+        and all(g.dtype == torch.float32 and g.dim() == 1 for g in grad_honests)):
+      return backend.anticge(grad_honests, f_decl, f_real)
+    return stock(grad_honests=grad_honests, f_decl=f_decl, f_real=f_real, **kwargs)
+  return attack
+
+_ATTACK_NAMES = ("little", "empire", "bulyan", "empire-strict")
+
+def install_attacks(attacks, backend=None, names=None):
   """ Replace `little`, `empire`, `bulyan` and `empire-strict` in the reference's `attacks` registry
   (attacks/__init__.py: `attacks`, `register`) with versions that, when the factor (epsilon) is negative
   and `defense` is a rule `install` registered, run the whole `line_maximize` search on the device and
@@ -161,23 +177,30 @@ def install_attacks(attacks, backend=None):
   torch statements.  Every other call — positive factors, a `--gars` mixture, a stock rule, CPU tensors,
   more rows than the search takes for the rule (`engine.search_max_rows`) — runs the stock attack unchanged.  The reference's `register` builds the
   checked wrappers, with the stock checks.
+  `names` may also list "anticge": the attack against CGE then runs on the device (`engine.anticge`) whenever
+  its honest rows are fp32 CUDA vectors and `bz_anticge` takes its arguments, whatever the defense.
   Args:
     attacks  The imported reference `attacks` package
-    backend  Provider of `line_search` (default: `engine`; tests substitute a stand-in)
+    backend  Provider of `line_search` and `anticge` (default: `engine`; tests substitute a stand-in)
+    names    Attacks to replace (default: the four line-searching ones)
   Returns:
     List of the replaced names """
   if backend is None:
     from . import engine as backend
   directions = {"little": _little, "empire": _empire, "bulyan": _bulyan}
   done = []
-  for name in ("little", "empire", "bulyan", "empire-strict"):
+  for name in (_ATTACK_NAMES if names is None else names):
     stock = attacks.attacks.get(name)
     if stock is None:
       continue
-    if name == "empire-strict":
+    if name == "anticge":
+      attack = _anticge(stock.unchecked, backend)
+    elif name == "empire-strict":
       attack = _empire_strict(stock.unchecked, backend)
-    else:
+    elif name in directions:
       attack = _identical(stock.unchecked, directions[name], backend)
+    else:
+      raise KeyError(f"no device version of the attack {name!r}")
     del attacks.attacks[name]                  # `register` refuses duplicates
     attacks.register(name, attack, stock.check)
     setattr(attacks, name, attacks.attacks[name])

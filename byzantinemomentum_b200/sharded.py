@@ -31,7 +31,7 @@ import torch.distributed as dist
 from . import _lib
 from . import engine as _engine
 
-__all__ = ["aggregate", "aggregate_p2p", "compute_avg_dev_max", "study_step", "replicate", "apply_update", "shard_bounds", "rows_aligned", "choose_exchange", "rows_exchange", "choose_search_exchange", "PeerExchange", "FusedExchange", "ShardedPlan", "GradientShards", "choose_delivery", "ShardedLineSearch", "line_search", "COORDINATE_WISE", "DISTANCE_BASED"]
+__all__ = ["aggregate", "aggregate_p2p", "compute_avg_dev_max", "study_step", "replicate", "apply_update", "shard_bounds", "rows_aligned", "choose_exchange", "rows_exchange", "choose_search_exchange", "PeerExchange", "FusedExchange", "ShardedPlan", "GradientShards", "choose_delivery", "ShardedLineSearch", "line_search", "ShardedAntiCGE", "anticge", "COORDINATE_WISE", "DISTANCE_BASED"]
 
 COORDINATE_WISE = ("average", "median", "trmean", "phocas", "meamed")
 DISTANCE_BASED = _engine.DISTANCE_BASED
@@ -914,6 +914,61 @@ def line_search(gar, grad_honests, f_real, f_decl, grad_avg, grad_att, evals, ne
   byz = search()
   factor, _ = search.result()
   return factor, byz
+
+class ShardedAntiCGE:
+  """ `engine.AntiCGE` on a d-sharded trainer: this rank's columns of the honest rows in, this rank's shard of the
+  attack row out, with the same order and the same factor on every rank.  Its stages, each enqueue only:
+    `norms()`            phase A of CGE (`bz_distance_partial`): this shard's sums of squares, nh doubles;
+    `sum(blocks)`        on the R gathered blocks [R, nh]: phase B of CGE (`bz_distance_select`, the order), then
+                         `bz_anticge_partial` (this shard of the unscaled attack); returns its fp64 sum of squares;
+    `scale(partials)`    on the R gathered sums [R]: `bz_anticge_scale`; returns [byz] * f_real.
+  The caller all-gathers between the stages (`anticge` does, with two collectives).  f_real > f_decl needs no
+  exchange: `engine.AntiCGE` fills the shard with NaN. """
+  def __init__(self, grad_honests, f_decl, f_real):
+    honest = list(grad_honests)
+    if not _engine.anticge_takes(honest, f_decl, f_real):
+      raise ValueError(f"the attack against CGE takes 1..{_lib.MAX_N_DISTANCE} honest rows, 1 <= f_decl <= nh and "
+                       f"f_real >= 0, got nh = {len(honest)}, f_decl = {f_decl!r}, f_real = {f_real!r}")
+    prep = self._prep = _engine._prepare_device(honest, "the sharded attack takes CUDA tensors", limit=_lib.MAX_N_DISTANCE)
+    self.rows, self.f_decl, self.f_real, self.device = honest, f_decl, f_real, prep.device
+    lib = _lib.lib()
+    self._dws = torch.empty(int(lib.bz_distance_workspace_bytes(prep.n)), dtype=torch.uint8, device=prep.device)
+    self._ws = torch.empty(int(lib.bz_anticge_workspace_bytes(prep.n)), dtype=torch.uint8, device=prep.device)
+    self.part = torch.empty(prep.n, dtype=torch.float64, device=prep.device)
+    self.order = torch.empty(prep.n, dtype=torch.int32, device=prep.device)
+    self.partial = torch.empty(1, dtype=torch.float64, device=prep.device)
+    self.byz = torch.empty(prep.d, dtype=torch.float32, device=prep.device)
+  def _stream(self):
+    return torch.cuda.current_stream(self.device).cuda_stream
+  def norms(self):
+    p, lib = self._prep, _lib.lib()
+    _engine._run(self.device, lib.bz_distance_partial, (_engine._SEARCH_RULES["cge"], p.ptrs, p.n, None, p.d, self.part.data_ptr(),
+                                                        self._dws.data_ptr(), self._dws.numel(), self._stream()))
+    return self.part
+  def sum(self, blocks):
+    p, lib = self._prep, _lib.lib()
+    self._blocks = blocks = blocks.contiguous()
+    _engine._run(self.device, lib.bz_distance_select, (_engine._SEARCH_RULES["cge"], blocks.data_ptr(), blocks.shape[0], p.n, 0, 0, 0,
+                                                       self.order.data_ptr(), None, self._stream()))
+    _engine._run(self.device, lib.bz_anticge_partial, (p.ptrs, p.n, self.f_decl, self.order.data_ptr(), p.d, self.byz.data_ptr(),
+                                                       self.partial.data_ptr(), self._ws.data_ptr(), self._ws.numel(), self._stream()))
+    return self.partial
+  def scale(self, partials):
+    p, lib = self._prep, _lib.lib()
+    self._partials = partials = partials.contiguous()
+    _engine._run(self.device, lib.bz_anticge_scale, (self._blocks.data_ptr(), self.order.data_ptr(), partials.data_ptr(),
+                                                     partials.numel(), p.n, self.f_decl, p.d, self.byz.data_ptr(), self._stream()))
+    return [self.byz] * self.f_real
+
+def anticge(grad_honests, f_decl, f_real, group=None):
+  """ attacks/anticge.py's attack on a d-sharded trainer (see `ShardedAntiCGE`): every rank passes its columns of
+  the nh honest gradients and gets its shard of the attack row, f_real times, aliased.  Two all-gathers, of nh and
+  of one double per rank; no host read. """
+  if isinstance(f_real, int) and isinstance(f_decl, int) and f_real > f_decl:
+    return _engine.anticge(grad_honests, f_decl, f_real)
+  attack = ShardedAntiCGE(grad_honests, f_decl, f_real)
+  blocks = _gather(attack.norms(), group)
+  return attack.scale(_gather(attack.sum(blocks), group).reshape(-1))
 
 def aggregate(gar, gradients, f=None, m=None, mode="mid", group=None, backend=None, return_selection=False):
   """ Aggregate this rank's shard.

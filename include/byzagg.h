@@ -304,4 +304,8 @@ BZ_API int bz_gradient_row(const float* grad, int64_t d, double clip, float* sam
  * bz_distance_partial, bz_distance_select, bz_distance_reduce. */
 #include "byzagg_distance_shards.h"
 
+/* The attack against CGE generated on the device for up to BZ_MAX_N_DISTANCE honest rows, on one GPU and on the
+ * d-sharded path: bz_anticge, bz_anticge_partial, bz_anticge_scale. */
+#include "byzagg_anticge.h"
+
 #endif /* BYZAGG_H */
