@@ -148,7 +148,8 @@ def test_wide_distance_goldens_cover_the_range_and_stay_apart():
   assert min(ns) == 65 and max(ns) == 128
   gars = {call["gar"] for g in goldens for call in g.calls}
   assert gars == {"krum", "bulyan", "aksel", "cge"}
-  assert {g.manifest["kind"] for g in goldens} >= {"iid", "empire", "little", "nan", "inf", "quant"}
+  assert {g.manifest["kind"] for g in goldens} >= {"iid", "empire", "little", "nan", "inf", "quant",
+                                                   "tiny80", "tiny110", "huge", "mixed", "hugebyz", "nearmax"}
   assert sum((WD_DIR / name).stat().st_size for name in names) < 2 * 1024 * 1024
   assert not list((ROOT / "tests" / "golden").glob("golden_wd_*.npz"))
   assert not list((ROOT / "tests" / "golden" / "wide").glob("golden_wd_*.npz"))
