@@ -11,10 +11,13 @@ Bars (BASELINE.json north_star; SURVEY.md §0.6-0.7, §7.3, Appendix A):
     where ATen's vectorised `mean(dim=0)` switches to another summation order on the
     AVX-512 box the goldens were generated on (<= 1e-6 relative there);
   * closest-m means (phocas, meamed, bulyan stage 2): the reference sums in `topk`'s
-    unspecified order -> 1e-6 relative to the magnitude of the summed values, and any
-    valid resolution of an exact key tie across the selection boundary is accepted; on
-    columns whose magnitudes add up past FLT_MAX the overflow itself depends on that order,
-    so only the column-range check applies there;
+    unspecified order -> 1e-6 relative to the magnitude of the summed values wherever the
+    chosen values are unique, non-finite ones included (`closest_ambiguous`).  Exempt: keys
+    tied across the selection boundary between different values (any valid resolution is
+    accepted), a NaN centre, and columns whose magnitudes add up past FLT_MAX (the overflow
+    itself depends on the order).  There the oracle gets the column-range check, and the
+    kernels are held to their restated order (tests/closest_columns.py for Phocas and MeaMed,
+    tests/bulyan_columns.py for Bulyan's stage 2);
   * distances and norms (krum, bulyan, brute, cge scores; the clip norm; the study scalars):
     ATen's fp32 `norm()` / `dot()` -> +inf once the sum of squares passes FLT_MAX, squares
     below 2^-150 are 0.  Not pinned: a sum within an ulp of the overflow boundary, and sums
@@ -76,23 +79,45 @@ def assert_trmean(got, ref, rows, what=""):
   if body < d:
     assert_close_scaled(got[body:], ref[body:], column_scale(np.asarray(rows)[:, body:]), what + " [ATen tail columns]")
 
-def closest_ambiguous(rows, m, center):
-  """ Coordinates where the m-closest choice is not unique (exact key tie across the
-  boundary) or involves non-finite keys, and columns large enough for an fp32 partial sum
-  to overflow (the reference sums in `topk`'s unspecified order, so +inf, -inf or a finite
-  mean are all possible there): any valid resolution is accepted there. """
+def _magnitude_key(x):
+  """ fl32|x| as ordered integers, every NaN (any sign or payload) largest. """
+  x = np.asarray(x, dtype=np.float32)
+  return np.where(np.isnan(x), np.int32(0x7fffffff), x.view(np.int32) & np.int32(0x7fffffff))
+
+def _value_key(x):
+  """ Integers equal exactly where the fp32 values are equal as values (-0 == +0, NaN == NaN). """
+  x = np.asarray(x, dtype=np.float32)
+  return np.where(np.isnan(x), np.int32(0x7fffffff), np.where(x == 0, np.int32(0), x.view(np.int32)))
+
+def value_ambiguous(rows, m, center):
+  """ Coordinates where the multiset of the m values with the smallest keys fl32|fl32(x - c)| (NaN
+  keys largest) is not unique: keys tie across the selection boundary and the tied entries are not
+  all the same value.  A tie among equal values (a plateau, aliased rows, NaN keys all from +inf)
+  leaves the chosen values, hence the mean up to summation order, unique. """
   rows = np.asarray(rows, dtype=np.float32)
   n = rows.shape[0]
+  if m >= n:
+    return np.zeros(rows.shape[1], dtype=bool)
   with np.errstate(all="ignore"):
-    key = np.abs((rows - center[None, :]).astype(np.float32))
-    magnitude = np.where(np.isfinite(rows), np.abs(rows.astype(np.float64)), 0.).sum(axis=0)
-  nonfinite = ~np.isfinite(key)
-  key = np.where(np.isnan(key), np.inf, key)
+    key = _magnitude_key(rows - np.asarray(center, dtype=np.float32)[None, :])
   sk = np.sort(key, axis=0)
-  amb = nonfinite.any(axis=0) | (magnitude > FLT_MAX)
-  if m < n:
-    amb |= sk[m - 1] == sk[m]
-  return amb
+  tied = (key == sk[m - 1][None, :]) & (sk[m - 1] == sk[m])[None, :]
+  val = _value_key(rows).astype(np.int64)
+  lo = np.where(tied, val, np.int64(1) << 40).min(axis=0)
+  hi = np.where(tied, val, -(np.int64(1) << 40)).max(axis=0)
+  return tied.any(axis=0) & (lo != hi)
+
+def closest_ambiguous(rows, m, center):
+  """ Coordinates where the reference's closest-m mean is not pinned down, so that any valid
+  resolution is accepted there: the chosen values are not unique (`value_ambiguous`), the centre is
+  NaN (the reference then ranks every entry on NaN keys, so which m it averages is unspecified), or
+  the column's magnitudes add up past FLT_MAX (the reference sums in `topk`'s unspecified order, so
+  +inf, -inf or a finite mean are all possible there).  Everywhere else, infinities and NaN included,
+  the chosen values are unique and the mean is compared. """
+  rows = np.asarray(rows, dtype=np.float32)
+  with np.errstate(all="ignore"):
+    magnitude = np.where(np.isfinite(rows), np.abs(rows.astype(np.float64)), 0.).sum(axis=0)
+  return value_ambiguous(rows, m, center) | np.isnan(np.asarray(center, dtype=np.float32)) | (magnitude > FLT_MAX)
 
 def assert_in_hull(got, rows, mask, what=""):
   """ On exempt coordinates a mean of column entries must still lie within the column's

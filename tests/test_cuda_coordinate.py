@@ -10,6 +10,7 @@ import numpy as np
 import pytest
 
 from conftest import Golden
+import closest_columns as cc
 import parity
 from oracle import byzoracle as orc
 from test_coordinate_abi import WIDE_DIR, closest_rtol
@@ -46,13 +47,6 @@ def _device_rows(x, offsets):
     rows.append(buf[off:off + d])
   return rows
 
-def _check_closest(name, got, x, f, center, what):
-  n = x.shape[0]
-  amb = parity.closest_ambiguous(x, n - f, center)
-  parity.assert_close_scaled(got, orc.GARS[name]([x[i] for i in range(n)], f), parity.column_scale(x), f"{name} {what}",
-                             rtol=closest_rtol(n - f), exempt=amb)
-  parity.assert_in_hull(got, x, amb, f"{name} {what}")
-
 def _check_all_rules(x, rows, what, fs=None):
   """ Every rule through bz_coordinate against the oracle: average, median and trimmed mean bit-exact. """
   n, d = x.shape
@@ -61,8 +55,8 @@ def _check_all_rules(x, rows, what, fs=None):
   parity.assert_bit_exact(_coordinate("median", rows, d).cpu().numpy(), orc.median(host), f"median {what}")
   for f in (fs or sorted({1, (n - 1) // 4, (n - 1) // 2})):
     parity.assert_bit_exact(_coordinate("trmean", rows, d, f).cpu().numpy(), orc.trmean(host, f), f"trmean {what} f={f}")
-    _check_closest("phocas", _coordinate("phocas", rows, d, f).cpu().numpy(), x, f, orc.trmean(host, f), f"{what} f={f}")
-    _check_closest("meamed", _coordinate("meamed", rows, d, f).cpu().numpy(), x, f, orc.median(host), f"{what} f={f}")
+    for name in cc.MODES:
+      cc.check_kernel(_coordinate(name, rows, d, f).cpu().numpy(), x, f, name, f"{name} {what} f={f}")
 
 # ---------------------------------------------------------------------------- #
 # The reference's outputs
@@ -99,7 +93,7 @@ def test_matches_the_reference_above_64_rows(g, call):
     center = orc.trmean(np_rows, f) if gar == "phocas" else orc.median(np_rows)
     amb = parity.closest_ambiguous(g.rows, g.n - f, center)
     parity.assert_close_scaled(got, ref, parity.column_scale(g.rows), tag, rtol=closest_rtol(g.n - f), exempt=amb)
-    parity.assert_in_hull(got, g.rows, amb, tag)
+    parity.assert_bit_exact(got, cc.k1_closest(g.rows, f, gar, center)[0], tag + " [K1's closest epilogue]")
 
 # ---------------------------------------------------------------------------- #
 # Every n: NaN, +-inf, -0, subnormals, ties; aligned rows and 4-byte offsets

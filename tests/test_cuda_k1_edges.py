@@ -5,13 +5,15 @@ some VEC groups of a row are all finite and others mixed.  Every n from 1 to 64 
 generic `k1_median` / `k1_sorted` (16-byte aligned rows and mixed-offset views, which take the
 scalar form even where n has a compile-time trimmed-mean network); shared-offset views take the
 shifted vector path.  Median and trimmed mean are bit-exact against the oracle; phocas and meamed
-meet the scaled bar of tests/parity.py."""
+are value for value K1's closest epilogue restated in tests/closest_columns.py, and meet the scaled
+bar of tests/parity.py against the oracle wherever the chosen values are unique."""
 
 import ctypes
 
 import numpy as np
 import pytest
 
+import closest_columns as cc
 import parity
 from oracle import byzoracle as orc
 
@@ -73,14 +75,10 @@ def _check(x, rows, what, fs=None):
   parity.assert_bit_exact(_call("median", rows, d), orc.median(host), f"median {what}")
   if fs is None:
     fs = sorted({1, (n - 1) // 4, (n - 1) // 2} - {0}) if n >= 3 else []
-  scale = parity.column_scale(x)
   for f in fs:
     parity.assert_bit_exact(_call("trmean", rows, d, f), orc.trmean(host, f), f"trmean {what} f={f}")
-    for name, center in (("phocas", orc.trmean(host, f)), ("meamed", orc.median(host))):
-      amb = parity.closest_ambiguous(x, n - f, center)
-      got = _call(name, rows, d, f)
-      parity.assert_close_scaled(got, orc.GARS[name](host, f), scale, f"{name} {what} f={f}", exempt=amb)
-      parity.assert_in_hull(got, x, amb, f"{name} {what} f={f}")
+    for name in cc.MODES:
+      cc.check_kernel(_call(name, rows, d, f), x, f, name, f"{name} {what} f={f}")
 
 @pytest.mark.parametrize("n", list(range(1, 65)))
 def test_special_values_every_n(n):
