@@ -2,7 +2,7 @@
 """ctypes binding of `libbyzagg.so` (C ABI: `include/byzagg.h`, `include/byzagg_shards.h`,
 `include/byzagg_attack.h`, `include/byzagg_search_shards.h`, `include/byzagg_search_peers.h`,
 `include/byzagg_coordinate.h`, `include/byzagg_peers_next.h`, `include/byzagg_distance.h`,
-`include/byzagg_distance_shards.h` and `include/byzagg_anticge.h`).
+`include/byzagg_distance_shards.h`, `include/byzagg_anticge.h` and `include/byzagg_anticge_peers.h`).
 
 The library is loaded lazily, on the first call that needs it, and the load FAILS LOUDLY:
 there is no CPU or PyTorch fallback anywhere in this package.  Build it in-tree with
@@ -139,6 +139,11 @@ ANTICGE_SIGNATURES = {
   "bz_anticge_partial": (_i, [_c_rows, _i, _i, _vp, _i64, _vp, _vp, _vp, _sz, _vp]),
   "bz_anticge_scale": (_i, [_vp, _vp, _vp, _i, _i, _i, _i64, _vp, _vp]),
 }
+# the same for include/byzagg_anticge_peers.h (that attack on the d-sharded path with its exchanges over peer memory)
+ANTICGE_PEER_SIGNATURES = {
+  "bz_anticge_peers": (_i, [_c_rows, _i, _i, _i, _i64, _vp, _vp, _i, _i, _c_rows, _c_rows, ctypes.c_uint, _vp, _sz, _vp]),
+  "bz_anticge_peers_next": (_i, [_c_rows, _i, _i, _i, _i64, _vp, _vp, _i, _i, _c_rows, _c_rows, _vp, _sz, _vp]),
+}
 SEARCH_STATE_BYTES = 64                     # BZ_SEARCH_STATE_BYTES
 CANDIDATE_FIRST, CANDIDATE_NEXT, CANDIDATE_FINAL = 0, 1, 2
 
@@ -161,7 +166,8 @@ def lib():
       except OSError as err:
         raise LibraryError(f"unable to load {path}: {err}") from err
       tables = (SIGNATURES, SHARD_SIGNATURES, ATTACK_SIGNATURES, SEARCH_SHARD_SIGNATURES, SEARCH_PEER_SIGNATURES,
-                COORDINATE_SIGNATURES, PEER_NEXT_SIGNATURES, DISTANCE_SIGNATURES, DISTANCE_SHARD_SIGNATURES, ANTICGE_SIGNATURES)
+                COORDINATE_SIGNATURES, PEER_NEXT_SIGNATURES, DISTANCE_SIGNATURES, DISTANCE_SHARD_SIGNATURES, ANTICGE_SIGNATURES,
+                ANTICGE_PEER_SIGNATURES)
       for name, (restype, argtypes) in [item for table in tables for item in table.items()]:
         try:
           fn = getattr(handle, name)

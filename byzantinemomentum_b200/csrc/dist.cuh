@@ -268,5 +268,20 @@ int launch_anticge_scale(float* out, int64_t d, const AntiCgeScale* scale, const
                          int nparts, int n, int maxpos, const int32_t* order, cudaStream_t st);
 // out[0, d) = NaN (0x7fc00000).
 int launch_nan_fill(float* out, int64_t d, cudaStream_t st);
+// The d-sharded form over peer memory (bz_anticge_peers).  K2'-norms: K2' in CGE mode in bz_distance_partial's
+// geometry, its last CTA exchanging phase A's n sums (PeerTail), keeping their R-summed values in parts[0, n) and
+// writing the stable order of the keys (bz_distance_select's); `ticket`: one word, zeroed here, left zero.
+int launch_anticge_norms(const RowTable& rows, int n, const float* const* host_rows, int64_t d, double* parts, int32_t* order,
+                         unsigned* ticket, const PeerTail& peers, cudaStream_t st);
+int launch_anticge_norms(const WideRowTable& rows, int n, const float* const* host_rows, int64_t d, double* parts,
+                         int32_t* order, unsigned* ticket, const PeerTail& peers, cudaStream_t st);
+// K10 as launch_anticge_sum's sharded form, chained by PDL, its last CTA exchanging the partial sum of squares and
+// writing the decision to `scale` from the R partials and the kept sums `sums` (n doubles).
+int launch_anticge_peers(const RowTable& rows, int n, const float* const* host_rows, int maxpos, const int32_t* order, int64_t d,
+                         float* out, double* parts, unsigned* ticket, const double* sums, AntiCgeScale* scale,
+                         const PeerTail& peers, cudaStream_t st);
+int launch_anticge_peers(const WideRowTable& rows, int n, const float* const* host_rows, int maxpos, const int32_t* order,
+                         int64_t d, float* out, double* parts, unsigned* ticket, const double* sums, AntiCgeScale* scale,
+                         const PeerTail& peers, cudaStream_t st);
 
 }  // namespace bz

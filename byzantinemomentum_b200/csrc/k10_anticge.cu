@@ -12,9 +12,13 @@
 // The d-sharded form (bz_anticge_partial, bz_anticge_scale): K10 writes this rank's unscaled shard and its fp64
 // partial Σ attack² instead of deciding; K11 then forms the same decision in every CTA from the R partials and
 // the gathered norm blocks, added in rank order, so the factor has the same bits on every rank.
+// The d-sharded form over peer memory (bz_anticge_peers, kernel k10_anticge_peers): K10 as in bz_anticge_partial,
+// then its last CTA exchanges the partial (peers.cuh), adds the R partials in rank order and decides from them and
+// the R-summed norms K2'-norms kept, as K11 of bz_anticge_scale does; K11 then reads the decision.
 #include "dist.cuh"
 #include "k5_device.cuh"
 #include "launch.cuh"
+#include "peers.cuh"
 
 namespace bz {
 
@@ -108,15 +112,12 @@ __device__ __forceinline__ void attack_vector(const float* const* srow, int maxp
   for (int c = 0; c < VEC; ++c) sq += (double)acc[c] * (double)acc[c];
 }
 
-// K10.  `nparts_k2` > 0: the single-GPU form, the last CTA writes the decision to `scale` from K2''s blocks `k2_parts`;
-// otherwise (bz_anticge_partial) it writes the fp64 sum of squares to `partial`.  `ticket` is zero on entry and again
-// on exit.
+// K10's pass: this CTA's columns of the attack row into `out`, its fp64 block of Σ out² into parts[blockIdx.x];
+// true in the last CTA to finish (the ticket), which may then read every block.
 template <int VEC, class Rows>
-__global__ void __launch_bounds__(kAcThreads)
-k10_anticge_sum(const __grid_constant__ Rows rows, const int n, const int maxpos, const int32_t* __restrict__ order,
-                const Geom g, float* __restrict__ out, double* __restrict__ parts, unsigned* __restrict__ ticket,
-                const double* __restrict__ k2_parts, const int nparts_k2, AntiCgeScale* __restrict__ scale,
-                double* __restrict__ partial) {
+__device__ __forceinline__ bool attack_pass(const Rows& rows, const int maxpos, const int32_t* __restrict__ order,
+                                            const Geom& g, float* __restrict__ out, double* __restrict__ parts,
+                                            unsigned* __restrict__ ticket) {
   __shared__ const float* srow[kMaxNDistance];
   __shared__ double warp_sum[kAcWarps];
   __shared__ bool last;
@@ -137,12 +138,68 @@ k10_anticge_sum(const __grid_constant__ Rows rows, const int n, const int maxpos
     last = atomicAdd(ticket, 1u) == gridDim.x - 1;
   }
   __syncthreads();
-  if (!last || threadIdx.x != 0) return;
+  return last;
+}
+
+// K10.  `nparts_k2` > 0: the single-GPU form, the last CTA writes the decision to `scale` from K2''s blocks `k2_parts`;
+// otherwise (bz_anticge_partial) it writes the fp64 sum of squares to `partial`.  `ticket` is zero on entry and again
+// on exit.
+template <int VEC, class Rows>
+__global__ void __launch_bounds__(kAcThreads)
+k10_anticge_sum(const __grid_constant__ Rows rows, const int n, const int maxpos, const int32_t* __restrict__ order,
+                const Geom g, float* __restrict__ out, double* __restrict__ parts, unsigned* __restrict__ ticket,
+                const double* __restrict__ k2_parts, const int nparts_k2, AntiCgeScale* __restrict__ scale,
+                double* __restrict__ partial) {
+  if (!attack_pass<VEC>(rows, maxpos, order, g, out, parts, ticket) || threadIdx.x != 0) return;
   __threadfence();
   double sum = 0.;                               // the blocks in block order
   for (int p = 0; p < (int)gridDim.x; ++p) sum += __ldcg(parts + p);
   if (partial != nullptr) *partial = sum;
   else                    *scale = anticge_decision(sum, rowdist_key(k2_parts, nparts_k2, n, order[maxpos]));
+  *ticket = 0u;
+}
+
+// K10 with the second exchange of bz_anticge_peers.  The last CTA forms bz_anticge_partial's sum, publishes it in
+// this rank's slot, flags and waits (peers.cuh), adds the R partials in rank order, ((p0 + p1) + p2) + ..., and
+// writes to `scale` the decision k11_anticge_scale forms from the gathered partials and blocks: the key of σ_maxpos
+// comes from `sums`, the R-summed norm sums K2'-norms kept in this rank's workspace (the peers' slots of the first
+// exchange may be rewritten once this rank has signalled).  A timeout sets *peers.status; it is never cleared here.
+template <int VEC, class Rows>
+__global__ void __launch_bounds__(kAcThreads)
+k10_anticge_peers(const __grid_constant__ Rows rows, const int n, const int maxpos, const int32_t* __restrict__ order,
+                  const Geom g, float* __restrict__ out, double* __restrict__ parts, unsigned* __restrict__ ticket,
+                  const double* __restrict__ sums, AntiCgeScale* __restrict__ scale, const __grid_constant__ PeerTail peers) {
+  __shared__ int peer_timeout;
+  if (!attack_pass<VEC>(rows, maxpos, order, g, out, parts, ticket)) return;
+  __threadfence();
+  // the epoch and the slot: by value, or (`next`) from this rank's own flags, which K2'-norms raised before this
+  // grid's pdl_wait; read by every thread that needs them before the barrier below
+  unsigned epoch = peers.epoch;
+  int slot = 0;
+  if (peers.next && (int)threadIdx.x < peers.nranks) {
+    epoch = next_epoch(peers.flag[0][peers.rank] + peers.rank, peers.flag[1][peers.rank] + peers.rank);
+    slot = (int)(epoch & 1u);
+  }
+  double* const* blocks = peers.block[slot];
+  unsigned* const* flags = peers.flag[slot];
+  if (threadIdx.x == 0) {
+    double sum = 0.;                             // the blocks in block order: bz_anticge_partial's sum
+    for (int p = 0; p < (int)gridDim.x; ++p) sum += __ldcg(parts + p);
+    blocks[peers.rank][0] = sum;
+    peer_timeout = 0;
+  }
+  __threadfence_system();
+  __syncthreads();
+  if ((int)threadIdx.x < peers.nranks &&
+      peer_signal_wait(flags[threadIdx.x] + peers.rank, flags[peers.rank] + threadIdx.x, epoch))
+    peer_timeout = 1;
+  __syncthreads();
+  asm volatile("" ::: "memory");      // the partial loads below stay below the flag wait
+  if (threadIdx.x != 0) return;
+  double sum = ld_relaxed_sys_f64(blocks[0]);
+  for (int r = 1; r < peers.nranks; ++r) sum += ld_relaxed_sys_f64(blocks[r]);
+  *scale = anticge_decision(sum, gathered_key(sums, 1, n, order[maxpos]));
+  if (peer_timeout && peers.status != nullptr) *peers.status = BZ_STATUS_PEER_TIMEOUT;
   *ticket = 0u;
 }
 
@@ -182,16 +239,22 @@ __global__ void __launch_bounds__(kAcThreads) k_nan_fill(float* __restrict__ out
   for (int64_t j = (int64_t)blockIdx.x * kAcThreads + threadIdx.x; j < d; j += stride) out[j] = quiet_nan();
 }
 
-template <class Rows>
-static int launch_sum(const Rows& rows, int n, const float* const* host_rows, int maxpos, const int32_t* order, int64_t d,
-                      float* out, double* parts, unsigned* ticket, const double* k2_parts, int nparts_k2,
-                      AntiCgeScale* scale, double* partial, cudaStream_t st) {
-  const Geom g = make_geom(host_rows, n, out, nullptr, d, 4);
+// K10's grid over the vectors of g: up to two CTAs per SM and kMaxParts blocks, at least one (an empty shard too).
+static unsigned sum_grid(const Geom& g) {
   int64_t grid = (g.nv + kAcThreads - 1) / kAcThreads;
   const int64_t cap = (int64_t)sm_count() * 2;
   if (grid > cap) grid = cap;
   if (grid > kMaxParts) grid = kMaxParts;
   if (grid < 1) grid = 1;
+  return (unsigned)grid;
+}
+
+template <class Rows>
+static int launch_sum(const Rows& rows, int n, const float* const* host_rows, int maxpos, const int32_t* order, int64_t d,
+                      float* out, double* parts, unsigned* ticket, const double* k2_parts, int nparts_k2,
+                      AntiCgeScale* scale, double* partial, cudaStream_t st) {
+  const Geom g = make_geom(host_rows, n, out, nullptr, d, 4);
+  const unsigned grid = sum_grid(g);
   const cudaError_t err = g.vec == 4
       ? launch_after(k10_anticge_sum<4, Rows>, (unsigned)grid, kAcThreads, 0, st, rows, n, maxpos, order, g, out, parts, ticket,
                      k2_parts, nparts_k2, scale, partial)
@@ -209,6 +272,31 @@ int launch_anticge_sum(const WideRowTable& rows, int n, const float* const* host
                        int64_t d, float* out, double* parts, unsigned* ticket, const double* k2_parts, int nparts_k2,
                        AntiCgeScale* scale, double* partial, cudaStream_t st) {
   return launch_sum(rows, n, host_rows, maxpos, order, d, out, parts, ticket, k2_parts, nparts_k2, scale, partial, st);
+}
+
+template <class Rows>
+static int launch_peers(const Rows& rows, int n, const float* const* host_rows, int maxpos, const int32_t* order, int64_t d,
+                        float* out, double* parts, unsigned* ticket, const double* sums, AntiCgeScale* scale,
+                        const PeerTail& peers, cudaStream_t st) {
+  const Geom g = make_geom(host_rows, n, out, nullptr, d, 4);       // bz_anticge_partial's geometry and grid
+  const unsigned grid = sum_grid(g);
+  const cudaError_t err = g.vec == 4
+      ? launch_after(k10_anticge_peers<4, Rows>, grid, kAcThreads, 0, st, rows, n, maxpos, order, g, out, parts, ticket, sums,
+                     scale, peers)
+      : launch_after(k10_anticge_peers<1, Rows>, grid, kAcThreads, 0, st, rows, n, maxpos, order, g, out, parts, ticket, sums,
+                     scale, peers);
+  return err == cudaSuccess ? 0 : -1;
+}
+
+int launch_anticge_peers(const RowTable& rows, int n, const float* const* host_rows, int maxpos, const int32_t* order, int64_t d,
+                         float* out, double* parts, unsigned* ticket, const double* sums, AntiCgeScale* scale,
+                         const PeerTail& peers, cudaStream_t st) {
+  return launch_peers(rows, n, host_rows, maxpos, order, d, out, parts, ticket, sums, scale, peers, st);
+}
+int launch_anticge_peers(const WideRowTable& rows, int n, const float* const* host_rows, int maxpos, const int32_t* order,
+                         int64_t d, float* out, double* parts, unsigned* ticket, const double* sums, AntiCgeScale* scale,
+                         const PeerTail& peers, cudaStream_t st) {
+  return launch_peers(rows, n, host_rows, maxpos, order, d, out, parts, ticket, sums, scale, peers, st);
 }
 
 int launch_anticge_scale(float* out, int64_t d, const AntiCgeScale* scale, const double* blocks, const double* partials,

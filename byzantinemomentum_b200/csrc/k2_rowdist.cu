@@ -32,7 +32,10 @@ constexpr int kRdFlush = 8;      // vectors between two flushes
 // PEERS (kernel k2_rowdist_peers): the last CTA exchanges its sum over peer memory first (`peers`,
 // PeerTail): the selection, or the transition, then runs on the R ranks' sums added in rank order,
 // bitwise the same on every rank.
-template <bool CENTER, int VEC, bool DOT, bool SEARCH, bool PEERS>
+// KEEP (kernel k2_anticge_norms, with PEERS): the last CTA also writes those R-summed sums to parts[0, n),
+// once it has read every block there, for the attack against CGE (k10_anticge.cu) to take the key of σ_maxpos
+// from after this rank's slot may have been rewritten by a peer.
+template <bool CENTER, int VEC, bool DOT, bool SEARCH, bool PEERS, bool KEEP = false>
 __device__ __forceinline__ void
 rowdist_body(const RowTable& rows, const int n, const float* __restrict__ center, const Geom g,
              double* __restrict__ parts, int32_t* __restrict__ order, unsigned* __restrict__ ticket, const int sqrt_norm,
@@ -189,6 +192,7 @@ rowdist_body(const RowTable& rows, const int n, const float* __restrict__ center
     if (threadIdx.x < n) {
       sum = ld_relaxed_sys_f64(blocks[0] + threadIdx.x);
       for (int r = 1; r < peers.nranks; ++r) sum += ld_relaxed_sys_f64(blocks[r] + threadIdx.x);
+      if (KEEP) parts[threadIdx.x] = sum;           // every block was read before the barrier above
     }
   }
   if (threadIdx.x < n) {
@@ -229,6 +233,14 @@ k2_rowdist_peers(const __grid_constant__ RowTable rows, const int n, const float
                  double* __restrict__ parts, int32_t* __restrict__ order, unsigned* __restrict__ ticket, const int sqrt_norm,
                  const SearchTail search, const __grid_constant__ PeerTail peers) {
   rowdist_body<CENTER, VEC, false, SEARCH, true>(rows, n, center, g, parts, order, ticket, sqrt_norm, search, peers);
+}
+
+// K2' in CGE mode with the peers tail, keeping the R-summed sums (bz_anticge_peers' first exchange).
+template <int VEC>
+__global__ void __launch_bounds__(kRdThreads, 2)
+k2_anticge_norms(const __grid_constant__ RowTable rows, const int n, const Geom g, double* __restrict__ parts,
+                 int32_t* __restrict__ order, unsigned* __restrict__ ticket, const __grid_constant__ PeerTail peers) {
+  rowdist_body<false, VEC, false, false, true, true>(rows, n, nullptr, g, parts, order, ticket, 1, SearchTail{}, peers);
 }
 
 // Blocks of a K2' launch over the vectors of g: up to two per SM, at least one (an empty shard too).
@@ -278,6 +290,17 @@ int launch_rowdist_peers(const RowTable& rows, int n, const float* const* host_r
     if (center) k2_rowdist_peers<true, 1, false><<<grid, kRdThreads, 0, st>>>(rows, n, center, g, parts, order, ticket, sqrt_norm, none, peers);
     else        k2_rowdist_peers<false, 1, false><<<grid, kRdThreads, 0, st>>>(rows, n, center, g, parts, order, ticket, sqrt_norm, none, peers);
   }
+  return (int)grid;
+}
+
+int launch_anticge_norms(const RowTable& rows, int n, const float* const* host_rows, int64_t d, double* parts, int32_t* order,
+                         unsigned* ticket, const PeerTail& peers, cudaStream_t st) {
+  // bz_distance_partial's geometry for CGE (bz_rowdist_partial's), as launch_rowdist_peers
+  const Geom g = make_geom(host_rows, n, (const void*)host_rows[0], nullptr, d, 4);
+  const unsigned grid = rowdist_grid(g);
+  cudaMemsetAsync(ticket, 0, sizeof(unsigned), st);
+  if (g.vec == 4) k2_anticge_norms<4><<<grid, kRdThreads, 0, st>>>(rows, n, g, parts, order, ticket, peers);
+  else            k2_anticge_norms<1><<<grid, kRdThreads, 0, st>>>(rows, n, g, parts, order, ticket, peers);
   return (int)grid;
 }
 

@@ -10,8 +10,12 @@
 // through shared memory in fixed order, one fp64 block per CTA; the last CTA (ticket) sums the blocks in S
 // interleaved classes, the class sums in class order, and writes the stable order of the n keys.
 // Deterministic; identical rows give identical sums.  Roofline: HBM, n·4 B per coordinate (+4 B for the centre).
+// K2'-norms (k2_anticge_norms_wide, bz_anticge_peers' first exchange): CGE mode with the exchange over peer memory
+// in the last CTA, as k2_rowdist's peers tail does up to 64 rows: it publishes the n sums K2'-share would write,
+// adds the R ranks' sums in rank order, keeps them in parts[0, n) and writes the stable order of their keys.
 #include "dist.cuh"
 #include "k5_device.cuh"
+#include "peers.cuh"
 #include "reduce.cuh"
 
 namespace bz {
@@ -20,12 +24,55 @@ constexpr int kRwThreads = 256;
 constexpr int kRwWarps = kRwThreads / 32;
 constexpr int kRwChunks = kMaxNDistance / 32;
 
+// The last CTA of K2'-norms after the class sums are in `partial`: thread c < n forms the sum K2'-share writes,
+// publishes it in this rank's slot, flags and waits (peers.cuh), adds the R ranks' sums in rank order,
+// ((p0 + p1) + p2) + ..., keeps that in parts[c] (every block was read before the caller's barrier), and the stable
+// order of the keys follows as in k2_rowdist_wide.  The epoch and the slot: by value, or (`next`) from this
+// rank's own flags, read before the barrier that precedes the signal.
+__device__ __forceinline__ void rowdist_wide_peers_tail(const PeerTail& peers, const double* partial, double* key, int S, int n,
+                                                        double* __restrict__ parts, int32_t* __restrict__ order,
+                                                        unsigned* __restrict__ ticket) {
+  __shared__ int peer_timeout;
+  double sum = 0.;
+  if (threadIdx.x < n)
+    for (int k = 0; k < S; ++k) sum += partial[k * n + threadIdx.x];
+  unsigned epoch = peers.epoch;
+  int slot = 0;
+  if (peers.next && ((int)threadIdx.x < n || (int)threadIdx.x < peers.nranks)) {
+    epoch = next_epoch(peers.flag[0][peers.rank] + peers.rank, peers.flag[1][peers.rank] + peers.rank);
+    slot = (int)(epoch & 1u);
+  }
+  double* const* blocks = peers.block[slot];
+  unsigned* const* flags = peers.flag[slot];
+  if (threadIdx.x == 0) peer_timeout = 0;
+  if (threadIdx.x < n) blocks[peers.rank][threadIdx.x] = sum;
+  __threadfence_system();
+  __syncthreads();
+  if ((int)threadIdx.x < peers.nranks &&
+      peer_signal_wait(flags[threadIdx.x] + peers.rank, flags[peers.rank] + threadIdx.x, epoch))
+    peer_timeout = 1;
+  __syncthreads();
+  asm volatile("" ::: "memory");      // the block loads below stay below the flag wait
+  if (threadIdx.x < n) {
+    sum = ld_relaxed_sys_f64(blocks[0] + threadIdx.x);
+    for (int r = 1; r < peers.nranks; ++r) sum += ld_relaxed_sys_f64(blocks[r] + threadIdx.x);
+    parts[threadIdx.x] = sum;
+    const double v = (double)fp32_norm(sum);           // cge.py:36-37: fp32 norm, non-finite -> +inf
+    key[threadIdx.x] = finite_d(v) ? v : CUDART_INF;
+  }
+  if (threadIdx.x == 0 && peers.status != nullptr) *peers.status = peer_timeout ? BZ_STATUS_PEER_TIMEOUT : BZ_STATUS_OK;
+  __syncthreads();
+  stable_order(key, n, order);
+  if (threadIdx.x == 0) *ticket = 0u;
+}
+
 // SUMS: the last CTA writes the n sums to `sums` (K2'-share); otherwise the stable order of their keys to `order`.
-template <bool CENTER, bool SUMS>
+// PEERS (CGE, not SUMS): the sums are exchanged first (`peers`), and the R-summed sums are kept in parts[0, n).
+template <bool CENTER, bool SUMS, bool PEERS = false>
 __device__ __forceinline__ void rowdist_wide_body(const WideRowTable& rows, const int n, const float* __restrict__ center,
                                                   const Geom& g, double* __restrict__ parts, int32_t* __restrict__ order,
                                                   unsigned* __restrict__ ticket, const int sqrt_norm,
-                                                  double* __restrict__ sums) {
+                                                  double* __restrict__ sums, const PeerTail* peers = nullptr) {
   __shared__ double warp_tot[kRwWarps][kMaxNDistance];
   __shared__ bool last;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -95,6 +142,10 @@ __device__ __forceinline__ void rowdist_wide_body(const WideRowTable& rows, cons
     partial[cls * n + c] = s;
   }
   __syncthreads();
+  if (PEERS) {
+    rowdist_wide_peers_tail(*peers, partial, key, S, n, parts, order, ticket);
+    return;
+  }
   if (threadIdx.x < n) {
     double sum = 0.;
     for (int k = 0; k < S; ++k) sum += partial[k * n + threadIdx.x];
@@ -132,7 +183,13 @@ k2_rowshare_wide(const __grid_constant__ WideRowTable rows, const int n, const f
   rowdist_wide_body<CENTER, true>(rows, n, center, g, parts, nullptr, ticket, 0, sums);
 }
 
-// The geometry of both kernels: at most two CTAs per SM and kMaxParts blocks; the ticket is zeroed first.
+__global__ void __launch_bounds__(kRwThreads, 2)
+k2_anticge_norms_wide(const __grid_constant__ WideRowTable rows, const int n, const Geom g, double* __restrict__ parts,
+                      int32_t* __restrict__ order, unsigned* __restrict__ ticket, const __grid_constant__ PeerTail peers) {
+  rowdist_wide_body<false, false, true>(rows, n, nullptr, g, parts, order, ticket, 1, nullptr, &peers);
+}
+
+// The geometry of the kernels: at most two CTAs per SM and kMaxParts blocks; the ticket is zeroed first.
 static unsigned rowdist_wide_grid(const float* const* host_rows, int n, const float* center, int64_t d, int reverse,
                                   unsigned* ticket, cudaStream_t st, Geom& g) {
   g = make_geom(host_rows, n, center, nullptr, d, 1);
@@ -161,6 +218,15 @@ int launch_rowshare(const WideRowTable& rows, int n, const float* const* host_ro
   const unsigned grid = rowdist_wide_grid(host_rows, n, center, d, reverse, ticket, st, g);
   if (center) k2_rowshare_wide<true><<<grid, kRwThreads, 0, st>>>(rows, n, center, g, parts, ticket, sums);
   else        k2_rowshare_wide<false><<<grid, kRwThreads, 0, st>>>(rows, n, center, g, parts, ticket, sums);
+  return (int)grid;
+}
+
+int launch_anticge_norms(const WideRowTable& rows, int n, const float* const* host_rows, int64_t d, double* parts,
+                         int32_t* order, unsigned* ticket, const PeerTail& peers, cudaStream_t st) {
+  Geom g;
+  // launch_rowshare's geometry for CGE (bz_distance_partial), so that the published sums are phase A's
+  const unsigned grid = rowdist_wide_grid(host_rows, n, nullptr, d, 0, ticket, st, g);
+  k2_anticge_norms_wide<<<grid, kRwThreads, 0, st>>>(rows, n, g, parts, order, ticket, peers);
   return (int)grid;
 }
 

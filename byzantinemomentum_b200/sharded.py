@@ -31,7 +31,7 @@ import torch.distributed as dist
 from . import _lib
 from . import engine as _engine
 
-__all__ = ["aggregate", "aggregate_p2p", "compute_avg_dev_max", "study_step", "replicate", "apply_update", "shard_bounds", "rows_aligned", "choose_exchange", "rows_exchange", "choose_search_exchange", "PeerExchange", "FusedExchange", "ShardedPlan", "GradientShards", "choose_delivery", "ShardedLineSearch", "line_search", "ShardedAntiCGE", "anticge", "COORDINATE_WISE", "DISTANCE_BASED"]
+__all__ = ["aggregate", "aggregate_p2p", "compute_avg_dev_max", "study_step", "replicate", "apply_update", "shard_bounds", "rows_aligned", "choose_exchange", "rows_exchange", "choose_search_exchange", "PeerExchange", "FusedExchange", "ShardedPlan", "GradientShards", "choose_delivery", "ShardedLineSearch", "line_search", "choose_anticge_exchange", "ShardedAntiCGE", "anticge", "COORDINATE_WISE", "DISTANCE_BASED"]
 
 COORDINATE_WISE = ("average", "median", "trmean", "phocas", "meamed")
 DISTANCE_BASED = _engine.DISTANCE_BASED
@@ -101,6 +101,10 @@ class FusedExchange:
   same buffer: one per call here, each advancing `epoch` by one.  That relies on one condition: the calls
   that share a FusedExchange (the search and the `ShardedPlan` of the same n) are issued on ONE stream, in
   the same order on every rank.
+  `ShardedAntiCGE(exchange="fused")` of nh honest rows runs its two exchanges (the nh norm sums, then the
+  attack's sum of squares) over the buffer of n = nh in one `bz_anticge_peers` call, advancing `epoch` by two
+  (by none when f_real > f_decl: the NaN fill exchanges nothing).  It shares the buffer with a `ShardedPlan`
+  or `ShardedLineSearch` of the same n on the same condition: one stream, the same order on every rank.
   `epoch` is the host's count of the exchanges issued so far; the flags hold the same count on the device
   (this rank's own entry [rank] of its flag array, in the slot of its last epoch).  The eager calls pass
   `epoch` by value.  A captured call (`ShardedPlan.graph()`, `ShardedLineSearch.graph()`) cannot: its
@@ -915,6 +919,25 @@ def line_search(gar, grad_honests, f_real, f_decl, grad_avg, grad_att, evals, ne
   factor, _ = search.result()
   return factor, byz
 
+def choose_anticge_exchange(exchange, symmetric, group=None):
+  """ The exchange of `ShardedAntiCGE`, the same on every rank of `group`: the local fact `symmetric` (symmetric
+  memory can be set up here) is agreed on with one all-reduce (MIN), as in `choose_search_exchange`.  "auto" takes
+  "fused" on 2 to 16 ranks that all have symmetric memory, else "nccl" (one rank keeps the collective stages).  An
+  explicit "fused" needs symmetric memory on every one of at most 16 ranks unless there is one rank (its buffer is
+  then plain device memory); otherwise it raises on every rank.  Rows may have any alignment.  Returns "fused" or
+  "nccl". """
+  if exchange not in SEARCH_EXCHANGES:
+    raise ValueError(f"unknown exchange {exchange!r}")
+  world = dist.get_world_size(group) if dist.is_initialized() else 1
+  (symmetric,) = map(bool, _agree([int(bool(symmetric))], group))
+  fusable = world == 1 or (symmetric and world <= _lib.MAX_PEERS)
+  if exchange == "auto":
+    return "fused" if world > 1 and fusable else "nccl"
+  if exchange == "fused" and not fusable:
+    raise ValueError(f"the fused exchange of the attack against CGE needs symmetric memory on every one of at most "
+                     f"{_lib.MAX_PEERS} ranks")
+  return exchange
+
 class ShardedAntiCGE:
   """ `engine.AntiCGE` on a d-sharded trainer: this rank's columns of the honest rows in, this rank's shard of the
   attack row out, with the same order and the same factor on every rank.  Its stages, each enqueue only:
@@ -922,15 +945,30 @@ class ShardedAntiCGE:
     `sum(blocks)`        on the R gathered blocks [R, nh]: phase B of CGE (`bz_distance_select`, the order), then
                          `bz_anticge_partial` (this shard of the unscaled attack); returns its fp64 sum of squares;
     `scale(partials)`    on the R gathered sums [R]: `bz_anticge_scale`; returns [byz] * f_real.
-  The caller all-gathers between the stages (`anticge` does, with two collectives).  f_real > f_decl needs no
-  exchange: `engine.AntiCGE` fills the shard with NaN. """
-  def __init__(self, grad_honests, f_decl, f_real):
+  The caller all-gathers between the stages.  f_real > f_decl needs no exchange: `engine.AntiCGE` fills the shard
+  with NaN.
+
+  `attack()` issues a whole step on the current stream, with no host read, and returns [byz] * f_real:
+  exchange: "nccl"   the stages and the two all-gathers (of nh doubles, then of one double per rank);
+            "fused"  one `bz_anticge_peers` call over the buffer of `fused_exchange(nh, ...)` (a plain device buffer
+                     on one rank): both exchanges run inside its kernels, over peer memory, and each call advances
+                     the buffer's `epoch` by two.  The same bits as "nccl".  The buffer may be shared with a
+                     `ShardedPlan` or `ShardedLineSearch` of the same n, whose calls are then issued on the same
+                     stream, in the same order on every rank;
+            "auto"   "fused" on 2..16 ranks that all have symmetric memory, else "nccl"; the ranks agree on it
+                     (`choose_anticge_exchange`).
+  `graph()` captures a step in a CUDA graph: "fused" on any number of ranks (the captured call takes its epoch from
+  the buffer, `bz_anticge_peers_next`), "nccl" on one rank.  Like a call, `graph()` and every replay are collective:
+  every rank issues them at the same point of its stream order. """
+  def __init__(self, grad_honests, f_decl, f_real, group=None, exchange="auto"):
     honest = list(grad_honests)
     if not _engine.anticge_takes(honest, f_decl, f_real):
       raise ValueError(f"the attack against CGE takes 1..{_lib.MAX_N_DISTANCE} honest rows, 1 <= f_decl <= nh and "
                        f"f_real >= 0, got nh = {len(honest)}, f_decl = {f_decl!r}, f_real = {f_real!r}")
     prep = self._prep = _engine._prepare_device(honest, "the sharded attack takes CUDA tensors", limit=_lib.MAX_N_DISTANCE)
     self.rows, self.f_decl, self.f_real, self.device = honest, f_decl, f_real, prep.device
+    self.group = group
+    self.world = dist.get_world_size(group) if dist.is_initialized() else 1
     lib = _lib.lib()
     self._dws = torch.empty(int(lib.bz_distance_workspace_bytes(prep.n)), dtype=torch.uint8, device=prep.device)
     self._ws = torch.empty(int(lib.bz_anticge_workspace_bytes(prep.n)), dtype=torch.uint8, device=prep.device)
@@ -938,6 +976,19 @@ class ShardedAntiCGE:
     self.order = torch.empty(prep.n, dtype=torch.int32, device=prep.device)
     self.partial = torch.empty(1, dtype=torch.float64, device=prep.device)
     self.byz = torch.empty(prep.d, dtype=torch.float32, device=prep.device)
+    self._graph, self.status = None, None
+    self.exchange = choose_anticge_exchange(exchange, _symmetric_memory_importable(), group)
+    if self.exchange == "fused":
+      self.status = torch.zeros(1, dtype=torch.int32, device=prep.device)
+      self._fuse(FusedExchange.local(prep.n, prep.device) if self.world == 1 else fused_exchange(prep.n, prep.device, group))
+  def _fuse(self, fx):
+    """ Run the fused exchanges over `fx`, a FusedExchange of n = nh. """
+    p = self._prep
+    self._fx = fx
+    self._fused_head = (p.ptrs, p.n, self.f_decl, self.f_real, p.d, self.byz.data_ptr(), self.status.data_ptr(), fx.rank,
+                        fx.world) + fx.both()
+    self._fused_tail = (self._ws.data_ptr(), self._ws.numel())
+    self._exchanges = 0 if self.f_real > self.f_decl else 2
   def _stream(self):
     return torch.cuda.current_stream(self.device).cuda_stream
   def norms(self):
@@ -959,16 +1010,58 @@ class ShardedAntiCGE:
     _engine._run(self.device, lib.bz_anticge_scale, (self._blocks.data_ptr(), self.order.data_ptr(), partials.data_ptr(),
                                                      partials.numel(), p.n, self.f_decl, p.d, self.byz.data_ptr(), self._stream()))
     return [self.byz] * self.f_real
+  def __call__(self):
+    """ One step on the current stream of the rows' device; returns [byz] * f_real. """
+    with _engine._on(self.device):
+      self._issue()
+    return [self.byz] * self.f_real
+  def graph(self):
+    """ Capture a step in a CUDA graph (after one eager step, the warm-up) and return `replay`: a callable that
+    launches it and returns [byz] * f_real.  With "fused", each replay advances the exchange's epoch by two. """
+    _capturable(self.exchange, self.world, "ShardedAntiCGE")
+    if self._graph is None:
+      self()
+      with _engine._on(self.device):
+        torch.cuda.synchronize(self.device)
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph):
+          self._issue(captured=True)
+      self._graph = graph
+    graph, byz, count = self._graph, self.byz, self.f_real
+    fx, exchanges = (self._fx, self._exchanges) if self.exchange == "fused" else (None, 0)
+    def replay():
+      graph.replay()
+      if fx is not None:
+        fx.epoch += exchanges
+      return [byz] * count
+    return replay
+  def _issue(self, captured=False):
+    """ A step's calls; `captured`: the fused call takes its epoch from the buffer. """
+    lib = _lib.lib()
+    if self.exchange == "fused":
+      if captured:
+        _engine._call(lib.bz_anticge_peers_next, self._fused_head + self._fused_tail + (self._stream(),))
+        return
+      fx = self._fx
+      epoch = (fx.epoch + 1) % (1 << 32)
+      fx.epoch += self._exchanges
+      _engine._call(lib.bz_anticge_peers, self._fused_head + (epoch,) + self._fused_tail + (self._stream(),))
+      return
+    if self.f_real > self.f_decl:
+      p = self._prep
+      _engine._call(lib.bz_anticge, (p.ptrs, p.n, self.f_decl, self.f_real, p.d, self.byz.data_ptr(), self._ws.data_ptr(),
+                                     self._ws.numel(), self._stream()))
+      return
+    blocks = _gather(self.norms(), self.group)
+    self.scale(_gather(self.sum(blocks), self.group).reshape(-1))
 
-def anticge(grad_honests, f_decl, f_real, group=None):
+def anticge(grad_honests, f_decl, f_real, group=None, exchange="auto"):
   """ attacks/anticge.py's attack on a d-sharded trainer (see `ShardedAntiCGE`): every rank passes its columns of
-  the nh honest gradients and gets its shard of the attack row, f_real times, aliased.  Two all-gathers, of nh and
-  of one double per rank; no host read. """
+  the nh honest gradients and gets its shard of the attack row, f_real times, aliased.  "nccl": two all-gathers, of
+  nh and of one double per rank; "fused": one call that exchanges over peer memory; no host read. """
   if isinstance(f_real, int) and isinstance(f_decl, int) and f_real > f_decl:
     return _engine.anticge(grad_honests, f_decl, f_real)
-  attack = ShardedAntiCGE(grad_honests, f_decl, f_real)
-  blocks = _gather(attack.norms(), group)
-  return attack.scale(_gather(attack.sum(blocks), group).reshape(-1))
+  return ShardedAntiCGE(grad_honests, f_decl, f_real, group, exchange)()
 
 def aggregate(gar, gradients, f=None, m=None, mode="mid", group=None, backend=None, return_selection=False):
   """ Aggregate this rank's shard.

@@ -308,4 +308,8 @@ BZ_API int bz_gradient_row(const float* grad, int64_t d, double clip, float* sam
  * d-sharded path: bz_anticge, bz_anticge_partial, bz_anticge_scale. */
 #include "byzagg_anticge.h"
 
+/* The d-sharded attack against CGE with both of its exchanges over peer memory inside its kernels, and its _next
+ * twin for CUDA graphs: bz_anticge_peers, bz_anticge_peers_next. */
+#include "byzagg_anticge_peers.h"
+
 #endif /* BYZAGG_H */
