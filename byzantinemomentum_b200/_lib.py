@@ -2,9 +2,11 @@
 """ctypes binding of `libbyzagg.so` (C ABI: `include/byzagg.h`, `include/byzagg_shards.h`,
 `include/byzagg_attack.h`, `include/byzagg_search_shards.h`, `include/byzagg_search_peers.h`,
 `include/byzagg_coordinate.h`, `include/byzagg_peers_next.h`, `include/byzagg_distance.h`,
-`include/byzagg_distance_shards.h`, `include/byzagg_anticge.h` and `include/byzagg_anticge_peers.h`).
+`include/byzagg_distance_shards.h`, `include/byzagg_anticge.h` and `include/byzagg_anticge_peers.h`), and of the
+second library `libbyzagg_peers.so` built next to it (C ABI: `include/byzagg_distance_peers.h`), which the callers
+compose with the first through their C ABIs.
 
-The library is loaded lazily, on the first call that needs it, and the load FAILS LOUDLY:
+Each library is loaded lazily, on the first call that needs it, and the load FAILS LOUDLY:
 there is no CPU or PyTorch fallback anywhere in this package.  Build it in-tree with
 `python -c "import __graft_entry__ as g; g.build()"` or `make -C byzantinemomentum_b200/csrc`.
 """
@@ -14,7 +16,7 @@ import os
 import pathlib
 import threading
 
-__all__ = ["lib", "LibraryError", "library_path", "check", "MAX_N", "MAX_N_COORDINATE", "MAX_N_DISTANCE", "STATUS_MESSAGES",
+__all__ = ["lib", "peers_lib", "LibraryError", "library_path", "peers_library_path", "check", "MAX_N", "MAX_N_COORDINATE", "MAX_N_DISTANCE", "STATUS_MESSAGES",
            "AKSEL_MODES", "STATUS_NO_FINITE_SET", "STATUS_DEGENERATE"]
 
 MAX_N = 64
@@ -38,6 +40,13 @@ def library_path():
   if override:
     return pathlib.Path(override)
   return pathlib.Path(__file__).resolve().parent / "libbyzagg.so"
+
+def peers_library_path():
+  """ libbyzagg_peers.so: next to libbyzagg.so, or where BYZAGG_PEERS_LIBRARY says. """
+  override = os.environ.get("BYZAGG_PEERS_LIBRARY")
+  if override:
+    return pathlib.Path(override)
+  return library_path().parent / "libbyzagg_peers.so"
 
 _c_rows = ctypes.POINTER(ctypes.c_void_p)
 _vp, _i, _i64, _sz, _dbl = ctypes.c_void_p, ctypes.c_int, ctypes.c_int64, ctypes.c_size_t, ctypes.c_double
@@ -144,11 +153,37 @@ ANTICGE_PEER_SIGNATURES = {
   "bz_anticge_peers": (_i, [_c_rows, _i, _i, _i, _i64, _vp, _vp, _i, _i, _c_rows, _c_rows, ctypes.c_uint, _vp, _sz, _vp]),
   "bz_anticge_peers_next": (_i, [_c_rows, _i, _i, _i, _i64, _vp, _vp, _i, _i, _c_rows, _c_rows, _vp, _sz, _vp]),
 }
+# the same for include/byzagg_distance_peers.h, the table of the second library (`peers_lib()`): phase B of the d-sharded
+# distance rules above MAX_N rows with its exchange over peer memory
+DISTANCE_PEER_SIGNATURES = {
+  "bz_distance_peers_last_error": (ctypes.c_char_p, []),
+  "bz_distance_select_peers": (_i, [_i, _vp, _i, _i, _i, _i, _vp, _vp, _i, _i, _c_rows, _c_rows, ctypes.c_uint, _vp]),
+  "bz_distance_select_peers_next": (_i, [_i, _vp, _i, _i, _i, _i, _vp, _vp, _i, _i, _c_rows, _c_rows, _vp]),
+}
 SEARCH_STATE_BYTES = 64                     # BZ_SEARCH_STATE_BYTES
 CANDIDATE_FIRST, CANDIDATE_NEXT, CANDIDATE_FINAL = 0, 1, 2
 
 _lock = threading.Lock()
 _lib = None
+_peers_lib = None
+
+def _load(path, tables):
+  """ The library at `path` with the signatures of `tables` bound; LibraryError when it is missing or stale. """
+  if not path.exists():
+    raise LibraryError(f"{path} not found: build the CUDA extension first (python -c 'import __graft_entry__ as g; g.build()'); "
+                       "this package has no CPU fallback")
+  try:
+    handle = ctypes.CDLL(str(path))
+  except OSError as err:
+    raise LibraryError(f"unable to load {path}: {err}") from err
+  for name, (restype, argtypes) in [item for table in tables for item in table.items()]:
+    try:
+      fn = getattr(handle, name)
+    except AttributeError as err:
+      raise LibraryError(f"{path} does not export {name!r} (stale build?)") from err
+    fn.restype = restype
+    fn.argtypes = argtypes
+  return handle
 
 def lib():
   """ The loaded library (loads it on first use). """
@@ -157,32 +192,27 @@ def lib():
     return _lib
   with _lock:
     if _lib is None:
-      path = library_path()
-      if not path.exists():
-        raise LibraryError(f"{path} not found: build the CUDA extension first (python -c 'import __graft_entry__ as g; g.build()'); "
-                           "this package has no CPU fallback")
-      try:
-        handle = ctypes.CDLL(str(path))
-      except OSError as err:
-        raise LibraryError(f"unable to load {path}: {err}") from err
-      tables = (SIGNATURES, SHARD_SIGNATURES, ATTACK_SIGNATURES, SEARCH_SHARD_SIGNATURES, SEARCH_PEER_SIGNATURES,
-                COORDINATE_SIGNATURES, PEER_NEXT_SIGNATURES, DISTANCE_SIGNATURES, DISTANCE_SHARD_SIGNATURES, ANTICGE_SIGNATURES,
-                ANTICGE_PEER_SIGNATURES)
-      for name, (restype, argtypes) in [item for table in tables for item in table.items()]:
-        try:
-          fn = getattr(handle, name)
-        except AttributeError as err:
-          raise LibraryError(f"{path} does not export {name!r} (stale build?)") from err
-        fn.restype = restype
-        fn.argtypes = argtypes
-      _lib = handle
+      _lib = _load(library_path(), (SIGNATURES, SHARD_SIGNATURES, ATTACK_SIGNATURES, SEARCH_SHARD_SIGNATURES, SEARCH_PEER_SIGNATURES,
+                                    COORDINATE_SIGNATURES, PEER_NEXT_SIGNATURES, DISTANCE_SIGNATURES, DISTANCE_SHARD_SIGNATURES,
+                                    ANTICGE_SIGNATURES, ANTICGE_PEER_SIGNATURES))
   return _lib
+
+def peers_lib():
+  """ The second library, libbyzagg_peers.so (loads it on first use; no fallback when it is missing). """
+  global _peers_lib
+  if _peers_lib is not None:
+    return _peers_lib
+  with _lock:
+    if _peers_lib is None:
+      _peers_lib = _load(peers_library_path(), (DISTANCE_PEER_SIGNATURES,))
+  return _peers_lib
 
 def check(code, what):
   """ Raise on a non-zero return code of a bz_* call. """
   if code == 0:
     return
-  message = lib().bz_last_error()
+  # each library keeps the message of its own last failure
+  message = peers_lib().bz_distance_peers_last_error() if what in DISTANCE_PEER_SIGNATURES else lib().bz_last_error()
   message = message.decode("utf-8", "replace") if message else ""
   kinds = {-1: "invalid argument", -2: "unsupported", -3: "CUDA error", -4: "workspace"}
   error = ValueError if code in (-1, -2) else LibraryError

@@ -9,6 +9,7 @@
 
 #include "launch.cuh"
 #include "dist.cuh"
+#include "api_shared.cuh"
 
 namespace bz {
 

@@ -268,6 +268,17 @@ int launch_anticge_scale(float* out, int64_t d, const AntiCgeScale* scale, const
                          int nparts, int n, int maxpos, const int32_t* order, cudaStream_t st);
 // out[0, d) = NaN (0x7fc00000).
 int launch_nan_fill(float* out, int64_t d, cudaStream_t st);
+
+// ---- libbyzagg_peers.so: phase B above kMaxN rows with the exchange over peer memory (k5_select_peers.cu) ----------
+// One CTA: this rank's phase-A block `part` (n x n, entries i < j) copied into its slot, the exchange (`peers`),
+// the R blocks added in rank order, then launch_blocks_select_wide's steps; status: the rule's word, then
+// BZ_STATUS_PEER_TIMEOUT on a timeout.
+void launch_blocks_select_peers(const double* part, int n, int count, int32_t* order, int f, int m, int bulyan,
+                                const PeerTail& peers, cudaStream_t st);
+// The same from the n sums of Aksel (sqrt_norm = 0) or CGE, with launch_rowkeys_select_wide's steps; status: 0 or
+// BZ_STATUS_PEER_TIMEOUT.
+void launch_rowkeys_select_peers(const double* part, int n, int sqrt_norm, int32_t* order, const PeerTail& peers,
+                                 cudaStream_t st);
 // The d-sharded form over peer memory (bz_anticge_peers).  K2'-norms: K2' in CGE mode in bz_distance_partial's
 // geometry, its last CTA exchanging phase A's n sums (PeerTail), keeping their R-summed values in parts[0, n) and
 // writing the stable order of the keys (bz_distance_select's); `ticket`: one word, zeroed here, left zero.

@@ -7,24 +7,9 @@
 // rows take 128 KB instead of 256 KB of shared memory.
 // Phase B of the d-sharded path (bz_distance_select) runs the same steps from the ranks' gathered blocks
 // (k5_blocks_select_wide), and selects the rows of Aksel and CGE from their gathered sums (k5_rowkeys_select_wide).
-#include "k5_device.cuh"
+#include "k5_wide.cuh"
 
 namespace bz {
-
-constexpr int kK5WideThreads = 1024;
-
-// The steps after the n x n table `dist` of fp32 norms is filled: each row sorted into `sorted`, the rule's
-// compensated sums into `score`, the stable order, the status word.
-__device__ __forceinline__ void score_from_floats(const float* dist, float* sorted, double* score, int n, int count,
-                                                  int32_t* __restrict__ order, int32_t* __restrict__ status, int f, int m,
-                                                  int bulyan) {
-  __syncthreads();
-  sort_rows(dist, sorted, n);
-  for (int i = threadIdx.x; i < n; i += blockDim.x) score[i] = py_sum(sorted + i * n, count);
-  __syncthreads();
-  stable_order(score, n, order);
-  if (threadIdx.x == 0 && status != nullptr) *status = bulyan ? bulyan_status(score, n, f, m) : BZ_STATUS_OK;
-}
 
 __global__ void __launch_bounds__(kK5WideThreads)
 k5_score_select_wide(const __grid_constant__ PassTables t, int n, int count, int32_t* __restrict__ order,
@@ -82,21 +67,6 @@ k5_rowkeys_select_wide(const double* __restrict__ parts, int nparts, int n, int 
   __syncthreads();
   stable_order(key, n, order);
 }
-
-constexpr size_t kScoreWideSmemMax = (size_t)kMaxNDistance * sizeof(double) + 2 * (size_t)kMaxNDistance * kMaxNDistance * sizeof(float);
-
-template <class K>
-static void opt_in_wide(K kernel, unsigned long long& opted) {
-  int dev = 0;
-  cudaGetDevice(&dev);
-  const unsigned long long bit = 1ull << (dev & 63);
-  if (!(opted & bit)) {
-    cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kScoreWideSmemMax);
-    opted |= bit;
-  }
-}
-
-static size_t score_wide_smem(int n) { return (size_t)n * sizeof(double) + 2 * (size_t)n * n * sizeof(float); }
 
 void launch_select_wide(const PassTables& t, int n, int count, int32_t* order, int32_t* status, int f, int m, int bulyan,
                         cudaStream_t st) {

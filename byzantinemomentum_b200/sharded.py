@@ -31,7 +31,7 @@ import torch.distributed as dist
 from . import _lib
 from . import engine as _engine
 
-__all__ = ["aggregate", "aggregate_p2p", "compute_avg_dev_max", "study_step", "replicate", "apply_update", "shard_bounds", "rows_aligned", "choose_exchange", "rows_exchange", "choose_search_exchange", "PeerExchange", "FusedExchange", "ShardedPlan", "GradientShards", "choose_delivery", "ShardedLineSearch", "line_search", "choose_anticge_exchange", "ShardedAntiCGE", "anticge", "COORDINATE_WISE", "DISTANCE_BASED"]
+__all__ = ["aggregate", "aggregate_p2p", "compute_avg_dev_max", "study_step", "replicate", "apply_update", "shard_bounds", "rows_aligned", "choose_exchange", "rows_exchange", "plan_exchange", "choose_search_exchange", "PeerExchange", "FusedExchange", "ShardedPlan", "GradientShards", "choose_delivery", "ShardedLineSearch", "line_search", "choose_anticge_exchange", "ShardedAntiCGE", "anticge", "COORDINATE_WISE", "DISTANCE_BASED"]
 
 COORDINATE_WISE = ("average", "median", "trmean", "phocas", "meamed")
 DISTANCE_BASED = _engine.DISTANCE_BASED
@@ -105,6 +105,10 @@ class FusedExchange:
   attack's sum of squares) over the buffer of n = nh in one `bz_anticge_peers` call, advancing `epoch` by two
   (by none when f_real > f_decl: the NaN fill exchanges nothing).  It shares the buffer with a `ShardedPlan`
   or `ShardedLineSearch` of the same n on the same condition: one stream, the same order on every rank.
+  `ShardedPlan(exchange="fused")` of Aksel and CGE up to MAX_N rows runs its exchange in K2′'s last CTA
+  (`bz_rowdist_peers`); above MAX_N rows, for all four rules, in phase B's kernel (`bz_distance_select_peers`,
+  which copies the plan's staged phase-A block into the slot first): one exchange per call or replay either way,
+  on the same condition of sharing.
   `epoch` is the host's count of the exchanges issued so far; the flags hold the same count on the device
   (this rank's own entry [rank] of its flag array, in the slot of its last epoch).  The eager calls pass
   `epoch` by value.  A captured call (`ShardedPlan.graph()`, `ShardedLineSearch.graph()`) cannot: its
@@ -237,6 +241,24 @@ def rows_exchange(exchange, n):
   raise ValueError(f"the {exchange} exchange serves at most MAX_N = {_lib.MAX_N} rows, not n = {n}: "
                    f"above, ShardedPlan exchanges through \"nccl\"")
 
+def plan_exchange(gar, n, exchange, aligned, symmetric, group=None):
+  """ The exchange of a `ShardedPlan` of n rows, the same on every rank of `group`.  "auto", "nccl" and "p2p"
+  resolve as `rows_exchange` then `choose_exchange` do.  An explicit "fused" is served wherever the rule's exchange
+  can run inside a kernel: krum and bulyan up to MAX_N rows keep `choose_exchange`'s rule (the distance ring's
+  exchange, 16-byte aligned rows); aksel and cge at every n (`bz_rowdist_peers` up to MAX_N rows), and krum and
+  bulyan above MAX_N rows, take rows of any alignment (above MAX_N rows, `bz_distance_select_peers` after phase A).
+  Those need symmetric memory on every one of at most MAX_PEERS ranks, agreed on with one all-reduce (MIN), or a
+  single rank.  A request some rank cannot serve raises on every rank.  Returns "fused",
+  "p2p" or "nccl". """
+  if exchange != "fused" or gar not in _engine.WIDE_DISTANCE or (gar in ("krum", "bulyan") and n <= _lib.MAX_N):
+    return choose_exchange(gar, rows_exchange(exchange, n), aligned, symmetric, group)
+  world = dist.get_world_size(group) if dist.is_initialized() else 1
+  (symmetric,) = map(bool, _agree([int(bool(symmetric))], group))
+  if not (world == 1 or (symmetric and world <= _lib.MAX_PEERS)):
+    raise ValueError(f"the fused exchange of {gar} on {n} rows needs symmetric memory on every one of at most "
+                     f"{_lib.MAX_PEERS} ranks")
+  return "fused"
+
 def _phases(be, gar, gradients, f, m, mode, group, p2p):
   """ (this rank's shard of the result, the selection) of a distance-based rule.  Phase A computes
   this rank's partial block; the R blocks are all-gathered into [R, ...] in rank order, or (`p2p`)
@@ -285,21 +307,28 @@ class ShardedPlan:
             "p2p"   the block is written straight into this rank's slot of a SYMMETRIC buffer, one
                     device-side barrier, and the selection kernel reads the R blocks in place from
                     the R peers over NVLink (`bz_*_select_peers`): gather + scoring in one kernel;
-            "fused" (krum, bulyan) the exchange runs INSIDE the distance pass: its last CTA publishes the
-                    block in the symmetric buffer, flags the peers, waits for theirs and scores — a step
-                    is the single-GPU rule's two launches, nothing else (`bz_krum_peers`);
-            "auto"  "fused" where it applies on every rank, else "p2p", when every rank of the group
-                    has symmetric memory; else "nccl".  The ranks agree on the choice
-                    (`choose_exchange`); a failing symmetric-memory setup raises.
-  Both exchanges use the same fixed summation order: bitwise identical selections on every rank.
+            "fused" the exchange runs inside a kernel, over the symmetric buffer of `fused_exchange(n, ...)`
+                    (which needs an initialised process group, or a buffer registered for it), one exchange
+                    per call: krum and bulyan up to MAX_N rows in the distance pass, whose last CTA
+                    publishes the block, flags the peers, waits for theirs and scores — a step is the single-GPU rule's two launches (`bz_krum_peers`,
+                    16-byte aligned rows); aksel and cge up to MAX_N rows in K2′'s last CTA
+                    (`bz_rowdist_peers`: [median], one call); the four rules above MAX_N rows in phase B
+                    (`bz_distance_partial` into a staging buffer, `bz_distance_select_peers` of the second
+                    library, `bz_distance_reduce`).  Rows of any alignment except for krum / bulyan up to
+                    MAX_N rows;
+            "auto"  "fused" where it applies on every rank (krum and bulyan up to MAX_N rows), else "p2p",
+                    when every rank of the group has symmetric memory; else "nccl".  The ranks agree on
+                    the choice (`plan_exchange`); a failing symmetric-memory setup raises.
+  Every exchange uses the same fixed summation order: bitwise identical selections on every rank, and the
+  fused exchange gives "nccl"'s bits.  `status` is always present with "fused" (0, or a peer that did not show up).
   Coordinate-wise rules need no exchange and simply wrap `engine.Plan`.
   Rows: up to MAX_N_DISTANCE for krum, bulyan, aksel and cge, MAX_N for brute.  Above MAX_N the exchange is
-  "nccl" (`rows_exchange`: "auto" resolves to it, "p2p" and "fused" raise), whose phases are
+  "nccl" or an explicit "fused" (`plan_exchange`: "auto" resolves to "nccl", "p2p" raises); "nccl"'s phases are
   `bz_distance_partial`, `bz_distance_select` and `bz_distance_reduce` at every n: the n x n block of 128 rows
   is 131 KB per rank.  One rank gives `engine.Plan`'s output, selection and status bit for bit.
 
   `graph()` captures a step in a CUDA graph, as `engine.Plan.graph()` does: "fused" on any number of ranks
-  (the captured kernel takes its epoch from the exchange buffer, `bz_*_peers_next`), any exchange on one
+  (the captured kernel takes its epoch from the exchange buffer, the `_next` calls), any exchange on one
   rank; a coordinate-wise plan returns `engine.Plan.graph()`.  Like a call, `graph()` and every replay are
   collective: every rank issues them at the same point of its stream order. """
   def __init__(self, gar, gradients, f=None, m=None, mode="mid", group=None, exchange="auto"):
@@ -317,7 +346,8 @@ class ShardedPlan:
       return
     rule = _engine._rule(gar, n, f, m, mode)
     self._local = None
-    exchange = rows_exchange(exchange, n)
+    if exchange not in EXCHANGES:
+      raise ValueError(f"unknown exchange {exchange!r}")
     limit = _lib.MAX_N_DISTANCE if gar in _engine.WIDE_DISTANCE else _lib.MAX_N
     prep = _engine._prepare_device(self.rows, limit=limit)
     if not all(g.is_contiguous() for g in self.rows):
@@ -335,20 +365,29 @@ class ShardedPlan:
     self.selection = self._meta[:rule.length]
     if rule.status:
       self.status = self._meta[n:]
-    exchange = self.exchange = choose_exchange(gar, exchange, rows_aligned(self.rows), _symmetric_memory_importable(), group)
-    if exchange == "fused":
+    facts = (rows_aligned(self.rows), _symmetric_memory_importable(), group)
+    if exchange == "fused" and not (dist.is_initialized() or (n, device.index, id(group)) in _fused):
+      # no process group to set the fused buffer up over and none registered (`fused_exchange`): resolved as before
+      exchange = self.exchange = choose_exchange(gar, rows_exchange(exchange, n), *facts)
+    else:
+      exchange = self.exchange = plan_exchange(gar, n, exchange, *facts)
+    if exchange == "fused" and rule.pair and n <= _lib.MAX_N:
       fx = self._fx = fused_exchange(n, device, group)
       self.status = self._meta[n:]                          # krum too: a peer that never signals
       self._fused_fn = getattr(_lib.lib(), f"bz_{gar}_peers")
-      self._fused_tables = [fx.tables(0), fx.tables(1)]
-      self._next_fn, self._next_tables = getattr(_lib.lib(), f"bz_{gar}_peers_next"), fx.both()
+      self._next_fn = getattr(_lib.lib(), f"bz_{gar}_peers_next")
       self._fused_head = (prep.ptrs, n) + rule.params + (prep.d, out, meta, status, fx.rank, fx.world)
       self._fused_tail = (ws.data_ptr(), ws.numel(), prep.stream)
+      self._fused_around = ([], [])
+      self._fused_tables, self._next_tables = [fx.tables(0), fx.tables(1)], fx.both()
       return
     # aksel: the coordinate-wise median of the local shard is the center of phase A
     self._median = _engine.Plan("median", self.rows) if rule.center else None
     center = None if self._median is None else self._median.out.data_ptr()
     width = n * n if rule.pair else n
+    if exchange == "fused":
+      self._fuse(rule, prep, center, ws, out, meta, status)
+      return
     if exchange == "p2p":
       def phases(part, blocks):
         return _engine._partial_call(prep, rule.pair, center, part, ws), _engine._select_call(rule, blocks, meta, prep.stream)
@@ -363,6 +402,30 @@ class ShardedPlan:
       a, b, self._c = rule.phase_entries(prep.ptrs, prep.d, center, self._part.data_ptr(), self._gathered.data_ptr(),
                                          self.world, out, meta, ws, prep.stream)
       self._ab = [(a, b)]
+  def _fuse(self, rule, prep, center, ws, out, meta, status):
+    """ The fused exchange of Aksel and CGE up to MAX_N rows (`bz_rowdist_peers`: phase A, the exchange, the
+    selection and the reduce in its kernels), and of the four rules above (`bz_distance_partial` into a staging
+    buffer, `bz_distance_select_peers` of the second library, `bz_distance_reduce`). """
+    n, device, gar = self.n, self.device, self.gar
+    fx = self._fx = fused_exchange(n, device, self.group)
+    self.status = self._meta[n:]
+    code, (m, mode) = _engine._SEARCH_RULES[gar], rule._m_mode()
+    before = [(self._median._fn, self._median._args)] if self._median is not None else []
+    if n <= _lib.MAX_N:
+      lib = _lib.lib()
+      self._fused_fn, self._next_fn = lib.bz_rowdist_peers, lib.bz_rowdist_peers_next
+      self._fused_head = (code, prep.ptrs, n, rule.f, mode, center, prep.d, out, meta, status, fx.rank, fx.world)
+      self._fused_tail = (ws.data_ptr(), ws.numel(), prep.stream)
+      self._fused_around = (before, [])
+    else:
+      peers = _lib.peers_lib()
+      self._part = torch.empty(n * n if rule.pair else n, dtype=torch.float64, device=device)
+      a, _, c = rule.phase_entries(prep.ptrs, prep.d, center, self._part.data_ptr(), None, 1, out, meta, ws, prep.stream)
+      self._fused_fn, self._next_fn = peers.bz_distance_select_peers, peers.bz_distance_select_peers_next
+      self._fused_head = (code, self._part.data_ptr(), n, rule.f, m, mode, meta, status, fx.rank, fx.world)
+      self._fused_tail = (prep.stream,)
+      self._fused_around = (before + [a], [c])
+    self._fused_tables, self._next_tables = [fx.tables(0), fx.tables(1)], fx.both()
   def __call__(self):
     if self._local is not None:
       return self._local()
@@ -388,12 +451,17 @@ class ShardedPlan:
   def _issue(self, call, captured=False):
     """ One step's calls through `call(fn, args)`; `captured`: the fused exchange takes its epoch from the buffer. """
     if self.exchange == "fused":
+      before, after = self._fused_around
+      for step in before:
+        call(*step)
       if captured:
         call(self._next_fn, self._fused_head + self._next_tables + self._fused_tail)
-        return
-      fx = self._fx
-      fx.epoch += 1
-      call(self._fused_fn, self._fused_head + self._fused_tables[fx.epoch % 2] + (fx.epoch,) + self._fused_tail)
+      else:
+        fx = self._fx
+        fx.epoch += 1
+        call(self._fused_fn, self._fused_head + self._fused_tables[fx.epoch % 2] + (fx.epoch,) + self._fused_tail)
+      for step in after:
+        call(*step)
       return
     if self._median is not None:
       call(self._median._fn, self._median._args)
