@@ -11,14 +11,15 @@ called from `attack.py:821-822`): same plugin interface, hand-written CUDA under
 
     import aggregators                              # the unmodified reference
     byzantinemomentum_b200.plugin.install(aggregators)   # registers "b200-<name>" rules
+    # or install(aggregators, wide=True): krum, bulyan, aksel and cge then take up to 128 rows
 
 Importing this package never touches CUDA; the compiled library is loaded on first use and
 its absence is an error (no CPU fallback).
 """
 
 from . import _lib, engine, gars as _gars, hostmem, plugin, sharded
-from .gars import gars, make_gar, register, UserException, last_selection
+from .gars import gars, wide_gars, make_gar, register, UserException, last_selection
 from .engine import config, Plan, compute_avg_dev_max, GradientStack
 
-__all__ = ["gars", "make_gar", "register", "UserException", "last_selection", "config", "Plan", "GradientStack", "compute_avg_dev_max", "engine", "hostmem", "plugin", "sharded"]
+__all__ = ["gars", "wide_gars", "make_gar", "register", "UserException", "last_selection", "config", "Plan", "GradientStack", "compute_avg_dev_max", "engine", "hostmem", "plugin", "sharded"]
 __version__ = "0.1.0"

@@ -2,7 +2,8 @@
 """ctypes binding of `libbyzagg.so` (C ABI: `include/byzagg.h`, `include/byzagg_shards.h`,
 `include/byzagg_attack.h`, `include/byzagg_search_shards.h`, `include/byzagg_search_peers.h`,
 `include/byzagg_coordinate.h`, `include/byzagg_peers_next.h`, `include/byzagg_distance.h`,
-`include/byzagg_distance_shards.h`, `include/byzagg_anticge.h` and `include/byzagg_anticge_peers.h`), and of the
+`include/byzagg_distance_shards.h`, `include/byzagg_anticge.h`, `include/byzagg_anticge_peers.h` and
+`include/byzagg_distance_search.h`), and of the
 second library `libbyzagg_peers.so` built next to it (C ABI: `include/byzagg_distance_peers.h`), which the callers
 compose with the first through their C ABIs.
 
@@ -153,6 +154,12 @@ ANTICGE_PEER_SIGNATURES = {
   "bz_anticge_peers": (_i, [_c_rows, _i, _i, _i, _i64, _vp, _vp, _i, _i, _c_rows, _c_rows, ctypes.c_uint, _vp, _sz, _vp]),
   "bz_anticge_peers_next": (_i, [_c_rows, _i, _i, _i, _i64, _vp, _vp, _i, _i, _c_rows, _c_rows, _vp, _sz, _vp]),
 }
+# the same for include/byzagg_distance_search.h (the line search against Multi-Krum, Bulyan, Aksel and CGE up to
+# MAX_N_DISTANCE rows)
+DISTANCE_SEARCH_SIGNATURES = {
+  "bz_distance_line_search_workspace_bytes": (_sz, [_i]),
+  "bz_distance_line_search": (_i, [_i, _c_rows, _i, _i, _i, _i, _i, _vp, _vp, _i64, _i, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+}
 # the same for include/byzagg_distance_peers.h, the table of the second library (`peers_lib()`): phase B of the d-sharded
 # distance rules above MAX_N rows with its exchange over peer memory
 DISTANCE_PEER_SIGNATURES = {
@@ -194,7 +201,7 @@ def lib():
     if _lib is None:
       _lib = _load(library_path(), (SIGNATURES, SHARD_SIGNATURES, ATTACK_SIGNATURES, SEARCH_SHARD_SIGNATURES, SEARCH_PEER_SIGNATURES,
                                     COORDINATE_SIGNATURES, PEER_NEXT_SIGNATURES, DISTANCE_SIGNATURES, DISTANCE_SHARD_SIGNATURES,
-                                    ANTICGE_SIGNATURES, ANTICGE_PEER_SIGNATURES))
+                                    ANTICGE_SIGNATURES, ANTICGE_PEER_SIGNATURES, DISTANCE_SEARCH_SIGNATURES))
   return _lib
 
 def peers_lib():

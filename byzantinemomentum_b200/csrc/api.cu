@@ -325,3 +325,4 @@ int bz_coordinate(int rule, const float* const* rows, int n, int f, int64_t d, f
 #include "api_distance_shards.inc"
 #include "api_anticge.inc"
 #include "api_anticge_peers.inc"
+#include "api_distance_search.inc"

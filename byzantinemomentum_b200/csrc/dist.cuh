@@ -68,8 +68,12 @@ struct SelectTail {
   double* const* peer_blocks;
   unsigned* const* peer_flags;
 };
+// star_row >= 0 (no `select`): a star pass without a tail, in the full pass's shape, grid and cluster size: only the
+// pairs of row star_row (and the self distances of `self_rows`) are written to the per-cluster blocks, with the bits
+// the full pass gives them; every other entry of the blocks is left as it was.  -1 where the star pass cannot run
+// (the caller then runs the full pass).
 int launch_pairdist_ring(const RowTable& rows, int n, int64_t d, double* parts, cudaStream_t st,
-                         const unsigned char* self_rows, int nself, SelectTail* select = nullptr);
+                         const unsigned char* self_rows, int nself, SelectTail* select = nullptr, int star_row = -1);
 // Dispatcher used by the rules: `rows` are the u unique rows, `to_unique` (or NULL) maps the n_orig
 // original rows to them; the self distance is produced for the unique rows that are aliased.
 // Runs the ring, or the cp.async kernel of k2_pairdist.cu when the ring returns -1.

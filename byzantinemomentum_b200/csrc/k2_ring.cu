@@ -784,7 +784,7 @@ static int launch_ring(int shape, const RowTable& rows, const SelfList& self, co
 // Returns the number of partial blocks written, or -1 when the rows are not 16-byte aligned or the
 // launch fails (the caller falls back to k2_pairdist).  `self_rows`: unique rows whose self distance K5 reads.
 int launch_pairdist_ring(const RowTable& rows, int n, int64_t d, double* parts, cudaStream_t st,
-                         const unsigned char* self_rows, int nself, SelectTail* select) {
+                         const unsigned char* self_rows, int nself, SelectTail* select, int star_row) {
   int shape, C;
   if (!ring_shape(n, shape, C)) return -1;
   const int W = kShapes[shape].W;
@@ -848,6 +848,14 @@ int launch_pairdist_ring(const RowTable& rows, int n, int64_t d, double* parts, 
         for (int k = 0; k < kMaxN; ++k) tail.old_index[k] = -1;
       }
     }
+  }
+  if (star_row >= 0) {
+    // the star pass of bz_distance_line_search: one fresh row, its slots picked as above
+    const int slots = (n + 2) / 3 > W * C ? kRSlots : 3;
+    if (select != nullptr || star_row >= n || n < 2 || (n + slots - 1) / slots > W * C) return -1;
+    star.count = 1;
+    star.slots = slots;
+    star.row[0] = (unsigned char)star_row;
   }
   const int nparts = nself > 0 ? launch_ring<true>(shape, rows, self, tail, star, n, C, d, parts, st)
                                : launch_ring<false>(shape, rows, self, tail, star, n, C, d, parts, st);

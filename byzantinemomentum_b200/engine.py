@@ -26,7 +26,7 @@ __all__ = ["average", "median", "trmean", "phocas", "meamed", "krum", "bulyan", 
            "pairdist_partial", "rowdist_partial", "select", "krum_select", "bulyan_select", "brute_select",
            "rowdist_select", "average_selected", "bulyan_reduce", "avg_dev_max_async", "compute_avg_dev_max", "rowdots_async", "study_step",
            "StudyPartials", "study_partials", "study_finish",
-           "LineSearch", "line_search", "AntiCGE", "anticge", "config", "Plan", "pair_cache_stats", "GradientStack", "gradient_scatter", "momentum_rows", "host_path_report"]
+           "wide_distance", "LineSearch", "line_search", "AntiCGE", "anticge", "config", "Plan", "pair_cache_stats", "GradientStack", "gradient_scatter", "momentum_rows", "host_path_report"]
 
 class _Config:
   """ strict_status: after brute / bulyan, read the device status word (one 4-byte D2H copy,
@@ -50,22 +50,26 @@ class _Prepared:
   __slots__ = ("rows", "n", "d", "device", "ptrs", "stream", "to_cpu", "keep", "host_mode", "host_t0")
 
 _workspaces = {}
+_wide_workspaces = {}
 _staging = {}
 
 _MAX_WORKSPACES = 16
 
-def _workspace(device, stream):
-  """ One scratch buffer per (device, stream), sized for MAX_N (~10 MB).  At most
-  `_MAX_WORKSPACES` are kept (least recently used dropped; the caching allocator keeps a dropped
-  buffer alive until the launches already queued on its stream have run). """
+def _workspace(device, stream, wide=False):
+  """ One scratch buffer per (device, stream), sized for MAX_N (~10 MB), or with `wide` for `bz_distance` up to
+  MAX_N_DISTANCE rows (~11 MB, kept apart).  At most `_MAX_WORKSPACES` of each are kept (least recently used
+  dropped; the caching allocator keeps a dropped buffer alive until the launches already queued on its stream
+  have run). """
+  cache = _wide_workspaces if wide else _workspaces
   key = (device.index, stream)
-  ws = _workspaces.pop(key, None)
+  ws = cache.pop(key, None)
   if ws is None:
-    nbytes = int(_lib.lib().bz_workspace_bytes(_lib.MAX_N))
+    lib = _lib.lib()
+    nbytes = int(lib.bz_distance_workspace_bytes(_lib.MAX_N_DISTANCE) if wide else lib.bz_workspace_bytes(_lib.MAX_N))
     ws = torch.empty(nbytes, dtype=torch.uint8, device=device)
-    while len(_workspaces) >= _MAX_WORKSPACES:
-      _workspaces.pop(next(iter(_workspaces)))
-  _workspaces[key] = ws          # most recently used last
+    while len(cache) >= _MAX_WORKSPACES:
+      cache.pop(next(iter(cache)))
+  cache[key] = ws          # most recently used last
   return ws
 
 def _row_buffer(rows, d, device):
@@ -558,6 +562,25 @@ def _distance(gar, gradients, f, m=None, mode="mid"):
     _raise_status(int(meta[prep.n].item()))
   return _finish(prep, out), meta[:rule.length]
 
+def wide_distance(gar, gradients, f, m=None, mode="mid"):
+  """ `_distance` for krum, bulyan, aksel and cge over 1 to MAX_N_DISTANCE rows: up to MAX_N exactly `_distance`
+  (the distance cache included), above it `bz_distance` with a per-(device, stream) workspace.  Above MAX_N no
+  distance is reused from one call to the next.  Host rows are staged as `_distance` stages them. """
+  if gar not in WIDE_DISTANCE:
+    raise KeyError(f"{gar!r} is not one of {WIDE_DISTANCE}")
+  n = len(gradients) if isinstance(gradients, (list, tuple)) else 0
+  if n <= _lib.MAX_N:
+    return _distance(gar, gradients, f, m, mode)
+  rule = _rule(gar, n, f, m, mode)
+  prep = _prepare(gradients, limit=_lib.MAX_N_DISTANCE)
+  out = torch.empty(prep.d, dtype=torch.float32, device=prep.device)
+  ws = _workspace(prep.device, prep.stream, wide=True)
+  meta = torch.empty(prep.n + 1, dtype=torch.int32, device=prep.device)   # order[n] + status
+  _run(prep.device, *rule.wide_entry(prep.ptrs, prep.d, out.data_ptr(), meta.data_ptr(), ws, prep.stream))
+  if rule.status and config.strict_status:
+    _raise_status(int(meta[prep.n].item()))
+  return _finish(prep, out), meta[:rule.length]
+
 def krum(gradients, f, m=None):
   return _distance("krum", gradients, f, m)
 
@@ -580,16 +603,19 @@ _SEARCH_RULES = dict(_RULE_CODES, krum=5, bulyan=6, brute=7, aksel=8, cge=9)    
 _SEARCH_KINDS = {"identical": 0, "empire-strict": 1}                             # BZ_ATTACK_*
 
 def search_max_rows(gar):
-  """ The most rows (honest + f_real) the line search takes against the rule `gar`: MAX_N_COORDINATE for
-  the coordinate-wise rules, MAX_N for the distance rules (`bz_line_search`'s limits).  `LineSearch`,
-  `sharded.ShardedLineSearch` and `plugin.install_attacks` all ask here. """
+  """ The most rows (honest + f_real) `bz_line_search` takes against the rule `gar`: MAX_N_COORDINATE for
+  the coordinate-wise rules, MAX_N for the distance rules.  It is the limit of `sharded.ShardedLineSearch`
+  and of the attacks `plugin.install_attacks` routes to a default `plugin.install` entry.  `LineSearch` takes
+  krum, bulyan, aksel and cge further, up to MAX_N_DISTANCE rows (`bz_distance_line_search`). """
   return _lib.MAX_N_COORDINATE if gar in _RULE_CODES else _lib.MAX_N
 
 class LineSearch:
   """ A prepared `bz_line_search`: `line_maximize(eval_factor, evals)` of the identical-family attacks
   (kind "identical": candidate `grad_avg + s * grad_att`, s = -x when `negative`) or of empire-strict
   (kind "empire-strict": `grad_avg.mul(-x)`) against the rule `gar` with its defaults and f = f_decl,
-  every evaluation, score and next factor computed on the device.  Like `Plan`, `search()` only issues
+  every evaluation, score and next factor computed on the device.  Against krum, bulyan, aksel and cge it takes
+  up to MAX_N_DISTANCE rows (honest + f_real): above MAX_N through `bz_distance_line_search`, with a workspace
+  of its own, as `Plan` does.  Like `Plan`, `search()` only issues
   the call (no allocation, no synchronisation; `graph()` captures it) and holds what it reads and writes:
       byz     the candidate row; after the call the attack's Byzantine gradient for the chosen factor
       record  fp64 [2 * evals + 2]: (x_k, y_k) per evaluation, the chosen factor, then the status word
@@ -600,7 +626,7 @@ class LineSearch:
     if kind not in _SEARCH_KINDS:
       raise ValueError(f"unknown attack kind {kind!r}, expected one of {sorted(_SEARCH_KINDS)}")
     honest = list(grad_honests)
-    limit = search_max_rows(gar)
+    limit = _lib.MAX_N_DISTANCE if gar in WIDE_DISTANCE else search_max_rows(gar)
     prep = _prepare(honest, limit=limit)
     if prep.to_cpu:
       raise ValueError("the line search takes CUDA tensors")
@@ -615,9 +641,12 @@ class LineSearch:
     self._out = torch.empty(prep.d, dtype=torch.float32, device=prep.device)
     self.record = torch.empty(2 * max(self.evals, 0) + 2, dtype=torch.float64, device=prep.device)
     n = prep.n + int(f_real)
-    self._ws = torch.empty(int(_lib.lib().bz_line_search_workspace_bytes(min(max(n, 1), limit))), dtype=torch.uint8, device=prep.device)
+    if n > _lib.MAX_N and gar in WIDE_DISTANCE:
+      self._fn, ws_bytes = _lib.lib().bz_distance_line_search, _lib.lib().bz_distance_line_search_workspace_bytes
+    else:
+      self._fn, ws_bytes = _lib.lib().bz_line_search, _lib.lib().bz_line_search_workspace_bytes
+    self._ws = torch.empty(int(ws_bytes(min(max(n, 1), limit))), dtype=torch.uint8, device=prep.device)
     status = self.record.data_ptr() + 8 * (self.record.numel() - 1)
-    self._fn = _lib.lib().bz_line_search
     self._args = (_SEARCH_RULES[gar], prep.ptrs, prep.n, int(f_real), int(f_decl), _SEARCH_KINDS[kind], int(bool(negative)),
                   grad_avg.data_ptr(), None if grad_att is None else grad_att.data_ptr(), prep.d, self.evals,
                   self.byz.data_ptr(), self._out.data_ptr(), self.record.data_ptr(), status,

@@ -6,6 +6,9 @@ callable taking keyword arguments only (`gradients`, `f`, `model`, plus rule spe
 unknown keywords are accepted and ignored), returning a NEW tensor, and carrying the members
 `check`, `checked`, `unchecked`, `upper_bound`, `influence`.  `gars` maps the reference's
 names (average, median, trmean, phocas, meamed, krum, bulyan, brute, aksel, cge) to them.
+`wide_gars` holds krum, bulyan, aksel and cge again, built the same way, for 1 to 128 gradients
+(`BZ_MAX_N_DISTANCE`): up to 64 they make exactly the call of their `gars` entry, above it they run
+`bz_distance`.  `plugin.install(..., wide=True)` registers them.
 The arithmetic runs in `libbyzagg.so` (see `engine.py`); this module only holds the
 argument checks, the closed-form bounds and the selection bookkeeping for `influence`.
 
@@ -14,16 +17,17 @@ Differences with the reference, all deliberate:
     reuses the selection computed on the device instead of recomputing all distances
     (attack.py:822 always follows attack.py:821);
   * the coordinate-wise rules (average, median, trmean, phocas, meamed) take up to 128 gradients
-    (`BZ_MAX_N_COORDINATE`); with more than 64 gradients the distance-based rules raise
-    (`BZ_MAX_N`), with a message saying so.
+    (`BZ_MAX_N_COORDINATE`); with more than 64 gradients the distance-based rules of `gars` raise
+    (`BZ_MAX_N`), with a message saying so, and those of `wide_gars` take up to 128.  Above 64
+    gradients a `wide_gars` call reuses no distance of the previous call.
 """
 
 import math
 
-from . import engine
+from . import _lib, engine
 from .engine import _Memo as _Selection, _rule
 
-__all__ = ["gars", "make_gar", "register", "UserException", "last_selection"]
+__all__ = ["gars", "wide_gars", "make_gar", "register", "UserException", "last_selection"]
 
 class UserException(RuntimeError):
   """ Raised by `checked` on invalid parameters (the reference raises tools.UserException). """
@@ -238,3 +242,30 @@ def _cge_influence(honests, attacks, f, **kwargs):
   return _accepted_ratio(order, len(honests), len(gradients) - f)
 
 register("cge", _cge, _cge_check, influence=_cge_influence)
+
+# ---------------------------------------------------------------------------- #
+# Multi-Krum, Bulyan, Aksel and CGE for up to 128 gradients
+
+def _wide(name):
+  """ The `wide_gars` entry of `name`: the check, bound and influence of `gars[name]`; up to MAX_N gradients its
+  call, above it `engine.wide_distance` (`bz_distance`), which stores the selection for `influence` as it does. """
+  narrow = gars[name]
+  def unchecked(gradients, f, m=None, mode="mid", **kwargs):
+    if not isinstance(gradients, list) or len(gradients) <= _lib.MAX_N:
+      return narrow.unchecked(gradients=gradients, f=f, m=m, mode=mode, **kwargs)
+    out, order = engine.wide_distance(name, gradients, f, m if name in ("krum", "bulyan") else None,
+                                      mode if name == "aksel" else "mid")
+    if name != "bulyan":
+      _last.store(name, (f,) if name == "krum" else (), gradients, order)
+    return out
+  unchecked.__name__ = narrow.unchecked.__name__
+  influence = None
+  if narrow.influence is not None:
+    def influence(honests, attacks, f, m=None, mode="mid", **kwargs):
+      gradients = honests + attacks
+      if len(gradients) > _lib.MAX_N and _last.lookup(name, (f,) if name == "krum" else (), gradients) is None:
+        unchecked(gradients=gradients, f=f, m=m, mode=mode)
+      return narrow.influence(honests, attacks, f=f, m=m, mode=mode, **kwargs)
+  return make_gar(unchecked, narrow.check, upper_bound=narrow.upper_bound, influence=influence, name=name)
+
+wide_gars = {name: _wide(name) for name in engine.WIDE_DISTANCE}

@@ -8,55 +8,65 @@ routes lead there without touching a reference file:
      check, upper_bound, influence)` (aggregators/__init__.py:71-86) for every rule, under
      `<prefix><name>` (default prefix "b200-"), or replaces the stock entries in place with
      `override=True` (`register` refuses duplicates, :82-84, so the entry is rebuilt with the
-     reference's `make_gar`).
+     reference's `make_gar`).  With `wide=True` it registers krum, bulyan, aksel and cge from
+     `gars.wide_gars`, which take up to 128 gradients instead of 64.
   2. the top-level `native` package of this repository: the reference already looks for
      `native.{median,krum,bulyan,brute}.aggregate` and registers `native-<name>` when it finds
      them (median.py:80-87, krum.py:159-166, bulyan.py:137-144, brute.py:149-156).
 
 `install_attacks(attacks)` then lets the line-searching attacks run their whole search on the device
 (`engine.line_search`) when the rule they attack is one `install` registered, and, asked for by name, the
-attack against CGE run on the device (`engine.anticge`).
+attack against CGE run on the device (`engine.anticge`).  The search takes the rows the entry takes: up to
+128 against a wide entry, and against a default entry as many as `bz_line_search` takes
+(`engine.search_max_rows`).
 """
 
 import math
 
-from .gars import gars
+from .gars import gars, wide_gars
 
 __all__ = ["install", "install_tools", "install_attacks"]
 
-# The reference registry's entries that `install` made, each mapped to the name of its rule here: the
-# attacks replaced by `install_attacks` recognise the rule they attack by identity.
+# The reference registry's entries that `install` made, each mapped to the name of its rule here and the most
+# rows the device search takes against it: the attacks replaced by `install_attacks` recognise the rule they
+# attack by identity.
 _installed = {}
 
-def _record(aggregators, key, name):
+def _record(aggregators, key, name, rule):
+  from . import engine, _lib
   entry = aggregators.gars.get(key)
-  if entry is not None and getattr(entry, "unchecked", None) is gars[name].unchecked:
-    _installed[entry] = name
+  if entry is not None and getattr(entry, "unchecked", None) is rule.unchecked:
+    wide = wide_gars.get(name) is rule
+    _installed[entry] = (name, _lib.MAX_N_DISTANCE if wide else engine.search_max_rows(name))
 
-def install(aggregators, prefix="b200-", override=False, names=None):
+def install(aggregators, prefix="b200-", override=False, names=None, wide=False):
   """ Register the CUDA rules in the reference's `aggregators` module.
   Args:
     aggregators  The imported reference package (duck-typed: needs `gars`, `register`, `make_gar`)
     prefix       Name prefix of the new entries (ignored with override)
     override     Replace the stock rules under their own names instead
     names        Iterable of rule names to install (default: all)
+    wide         Register krum, bulyan, aksel and cge from `gars.wide_gars`: up to 128 gradients, and the
+                 attacks' device search against them up to 128 rows.  The default, False, keeps `gars`' entries,
+                 which stop at 64 gradients, as every earlier release did; the other six rules are the same
+                 either way
   Returns:
     List of the registered names
   """
   done = []
   for name in (names or gars.keys()):
-    rule = gars[name]
+    rule = wide_gars[name] if wide and name in wide_gars else gars[name]
     if override:
       wrapped = aggregators.make_gar(rule.unchecked, rule.check, upper_bound=rule.upper_bound, influence=rule.influence)
       aggregators.gars[name] = wrapped
       setattr(aggregators, name, wrapped)
-      _record(aggregators, name, name)
+      _record(aggregators, name, name, rule)
       done.append(name)
     else:
       target = prefix + name
       if target not in aggregators.gars:
         aggregators.register(target, rule.unchecked, rule.check, upper_bound=rule.upper_bound, influence=rule.influence)
-      _record(aggregators, target, name)
+      _record(aggregators, target, name, rule)
       done.append(target)
   return done
 
@@ -88,19 +98,19 @@ def _is_cuda(tensors):
 def _device_rule(defense, grad_honests, f_real, f_decl, model):
   """ The name of the rule here that `defense` is, when the attack's search can run on the device:
   `defense` is an entry `install` registered, there are Byzantine rows to generate, every honest
-  gradient is a float32 CUDA vector, the rule's input fits the search's row limit for that rule
-  (`engine.search_max_rows`: 128 rows for the coordinate-wise rules, 64 for the distance rules), and the
-  rule accepts its parameters.  None otherwise: the stock attack then runs (and fails, if it must, as it
-  always did). """
+  gradient is a float32 CUDA vector, the rule's input fits the search's row limit for that entry
+  (128 rows for a wide entry of `install(..., wide=True)`; otherwise `engine.search_max_rows`: 128 rows for
+  the coordinate-wise rules, 64 for the distance rules), and the rule accepts its parameters.  None
+  otherwise: the stock attack then runs (and fails, if it must, as it always did). """
   import torch
-  from . import engine
   try:
-    name = _installed.get(defense)
+    installed = _installed.get(defense)
   except TypeError:                            # unhashable: not one of ours
     return None
-  if name is None or not isinstance(f_real, int) or f_real < 1 or not isinstance(grad_honests, list) or not grad_honests:
+  if installed is None or not isinstance(f_real, int) or f_real < 1 or not isinstance(grad_honests, list) or not grad_honests:
     return None
-  if len(grad_honests) + f_real > engine.search_max_rows(name) or not _is_cuda(grad_honests):
+  name, limit = installed
+  if len(grad_honests) + f_real > limit or not _is_cuda(grad_honests):
     return None
   if any(g.dtype != torch.float32 or g.dim() != 1 for g in grad_honests):
     return None
@@ -175,7 +185,8 @@ def install_attacks(attacks, backend=None, names=None):
   and `defense` is a rule `install` registered, run the whole `line_maximize` search on the device and
   read its outcome once (`engine.line_search`).  The attack direction is computed with the reference's
   torch statements.  Every other call — positive factors, a `--gars` mixture, a stock rule, CPU tensors,
-  more rows than the search takes for the rule (`engine.search_max_rows`) — runs the stock attack unchanged.  The reference's `register` builds the
+  more rows than the search takes against the entry (128 for a wide entry, `engine.search_max_rows` otherwise) —
+  runs the stock attack unchanged.  The reference's `register` builds the
   checked wrappers, with the stock checks.
   `names` may also list "anticge": the attack against CGE then runs on the device (`engine.anticge`) whenever
   its honest rows are fp32 CUDA vectors and `bz_anticge` takes its arguments, whatever the defense.
