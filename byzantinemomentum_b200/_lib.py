@@ -3,9 +3,10 @@
 `include/byzagg_attack.h`, `include/byzagg_search_shards.h`, `include/byzagg_search_peers.h`,
 `include/byzagg_coordinate.h`, `include/byzagg_peers_next.h`, `include/byzagg_distance.h`,
 `include/byzagg_distance_shards.h`, `include/byzagg_anticge.h`, `include/byzagg_anticge_peers.h` and
-`include/byzagg_distance_search.h`), and of the
-second library `libbyzagg_peers.so` built next to it (C ABI: `include/byzagg_distance_peers.h`), which the callers
-compose with the first through their C ABIs.
+`include/byzagg_distance_search.h` and `include/byzagg_distance_search_shards.h`), of the
+second library `libbyzagg_peers.so` built next to it (C ABI: `include/byzagg_distance_peers.h`) and of the third,
+`libbyzagg_star.so` (C ABI: `include/byzagg_rowshare_star.h`), which the callers compose with the first through their
+C ABIs.
 
 Each library is loaded lazily, on the first call that needs it, and the load FAILS LOUDLY:
 there is no CPU or PyTorch fallback anywhere in this package.  Build it in-tree with
@@ -17,7 +18,7 @@ import os
 import pathlib
 import threading
 
-__all__ = ["lib", "peers_lib", "LibraryError", "library_path", "peers_library_path", "check", "MAX_N", "MAX_N_COORDINATE", "MAX_N_DISTANCE", "STATUS_MESSAGES",
+__all__ = ["lib", "peers_lib", "star_lib", "LibraryError", "library_path", "peers_library_path", "star_library_path", "check", "MAX_N", "MAX_N_COORDINATE", "MAX_N_DISTANCE", "STATUS_MESSAGES",
            "AKSEL_MODES", "STATUS_NO_FINITE_SET", "STATUS_DEGENERATE"]
 
 MAX_N = 64
@@ -48,6 +49,13 @@ def peers_library_path():
   if override:
     return pathlib.Path(override)
   return library_path().parent / "libbyzagg_peers.so"
+
+def star_library_path():
+  """ libbyzagg_star.so: next to libbyzagg.so, or where BYZAGG_STAR_LIBRARY says. """
+  override = os.environ.get("BYZAGG_STAR_LIBRARY")
+  if override:
+    return pathlib.Path(override)
+  return library_path().parent / "libbyzagg_star.so"
 
 _c_rows = ctypes.POINTER(ctypes.c_void_p)
 _vp, _i, _i64, _sz, _dbl = ctypes.c_void_p, ctypes.c_int, ctypes.c_int64, ctypes.c_size_t, ctypes.c_double
@@ -160,6 +168,12 @@ DISTANCE_SEARCH_SIGNATURES = {
   "bz_distance_line_search_workspace_bytes": (_sz, [_i]),
   "bz_distance_line_search": (_i, [_i, _c_rows, _i, _i, _i, _i, _i, _vp, _vp, _i64, _i, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
 }
+# the same for include/byzagg_distance_search_shards.h (phase A of the d-sharded line search against Multi-Krum and
+# Bulyan above MAX_N rows, with the honest rows' distances kept between evaluations)
+DISTANCE_SEARCH_SHARD_SIGNATURES = {
+  "bz_distance_pass_tables_bytes": (_sz, []),
+  "bz_distance_partial_reuse": (_i, [_i, _c_rows, _i, _i64, _vp, _vp, _vp, _i, _vp, _vp, _vp, _sz, _vp]),
+}
 # the same for include/byzagg_distance_peers.h, the table of the second library (`peers_lib()`): phase B of the d-sharded
 # distance rules above MAX_N rows with its exchange over peer memory
 DISTANCE_PEER_SIGNATURES = {
@@ -167,12 +181,20 @@ DISTANCE_PEER_SIGNATURES = {
   "bz_distance_select_peers": (_i, [_i, _vp, _i, _i, _i, _i, _vp, _vp, _i, _i, _c_rows, _c_rows, ctypes.c_uint, _vp]),
   "bz_distance_select_peers_next": (_i, [_i, _vp, _i, _i, _i, _i, _vp, _vp, _i, _i, _c_rows, _c_rows, _vp]),
 }
+# the same for include/byzagg_rowshare_star.h, the table of the third library (`star_lib()`): CGE's candidate-only
+# phase A of the d-sharded line search above MAX_N rows
+ROWSHARE_STAR_SIGNATURES = {
+  "bz_rowshare_star_last_error": (ctypes.c_char_p, []),
+  "bz_rowshare_star_workspace_bytes": (_sz, [_i]),
+  "bz_rowshare_star": (_i, [_c_rows, _i, _i, _i64, _vp, _vp, _sz, _vp]),
+}
 SEARCH_STATE_BYTES = 64                     # BZ_SEARCH_STATE_BYTES
 CANDIDATE_FIRST, CANDIDATE_NEXT, CANDIDATE_FINAL = 0, 1, 2
 
 _lock = threading.Lock()
 _lib = None
 _peers_lib = None
+_star_lib = None
 
 def _load(path, tables):
   """ The library at `path` with the signatures of `tables` bound; LibraryError when it is missing or stale. """
@@ -201,7 +223,8 @@ def lib():
     if _lib is None:
       _lib = _load(library_path(), (SIGNATURES, SHARD_SIGNATURES, ATTACK_SIGNATURES, SEARCH_SHARD_SIGNATURES, SEARCH_PEER_SIGNATURES,
                                     COORDINATE_SIGNATURES, PEER_NEXT_SIGNATURES, DISTANCE_SIGNATURES, DISTANCE_SHARD_SIGNATURES,
-                                    ANTICGE_SIGNATURES, ANTICGE_PEER_SIGNATURES, DISTANCE_SEARCH_SIGNATURES))
+                                    ANTICGE_SIGNATURES, ANTICGE_PEER_SIGNATURES, DISTANCE_SEARCH_SIGNATURES,
+                                    DISTANCE_SEARCH_SHARD_SIGNATURES))
   return _lib
 
 def peers_lib():
@@ -214,12 +237,27 @@ def peers_lib():
       _peers_lib = _load(peers_library_path(), (DISTANCE_PEER_SIGNATURES,))
   return _peers_lib
 
+def star_lib():
+  """ The third library, libbyzagg_star.so (loads it on first use; no fallback when it is missing). """
+  global _star_lib
+  if _star_lib is not None:
+    return _star_lib
+  with _lock:
+    if _star_lib is None:
+      _star_lib = _load(star_library_path(), (ROWSHARE_STAR_SIGNATURES,))
+  return _star_lib
+
 def check(code, what):
   """ Raise on a non-zero return code of a bz_* call. """
   if code == 0:
     return
   # each library keeps the message of its own last failure
-  message = peers_lib().bz_distance_peers_last_error() if what in DISTANCE_PEER_SIGNATURES else lib().bz_last_error()
+  if what in DISTANCE_PEER_SIGNATURES:
+    message = peers_lib().bz_distance_peers_last_error()
+  elif what in ROWSHARE_STAR_SIGNATURES:
+    message = star_lib().bz_rowshare_star_last_error()
+  else:
+    message = lib().bz_last_error()
   message = message.decode("utf-8", "replace") if message else ""
   kinds = {-1: "invalid argument", -2: "unsupported", -3: "CUDA error", -4: "workspace"}
   error = ValueError if code in (-1, -2) else LibraryError

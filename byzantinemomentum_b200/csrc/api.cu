@@ -326,3 +326,4 @@ int bz_coordinate(int rule, const float* const* rows, int n, int f, int64_t d, f
 #include "api_anticge.inc"
 #include "api_anticge_peers.inc"
 #include "api_distance_search.inc"
+#include "api_distance_search_shards.inc"

@@ -31,7 +31,7 @@ import torch.distributed as dist
 from . import _lib
 from . import engine as _engine
 
-__all__ = ["aggregate", "aggregate_p2p", "compute_avg_dev_max", "study_step", "replicate", "apply_update", "shard_bounds", "rows_aligned", "choose_exchange", "rows_exchange", "plan_exchange", "choose_search_exchange", "PeerExchange", "FusedExchange", "ShardedPlan", "GradientShards", "choose_delivery", "ShardedLineSearch", "line_search", "choose_anticge_exchange", "ShardedAntiCGE", "anticge", "COORDINATE_WISE", "DISTANCE_BASED"]
+__all__ = ["aggregate", "aggregate_p2p", "compute_avg_dev_max", "study_step", "replicate", "apply_update", "shard_bounds", "rows_aligned", "choose_exchange", "rows_exchange", "plan_exchange", "choose_search_exchange", "PeerExchange", "FusedExchange", "ShardedPlan", "GradientShards", "choose_delivery", "ShardedLineSearch", "line_search", "search_rows", "search_exchange", "choose_anticge_exchange", "ShardedAntiCGE", "anticge", "COORDINATE_WISE", "DISTANCE_BASED"]
 
 COORDINATE_WISE = ("average", "median", "trmean", "phocas", "meamed")
 DISTANCE_BASED = _engine.DISTANCE_BASED
@@ -98,7 +98,8 @@ class FusedExchange:
   slots make that enough (a rank rewrites slot s only after every peer has signalled the step in
   between, i.e. finished reading s).
   `ShardedLineSearch(exchange="fused")` runs its exchanges (the rule's block, the score's share) over the
-  same buffer: one per call here, each advancing `epoch` by one.  That relies on one condition: the calls
+  same buffer: one per call here, each advancing `epoch` by one; above MAX_N rows (`wide=True`) the rule's block goes
+  through `bz_distance_select_peers`, as `ShardedPlan`'s does.  That relies on one condition: the calls
   that share a FusedExchange (the search and the `ShardedPlan` of the same n) are issued on ONE stream, in
   the same order on every rank.
   `ShardedAntiCGE(exchange="fused")` of nh honest rows runs its two exchanges (the nh norm sums, then the
@@ -108,7 +109,8 @@ class FusedExchange:
   `ShardedPlan(exchange="fused")` of Aksel and CGE up to MAX_N rows runs its exchange in K2′'s last CTA
   (`bz_rowdist_peers`); above MAX_N rows, for all four rules, in phase B's kernel (`bz_distance_select_peers`,
   which copies the plan's staged phase-A block into the slot first): one exchange per call or replay either way,
-  on the same condition of sharing.
+  on the same condition of sharing.  So a buffer of n rows serves a `ShardedPlan`, a `ShardedAntiCGE` and a
+  `ShardedLineSearch` of those n rows at any n, above MAX_N rows the search with `wide=True`.
   `epoch` is the host's count of the exchanges issued so far; the flags hold the same count on the device
   (this rank's own entry [rank] of its flag array, in the slot of its last epoch).  The eager calls pass
   `epoch` by value.  A captured call (`ShardedPlan.graph()`, `ShardedLineSearch.graph()`) cannot: its
@@ -326,6 +328,9 @@ class ShardedPlan:
   "nccl" or an explicit "fused" (`plan_exchange`: "auto" resolves to "nccl", "p2p" raises); "nccl"'s phases are
   `bz_distance_partial`, `bz_distance_select` and `bz_distance_reduce` at every n: the n x n block of 128 rows
   is 131 KB per rank.  One rank gives `engine.Plan`'s output, selection and status bit for bit.
+  With "fused" the buffer of `fused_exchange(n, ...)` can be shared with a `ShardedAntiCGE` of n honest rows and a
+  `ShardedLineSearch` of n rows (above MAX_N rows with `wide=True`), their calls on one stream in the same order on
+  every rank.
 
   `graph()` captures a step in a CUDA graph, as `engine.Plan.graph()` does: "fused" on any number of ranks
   (the captured kernel takes its epoch from the exchange buffer, the `_next` calls), any exchange on one
@@ -482,6 +487,14 @@ class ShardedPlan:
 
 SEARCH_EXCHANGES = ("auto", "fused", "nccl")
 
+def search_rows(gar, wide=False):
+  """ The most rows (honest + f_real) `ShardedLineSearch` takes against the rule `gar`: `engine.search_max_rows(gar)`,
+  and with `wide` MAX_N_DISTANCE for krum, bulyan, aksel and cge (brute stays at MAX_N, the coordinate-wise rules
+  at MAX_N_COORDINATE). """
+  if wide and gar in _engine.WIDE_DISTANCE:
+    return _lib.MAX_N_DISTANCE
+  return _engine.search_max_rows(gar)
+
 def choose_search_exchange(exchange, aligned, symmetric, engine, group=None):
   """ The exchange of `ShardedLineSearch`, the same on every rank of `group`: the local facts — `aligned`:
   this rank's rows suit the rule's fused call (16-byte aligned for Multi-Krum, Bulyan and brute, any for
@@ -502,6 +515,16 @@ def choose_search_exchange(exchange, aligned, symmetric, engine, group=None):
     raise ValueError(f"the fused exchange of the line search needs 16-byte aligned rows for krum / bulyan / brute on every rank, "
                      f"and symmetric memory on every one of at most {_lib.MAX_PEERS} ranks")
   return exchange
+
+def search_exchange(gar, n, exchange, aligned, symmetric, engine, group=None, wide=False):
+  """ The exchange of a `ShardedLineSearch` of n rows against `gar`, the same on every rank of `group`:
+  `choose_search_exchange`'s, except with `wide` for krum, bulyan, aksel and cge above MAX_N rows.  There the
+  exchange runs in phase B's kernel (`bz_distance_select_peers`), so rows of any alignment are served, and "auto"
+  resolves to "nccl", as `ShardedPlan` resolves it above MAX_N rows.  The ranks still agree through
+  `choose_search_exchange`'s one all-reduce. """
+  if wide and gar in _engine.WIDE_DISTANCE and n > _lib.MAX_N:
+    return choose_search_exchange("nccl" if exchange == "auto" else exchange, True, symmetric, engine, group)
+  return choose_search_exchange(exchange, aligned, symmetric, engine, group)
 
 DELIVERIES = ("auto", "p2p", "collective")
 
@@ -675,11 +698,11 @@ class _SearchShard:
     blocks, part   [world, width] gathered partial blocks of the rule / this rank's block (blocks[0] on one rank)
     scores, score  [world] gathered score shares / this rank's share (scores[:1] on one rank)
   `fuse(fx)` prepares the stages of the fused exchange over the FusedExchange `fx` as well. """
-  def __init__(self, gar, grad_honests, f_real, f_decl, grad_avg, grad_att, evals, negative, kind, world):
+  def __init__(self, gar, grad_honests, f_real, f_decl, grad_avg, grad_att, evals, negative, kind, world, wide=False):
     honest = list(grad_honests)
     f_real = int(f_real)
     n = len(honest) + f_real
-    limit = _engine.search_max_rows(gar)
+    limit = search_rows(gar, wide)
     if f_real < 1 or n > limit:
       raise ValueError(f"f_real = {f_real} with {len(honest)} honest rows: expected f_real >= 1 and at most {limit} rows")
     prep = _engine._prepare_device(honest, "the line search takes CUDA tensors", limit=limit)
@@ -709,9 +732,12 @@ class _SearchShard:
     self._stream = stream
     self.call = _engine._call           # every stage's calls go through it (`ShardedLineSearch.graph()` swaps it)
     self.distance = gar in DISTANCE_BASED
+    self.wide = self.distance and n > _lib.MAX_N
     eval_status = None
     self._pair = False
-    if not self.distance:
+    if self.wide:
+      eval_status = self._wide(gar, n, f_decl, honest, inputs, world)
+    elif not self.distance:
       self._coordinate = _engine._coordinate_call(gar, rows, f_decl, out)
     else:
       rule = self._rule = _engine._rule(gar, n, f_decl)
@@ -751,6 +777,58 @@ class _SearchShard:
     record = self.record.data_ptr()
     self._steps = [(lib.bz_search_step, (self.scores.data_ptr(), world, state, record, eval_status, record + 8 * (2 * evals + 1),
                                          k, evals, stream)) for k in range(evals)]
+  def _wide(self, gar, n, f_decl, honest, inputs, world):
+    """ The stages of a distance rule above MAX_N rows (krum, bulyan, aksel, cge): phase A through
+    `bz_distance_partial_reuse` (krum, bulyan: the honest rows' pass tables kept in two tables the evaluations
+    alternate between), `bz_distance_partial` (aksel after its local median; cge at the first evaluation, then
+    `bz_rowshare_star` of the third library, which rewrites only the candidate's sums), phases B and C through
+    `bz_distance_select` and `bz_distance_reduce`.  The search owns its workspace and tables, so nothing else on the
+    stream rewrites them between two evaluations.  Returns the evaluation's status word for the transition. """
+    lib = _lib.lib()
+    rows, device, stream, d = self._rows, self.device, self._stream, self._rows.d
+    out = self.out.data_ptr()
+    rule = self._rule = _engine._rule(gar, n, f_decl)
+    width = n * n if rule.pair else n
+    self.blocks = torch.zeros((world, width), dtype=torch.float64, device=device)
+    self.part = self.blocks[0] if world == 1 else torch.zeros(width, dtype=torch.float64, device=device)
+    self._meta = torch.zeros(n + 1, dtype=torch.int32, device=device)      # order[n] + status
+    meta = self._meta.data_ptr()
+    ws = self._ws = torch.empty(int(lib.bz_distance_workspace_bytes(n)), dtype=torch.uint8, device=device)
+    fn, args = self._score
+    self._score = fn, args[:5] + (ws.data_ptr(), ws.numel(), stream)
+    self._median = _engine._coordinate_call("median", rows, None, out) if rule.center else None
+    part = self.part.data_ptr()
+    full, select, self._reduce = rule.phase_entries(rows.ptrs, d, out if rule.center else None, part, self.blocks.data_ptr(),
+                                                    world, out, meta, ws, stream)
+    self._select = select
+    self._pair = rule.pair
+    if rule.pair:
+      # as up to MAX_N rows: the honest rows keep their unique rows, the candidate (one tensor f_real times) is the
+      # last unique row; evaluation k writes table k % 2, reading table (k - 1) % 2 after the first
+      first = {}
+      for g in inputs:
+        first.setdefault(g.data_ptr(), len(first))
+      u = len(first)
+      old_index = (ctypes.c_int32 * n)(*[first[g.data_ptr()] if i < len(honest) else -1 for i, g in enumerate(inputs)])
+      self._tables = torch.empty((2, int(lib.bz_distance_pass_tables_bytes()) // 8), dtype=torch.float64, device=device)
+      self._mode = ctypes.c_int(-1)
+      tables = [t.data_ptr() for t in self._tables]
+      code = _engine._SEARCH_RULES[gar]
+      def phase_a(s, reused):
+        reuse = (old_index, tables[1 - s], u) if reused else (None, None, 0)
+        return lib.bz_distance_partial_reuse, ((code, rows.ptrs, n, d, part) + reuse + (tables[s], ctypes.byref(self._mode))
+                                               + (ws.data_ptr(), ws.numel(), stream))
+      self._phase_a = [[phase_a(s, reused) for reused in (False, True)] for s in (0, 1)]
+    elif gar == "cge":
+      # after the first evaluation only the candidate's sums change: K2'-star (libbyzagg_star) rewrites part[nh, n)
+      star = _lib.star_lib()
+      self._star_ws = torch.empty(int(star.bz_rowshare_star_workspace_bytes(n)), dtype=torch.uint8, device=device)
+      self._phase_a = [full, (star.bz_rowshare_star, (rows.ptrs, n, len(honest), d, part, self._star_ws.data_ptr(),
+                                                      self._star_ws.numel(), stream))]
+    else:
+      self._phase_a = full
+    status = meta + 4 * n if rule.status else None
+    return None if gar == "krum" else status
   def fuse(self, fx):
     """ Prepare the stages of the fused exchange over `fx` (a `FusedExchange` of n rows): per evaluation the
     rule's `*_peers` call (distance rules) and `bz_search_score_peers`, every argument but the slot's
@@ -769,7 +847,13 @@ class _SearchShard:
       rule, meta = self._rule, self._meta.data_ptr()
       code = _engine._SEARCH_RULES[rule.gar]
       eval_status = meta + 4 * n
-      if self._pair:
+      if self.wide:
+        # above MAX_N rows: phase A into the staging block `part`, then phase B's kernel copies it into the slot and
+        # exchanges it (libbyzagg_peers), then phase C
+        peers_lib, (m, mode) = _lib.peers_lib(), rule._m_mode()
+        self._rule_peers = (peers_lib.bz_distance_select_peers, peers_lib.bz_distance_select_peers_next,
+                            (code, self.part.data_ptr(), n, rule.f, m, mode, meta, eval_status) + peers)
+      elif self._pair:
         head = (code, rows.ptrs, n, rule.f, rule.m, d, out, meta, eval_status)
         self._rule_peers = [[(lib.bz_pairdist_reuse_peers, lib.bz_pairdist_reuse_peers_next, head + reuse + peers)
                              for reuse in self._reuse[s]] for s in (0, 1)]
@@ -780,13 +864,24 @@ class _SearchShard:
     self._score_peers = [(lib.bz_search_score_peers, lib.bz_search_score_peers_next,
                           (out, self._avg, d, state, record, eval_status, record + 8 * (2 * self.evals + 1), k, self.evals) + peers)
                          for k in range(self.evals)]
-  def _with_slot(self, fn, fn_next, head, epoch):
-    """ An exchanging call: by value at `epoch`, or (None) its `_next` twin, which takes the epoch from the flags. """
+  def _with_slot(self, fn, fn_next, head, epoch, tail=None):
+    """ An exchanging call: by value at `epoch`, or (None) its `_next` twin, which takes the epoch from the flags.
+    `tail`: the arguments after the epoch (default: the workspace and the stream). """
+    tail = self._tail if tail is None else tail
     if epoch is None:
-      self.call(fn_next, head + self._both + self._tail)
+      self.call(fn_next, head + self._both + tail)
     else:
       blocks, flags = self._slots[epoch % 2]
-      self.call(fn, head + (blocks, flags, epoch) + self._tail)
+      self.call(fn, head + (blocks, flags, epoch) + tail)
+  def _phase_a_call(self, k):
+    """ (fn, args) of evaluation k's phase A on the distance-rule paths that reuse pair distances or take no reuse. """
+    if self.wide and self._rule.gar == "cge":
+      return self._phase_a[int(k > 0)]
+    if not self._pair:
+      return self._phase_a
+    if self.wide:
+      return self._phase_a[k % 2][int(k > 0)]
+    return self._phase_a[k % 2][int(k > 0 and self._mode.value >= 0)]
   def evaluate_fused(self, k, epoch):
     """ Evaluation k up to its score with the fused exchange: the candidate row, then the rule (distance
     rules: its exchange at `epoch`, or None: at the epoch the flags give; coordinate-wise rules: no exchange). """
@@ -794,6 +889,12 @@ class _SearchShard:
       self.call(*self._candidates[_lib.CANDIDATE_FIRST if k == 0 else _lib.CANDIDATE_NEXT])
       if not self.distance:
         self.call(*self._coordinate)
+      elif self.wide:
+        if self._median is not None:
+          self.call(*self._median)
+        self.call(*self._phase_a_call(k))
+        self._with_slot(*self._rule_peers, epoch, tail=(self._stream,))
+        self.call(*self._reduce)
       elif self._pair:
         self._with_slot(*self._rule_peers[k % 2][int(k > 0 and self._mode.value >= 0)], epoch)
       else:
@@ -812,15 +913,18 @@ class _SearchShard:
         call(*self._coordinate)
         call(*self._score)
         return self.score
-      if self._pair:
-        call(*self._phase_a[k % 2][int(k > 0 and self._mode.value >= 0)])
-      else:
-        if self._median is not None:
-          call(*self._median)
-        call(*self._phase_a)
+      if not self._pair and self._median is not None:
+        call(*self._median)
+      call(*self._phase_a_call(k))
     return self.part
   def conclude(self, blocks):
-    select = self._select if blocks is self.blocks else _engine._select_call(self._rule, blocks, self._meta.data_ptr(), self._stream)
+    if blocks is self.blocks:
+      select = self._select
+    elif self.wide:
+      fn, args = self._select
+      select = fn, args[:1] + (blocks.data_ptr(), blocks.shape[0]) + args[3:]
+    else:
+      select = _engine._select_call(self._rule, blocks, self._meta.data_ptr(), self._stream)
     with _engine._on(self.device):
       self.call(*select)
       self.call(*self._reduce)
@@ -880,11 +984,20 @@ class ShardedLineSearch:
             "auto"   "fused" on 2..16 ranks with symmetric memory, the CUDA engine and (Multi-Krum, Bulyan,
                      brute) 16-byte aligned rows on every rank, else "nccl"; the ranks agree on it
                      (`choose_search_exchange`).
+  wide:     False (default): the limits of `engine.search_max_rows` (64 rows against a distance rule), as before.
+            True: krum, bulyan, aksel and cge up to MAX_N_DISTANCE rows (`search_rows`; brute stays at MAX_N).
+            Above MAX_N rows phase A is `bz_distance_partial_reuse` (krum, bulyan: star passes of the candidate
+            after the first evaluation, over two pass tables the search owns), `bz_distance_partial` (aksel after
+            its local median; cge at the first evaluation, then `bz_rowshare_star` of libbyzagg_star.so, which reads
+            the candidate row alone), phases B and C `bz_distance_select` and `bz_distance_reduce`; "fused" exchanges
+            the block in `bz_distance_select_peers` (libbyzagg_peers.so, rows of any alignment), 2 exchanges per
+            evaluation; "auto" resolves to "nccl" there (`search_exchange`).  A stand-in backend gets
+            `wide=True` as a keyword after its 10 arguments.
   `graph()` captures the whole search in a CUDA graph, as `engine.LineSearch.graph()` does: "fused" on any
   number of ranks, "nccl" on one rank (no collective).  Like a search, `graph()` and every replay are
   collective: every rank issues them at the same point of its stream order. """
   def __init__(self, gar, grad_honests, f_real, f_decl, grad_avg, grad_att, evals, negative=False, kind="identical",
-               group=None, backend=None, exchange="auto"):
+               group=None, backend=None, exchange="auto", wide=False):
     if gar not in _engine._SEARCH_RULES:
       raise KeyError(f"unknown aggregation rule {gar!r}")
     if kind not in _engine._SEARCH_KINDS:
@@ -895,11 +1008,12 @@ class ShardedLineSearch:
     self.world = dist.get_world_size(group) if dist.is_initialized() else 1
     honest = list(grad_honests)
     pair = gar in ("krum", "bulyan", "brute")
-    self.exchange = choose_search_exchange(exchange, not pair or rows_aligned(honest), _symmetric_memory_importable(),
-                                           backend is None, group)
+    self.exchange = search_exchange(gar, len(honest) + int(f_real), exchange, not pair or rows_aligned(honest),
+                                    _symmetric_memory_importable(), backend is None, group, wide)
     make = _SearchShard if backend is None else backend.search_shard
     self._backend, self._graph = backend, None
-    self._shard = make(gar, honest, f_real, f_decl, grad_avg, grad_att, self.evals, negative, kind, self.world)
+    extra = {"wide": True} if wide else {}
+    self._shard = make(gar, honest, f_real, f_decl, grad_avg, grad_att, self.evals, negative, kind, self.world, **extra)
     self.byz, self.record = self._shard.byz, self._shard.record
     if self.exchange == "fused":
       n, device = len(honest) + int(f_real), self._shard.device
@@ -978,11 +1092,12 @@ class ShardedLineSearch:
     return _engine._search_outcome(self.record, self.evals)
 
 def line_search(gar, grad_honests, f_real, f_decl, grad_avg, grad_att, evals, negative=False, kind="identical", group=None,
-                exchange="auto"):
-  """ `engine.line_search` on a d-sharded trainer (see `ShardedLineSearch`): returns (factor, this rank's
-  shard of the Byzantine gradient), the factor the same Python float on every rank. """
+                exchange="auto", wide=False):
+  """ `engine.line_search` on a d-sharded trainer (see `ShardedLineSearch`, and its `wide` for krum, bulyan, aksel
+  and cge above MAX_N rows): returns (factor, this rank's shard of the Byzantine gradient), the factor the same
+  Python float on every rank. """
   search = ShardedLineSearch(gar, grad_honests, f_real, f_decl, grad_avg, grad_att, evals, negative, kind, group,
-                             exchange=exchange)
+                             exchange=exchange, wide=wide)
   byz = search()
   factor, _ = search.result()
   return factor, byz
