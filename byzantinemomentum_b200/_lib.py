@@ -6,7 +6,7 @@
 `include/byzagg_distance_search.h` and `include/byzagg_distance_search_shards.h`), of the
 second library `libbyzagg_peers.so` built next to it (C ABI: `include/byzagg_distance_peers.h`) and of the third,
 `libbyzagg_star.so` (C ABI: `include/byzagg_rowshare_star.h`), which the callers compose with the first through their
-C ABIs.
+C ABIs, and of the fourth, `libbyzagg_many.so` (C ABI: `include/byzagg_coordinate_many.h`), which links against the first.
 
 Each library is loaded lazily, on the first call that needs it, and the load FAILS LOUDLY:
 there is no CPU or PyTorch fallback anywhere in this package.  Build it in-tree with
@@ -18,11 +18,13 @@ import os
 import pathlib
 import threading
 
-__all__ = ["lib", "peers_lib", "star_lib", "LibraryError", "library_path", "peers_library_path", "star_library_path", "check", "MAX_N", "MAX_N_COORDINATE", "MAX_N_DISTANCE", "STATUS_MESSAGES",
+__all__ = ["lib", "peers_lib", "star_lib", "many_lib", "LibraryError", "library_path", "peers_library_path", "star_library_path",
+           "many_library_path", "check", "MAX_N", "MAX_N_COORDINATE", "MAX_N_MANY", "MAX_N_DISTANCE", "STATUS_MESSAGES",
            "AKSEL_MODES", "STATUS_NO_FINITE_SET", "STATUS_DEGENERATE"]
 
 MAX_N = 64
 MAX_N_COORDINATE = 128      # BZ_MAX_N_COORDINATE: the coordinate-wise rules through bz_coordinate
+MAX_N_MANY = 1024           # BZ_MAX_N_MANY: the coordinate-wise rules through bz_coordinate_many
 MAX_N_DISTANCE = 128        # BZ_MAX_N_DISTANCE: Multi-Krum, Bulyan, Aksel and CGE through bz_distance
 MAX_PEERS = 16
 STATUS_NO_FINITE_SET = 1
@@ -56,6 +58,13 @@ def star_library_path():
   if override:
     return pathlib.Path(override)
   return library_path().parent / "libbyzagg_star.so"
+
+def many_library_path():
+  """ libbyzagg_many.so: next to libbyzagg.so, or where BYZAGG_MANY_LIBRARY says. """
+  override = os.environ.get("BYZAGG_MANY_LIBRARY")
+  if override:
+    return pathlib.Path(override)
+  return library_path().parent / "libbyzagg_many.so"
 
 _c_rows = ctypes.POINTER(ctypes.c_void_p)
 _vp, _i, _i64, _sz, _dbl = ctypes.c_void_p, ctypes.c_int, ctypes.c_int64, ctypes.c_size_t, ctypes.c_double
@@ -139,6 +148,12 @@ PEER_NEXT_SIGNATURES = {
 COORDINATE_SIGNATURES = {
   "bz_coordinate": (_i, [_i, _c_rows, _i, _i, _i64, _vp, _vp]),
 }
+# the same for include/byzagg_coordinate_many.h, the table of the fourth library (`many_lib()`): the coordinate-wise
+# rules up to MAX_N_MANY rows
+COORDINATE_MANY_SIGNATURES = {
+  "bz_coordinate_many_last_error": (ctypes.c_char_p, []),
+  "bz_coordinate_many": (_i, [_i, _c_rows, _i, _i, _i64, _vp, _vp]),
+}
 # the same for include/byzagg_distance.h (Multi-Krum, Bulyan, Aksel and CGE up to MAX_N_DISTANCE rows)
 DISTANCE_SIGNATURES = {
   "bz_distance_workspace_bytes": (_sz, [_i]),
@@ -195,6 +210,7 @@ _lock = threading.Lock()
 _lib = None
 _peers_lib = None
 _star_lib = None
+_many_lib = None
 
 def _load(path, tables):
   """ The library at `path` with the signatures of `tables` bound; LibraryError when it is missing or stale. """
@@ -247,6 +263,17 @@ def star_lib():
       _star_lib = _load(star_library_path(), (ROWSHARE_STAR_SIGNATURES,))
   return _star_lib
 
+def many_lib():
+  """ The fourth library, libbyzagg_many.so (loads it on first use; no fallback when it is missing). """
+  global _many_lib
+  if _many_lib is not None:
+    return _many_lib
+  lib()                          # libbyzagg.so first: the fourth library links against it
+  with _lock:
+    if _many_lib is None:
+      _many_lib = _load(many_library_path(), (COORDINATE_MANY_SIGNATURES,))
+  return _many_lib
+
 def check(code, what):
   """ Raise on a non-zero return code of a bz_* call. """
   if code == 0:
@@ -256,6 +283,8 @@ def check(code, what):
     message = peers_lib().bz_distance_peers_last_error()
   elif what in ROWSHARE_STAR_SIGNATURES:
     message = star_lib().bz_rowshare_star_last_error()
+  elif what in COORDINATE_MANY_SIGNATURES:
+    message = many_lib().bz_coordinate_many_last_error()
   else:
     message = lib().bz_last_error()
   message = message.decode("utf-8", "replace") if message else ""

@@ -32,6 +32,13 @@ struct WideRowTable {
 // signature that names a constant of internal linkage would make their instantiations internal as well.
 template <int N> using RowsOf = typename std::conditional<(N <= BZ_MAX_N), RowTable, WideRowTable>::type;
 
+// The same for bz_coordinate_many above kMaxNCoordinate rows: 8 KB, a __grid_constant__ parameter (sm_70+
+// kernels take up to 32,764 bytes of parameters since CUDA 12.1).  Only the kernels of k1_many.cu take it.
+constexpr int kMaxNMany = BZ_MAX_N_MANY;
+struct ManyRowTable {
+  const float* p[kMaxNMany];
+};
+
 // Geometry of a launch over d coordinates with VEC per thread.  All rows (and the output)
 // share the same misalignment, so shifting the element index by `shift` (0..VEC-1) makes every
 // interior vector naturally aligned: logical vector v covers elements [v*VEC - shift,

@@ -22,7 +22,7 @@ import torch
 
 from . import _lib, hostmem
 
-__all__ = ["average", "median", "trmean", "phocas", "meamed", "krum", "bulyan", "brute", "aksel", "cge",
+__all__ = ["average", "median", "trmean", "phocas", "meamed", "coordinate_many", "krum", "bulyan", "brute", "aksel", "cge",
            "pairdist_partial", "rowdist_partial", "select", "krum_select", "bulyan_select", "brute_select",
            "rowdist_select", "average_selected", "bulyan_reduce", "avg_dev_max_async", "compute_avg_dev_max", "rowdots_async", "study_step",
            "StudyPartials", "study_partials", "study_finish",
@@ -157,8 +157,8 @@ def _copy_streams(device):
   return lanes
 
 def _validate(gradients, limit=_lib.MAX_N):
-  """ One pass over the list: types, dtype, rank, length (at most `limit` rows: MAX_N, or
-  MAX_N_COORDINATE for the coordinate-wise rules); returns (first, all_contiguous). """
+  """ One pass over the list: types, dtype, rank, length (at most `limit` rows: MAX_N, MAX_N_DISTANCE,
+  or MAX_N_MANY for the coordinate-wise rules); returns (first, all_contiguous). """
   if not isinstance(gradients, (list, tuple)) or len(gradients) < 1:
     raise ValueError(f"expected a non-empty list of gradients, got {type(gradients).__name__} of length {len(gradients) if hasattr(gradients, '__len__') else '?'}")
   first = gradients[0]
@@ -359,19 +359,24 @@ def _coordinate_pipeline(name, gradients, f, path, device):
   return result
 
 def _coordinate_call(name, prep, f, out):
-  """ (fn, args) of the coordinate-wise rule `name` writing to the address `out`. """
-  return _lib.lib().bz_coordinate, (_RULE_CODES[name], prep.ptrs, prep.n, 0 if f is None else int(f), prep.d, out, prep.stream)
+  """ (fn, args) of the coordinate-wise rule `name` writing to the address `out`: `bz_coordinate` up to
+  MAX_N_COORDINATE rows, `bz_coordinate_many` above. """
+  fn = _lib.many_lib().bz_coordinate_many if prep.n > _lib.MAX_N_COORDINATE else _lib.lib().bz_coordinate
+  return fn, (_RULE_CODES[name], prep.ptrs, prep.n, 0 if f is None else int(f), prep.d, out, prep.stream)
 
-def _coordinate(name, gradients, f=None):
+def _coordinate(name, gradients, f=None, limit=_lib.MAX_N_COORDINATE):
+  if limit == _lib.MAX_N_COORDINATE and type(gradients) in (list, tuple) and len(gradients) > limit:
+    raise ValueError(f"{len(gradients)} gradients exceed the supported maximum of {limit} (`gars.many_gars`, "
+                     f"`engine.coordinate_many` and `Plan` take the coordinate-wise rules up to {_lib.MAX_N_MANY})")
   if type(gradients) in (list, tuple) and len(gradients) > 0 and isinstance(gradients[0], torch.Tensor) and gradients[0].device.type == "cpu" and torch.cuda.is_available():
-    _validate(gradients, _lib.MAX_N_COORDINATE)
+    _validate(gradients, limit)
     _lib.lib()
     device = torch.device("cuda", torch.cuda.current_device())
     path = _host_path(device)
     if len(gradients) <= _lib.MAX_N and path.choose(True, False) == "pipeline":
       torch.cuda.current_stream(device).synchronize()        # the clock times this call only
       return _coordinate_pipeline(name, gradients, f, path, device)
-  prep = _prepare(gradients, single_pass=True, limit=_lib.MAX_N_COORDINATE)
+  prep = _prepare(gradients, single_pass=True, limit=limit)
   out = torch.empty(prep.d, dtype=torch.float32, device=prep.device)
   _run(prep.device, *_coordinate_call(name, prep, f, out.data_ptr()))
   return _finish(prep, out)
@@ -390,6 +395,15 @@ def phocas(gradients, f):
 
 def meamed(gradients, f):
   return _coordinate("meamed", gradients, f)
+
+def coordinate_many(name, gradients, f=None):
+  """ The coordinate-wise rule `name` (average, median, trmean, phocas, meamed) over up to MAX_N_MANY
+  gradients: the call of `engine.<name>` up to MAX_N_COORDINATE rows, `bz_coordinate_many` above.  CUDA rows
+  give a CUDA vector; host rows are staged (per-row copies above MAX_N rows) and give a host vector.
+  `engine.<name>` and the `gars` entries keep their MAX_N_COORDINATE rows; `gars.many_gars` calls this. """
+  if name not in _RULE_CODES:
+    raise ValueError(f"unknown coordinate-wise rule {name!r}, expected one of {sorted(_RULE_CODES)}")
+  return _coordinate(name, gradients, f, limit=_lib.MAX_N_MANY)
 
 # ---------------------------------------------------------------------------- #
 # Distance reuse across calls (SURVEY.md §8(f) row 1)
@@ -1260,13 +1274,13 @@ class Plan:
       plan = engine.Plan("krum", gradients, f=5)
       aggregated = plan()          # same tensor every time: plan.out
       plan.selection               # device int32 (distance-based rules)
-  Up to MAX_N_COORDINATE rows for the coordinate-wise rules, MAX_N_DISTANCE for krum, bulyan, aksel and cge
+  Up to MAX_N_MANY rows for the coordinate-wise rules (above MAX_N_COORDINATE through `bz_coordinate_many`), MAX_N_DISTANCE for krum, bulyan, aksel and cge
   (above MAX_N through `bz_distance`, with a workspace of its own), MAX_N for brute.
   For brute / bulyan the device status word is NOT checked here (that would synchronise);
   read `plan.status` when needed: non-zero means the rule is undefined on this data and `out`
   is NaN. """
   def __init__(self, gar, gradients, f=None, m=None, mode="mid", out=None):
-    limit = _lib.MAX_N_COORDINATE if gar in _RULE_CODES else _lib.MAX_N_DISTANCE if gar in WIDE_DISTANCE else _lib.MAX_N
+    limit = _lib.MAX_N_MANY if gar in _RULE_CODES else _lib.MAX_N_DISTANCE if gar in WIDE_DISTANCE else _lib.MAX_N
     prep = _prepare(list(gradients), limit=limit)
     if prep.to_cpu:
       raise ValueError("Plan takes CUDA tensors (host tensors go through the plain call, which stages them)")

@@ -8,7 +8,9 @@ unknown keywords are accepted and ignored), returning a NEW tensor, and carrying
 names (average, median, trmean, phocas, meamed, krum, bulyan, brute, aksel, cge) to them.
 `wide_gars` holds krum, bulyan, aksel and cge again, built the same way, for 1 to 128 gradients
 (`BZ_MAX_N_DISTANCE`): up to 64 they make exactly the call of their `gars` entry, above it they run
-`bz_distance`.  `plugin.install(..., wide=True)` registers them.
+`bz_distance`.  `plugin.install(..., wide=True)` registers them.  `many_gars` holds the five coordinate-wise
+rules again, for 1 to 1024 gradients (`BZ_MAX_N_MANY`): up to 128 they make exactly the call of their `gars`
+entry, above it they run `bz_coordinate_many`.  `plugin.install(..., many=True)` registers them.
 The arithmetic runs in `libbyzagg.so` (see `engine.py`); this module only holds the
 argument checks, the closed-form bounds and the selection bookkeeping for `influence`.
 
@@ -17,7 +19,7 @@ Differences with the reference, all deliberate:
     reuses the selection computed on the device instead of recomputing all distances
     (attack.py:822 always follows attack.py:821);
   * the coordinate-wise rules (average, median, trmean, phocas, meamed) take up to 128 gradients
-    (`BZ_MAX_N_COORDINATE`); with more than 64 gradients the distance-based rules of `gars` raise
+    (`BZ_MAX_N_COORDINATE`), and those of `many_gars` up to 1024 (`BZ_MAX_N_MANY`); with more than 64 gradients the distance-based rules of `gars` raise
     (`BZ_MAX_N`), with a message saying so, and those of `wide_gars` take up to 128.  Above 64
     gradients a `wide_gars` call reuses no distance of the previous call.
 """
@@ -27,7 +29,7 @@ import math
 from . import _lib, engine
 from .engine import _Memo as _Selection, _rule
 
-__all__ = ["gars", "wide_gars", "make_gar", "register", "UserException", "last_selection"]
+__all__ = ["gars", "wide_gars", "many_gars", "make_gar", "register", "UserException", "last_selection"]
 
 class UserException(RuntimeError):
   """ Raised by `checked` on invalid parameters (the reference raises tools.UserException). """
@@ -269,3 +271,18 @@ def _wide(name):
   return make_gar(unchecked, narrow.check, upper_bound=narrow.upper_bound, influence=influence, name=name)
 
 wide_gars = {name: _wide(name) for name in engine.WIDE_DISTANCE}
+
+# ---------------------------------------------------------------------------- #
+# The coordinate-wise rules for up to 1024 gradients
+
+def _many(name):
+  """ The `many_gars` entry of `name`: the check, bound and influence of `gars[name]`, the call of
+  `engine.coordinate_many` (which is `gars[name]`'s call up to MAX_N_COORDINATE gradients). """
+  narrow = gars[name]
+  takes_f = name in ("trmean", "phocas", "meamed")
+  def unchecked(gradients, f=None, **kwargs):
+    return engine.coordinate_many(name, gradients, f if takes_f else None)
+  unchecked.__name__ = narrow.unchecked.__name__
+  return make_gar(unchecked, narrow.check, upper_bound=narrow.upper_bound, influence=narrow.influence, name=name)
+
+many_gars = {name: _many(name) for name in ("average", "median", "trmean", "phocas", "meamed")}

@@ -9,7 +9,8 @@ routes lead there without touching a reference file:
      `<prefix><name>` (default prefix "b200-"), or replaces the stock entries in place with
      `override=True` (`register` refuses duplicates, :82-84, so the entry is rebuilt with the
      reference's `make_gar`).  With `wide=True` it registers krum, bulyan, aksel and cge from
-     `gars.wide_gars`, which take up to 128 gradients instead of 64.
+     `gars.wide_gars`, which take up to 128 gradients instead of 64; with `many=True`, average, median,
+     trmean, phocas and meamed from `gars.many_gars`, which take up to 1024 gradients instead of 128.
   2. the top-level `native` package of this repository: the reference already looks for
      `native.{median,krum,bulyan,brute}.aggregate` and registers `native-<name>` when it finds
      them (median.py:80-87, krum.py:159-166, bulyan.py:137-144, brute.py:149-156).
@@ -23,7 +24,7 @@ attack against CGE run on the device (`engine.anticge`).  The search takes the r
 
 import math
 
-from .gars import gars, wide_gars
+from .gars import gars, wide_gars, many_gars
 
 __all__ = ["install", "install_tools", "install_attacks"]
 
@@ -39,7 +40,7 @@ def _record(aggregators, key, name, rule):
     wide = wide_gars.get(name) is rule
     _installed[entry] = (name, _lib.MAX_N_DISTANCE if wide else engine.search_max_rows(name))
 
-def install(aggregators, prefix="b200-", override=False, names=None, wide=False):
+def install(aggregators, prefix="b200-", override=False, names=None, wide=False, many=False):
   """ Register the CUDA rules in the reference's `aggregators` module.
   Args:
     aggregators  The imported reference package (duck-typed: needs `gars`, `register`, `make_gar`)
@@ -50,12 +51,15 @@ def install(aggregators, prefix="b200-", override=False, names=None, wide=False)
                  attacks' device search against them up to 128 rows.  The default, False, keeps `gars`' entries,
                  which stop at 64 gradients, as every earlier release did; the other six rules are the same
                  either way
+    many         Register average, median, trmean, phocas and meamed from `gars.many_gars`: up to 1024 gradients.
+                 The attacks' device search against them keeps its 128 rows; above, the stock attack runs and calls
+                 the entry for each evaluation.  The default, False, keeps `gars`' entries, which stop at 128
   Returns:
     List of the registered names
   """
   done = []
   for name in (names or gars.keys()):
-    rule = wide_gars[name] if wide and name in wide_gars else gars[name]
+    rule = wide_gars[name] if wide and name in wide_gars else many_gars[name] if many and name in many_gars else gars[name]
     if override:
       wrapped = aggregators.make_gar(rule.unchecked, rule.check, upper_bound=rule.upper_bound, influence=rule.influence)
       aggregators.gars[name] = wrapped

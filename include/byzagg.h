@@ -28,7 +28,8 @@
  *   - Return value: 0 on success, a negative BZ_E* code otherwise; bz_last_error() returns
  *     a thread-local message for the last failure.
  *   - 1 <= n <= bz_max_n() (= 64), d >= 0 (d = 0 is a no-op).  The coordinate-wise rules take up
- *     to 128 rows through bz_coordinate (byzagg_coordinate.h, included at the end), and so do
+ *     to 128 rows through bz_coordinate (byzagg_coordinate.h, included at the end), and to 1024 through
+ *     bz_coordinate_many (byzagg_coordinate_many.h); up to 128 rows so do
  *     bz_avg_dev_max and bz_line_search with a coordinate-wise rule.  Multi-Krum, Bulyan, Aksel
  *     and CGE take up to 128 rows through bz_distance (byzagg_distance.h, included at the end).
  *   - Parameter validity (f, m ranges) is the caller's job, exactly like the reference's
@@ -292,6 +293,9 @@ BZ_API int bz_gradient_row(const float* grad, int64_t d, double clip, float* sam
 /* The coordinate-wise rules (average, median, trimmed mean, Phocas, MeaMed) for up to
  * BZ_MAX_N_COORDINATE = 128 rows: bz_coordinate. */
 #include "byzagg_coordinate.h"
+
+/* The same rules for up to BZ_MAX_N_MANY = 1024 rows, each column sorted by a warp: bz_coordinate_many. */
+#include "byzagg_coordinate_many.h"
 
 /* The exchanges over peer memory (bz_krum_peers ... bz_search_score_peers) with the epoch taken from the
  * exchange buffer instead of an argument, so that a CUDA graph can capture them: the _next calls. */
