@@ -147,13 +147,14 @@ k1_median(const __grid_constant__ WideRowTable rows, const Geom g, float* __rest
 
 // ---- trimmed mean of a sorted column (trmean.py:33) -----------------------------------------
 // `values[f:-f].mean(dim=0)`: ATen sums rows in a cascade of 16-row blocks (sequential when
-// R = n - 2f <= 16), then divides by R with one IEEE division.
+// R = n - 2f <= 16), then divides by R with one IEEE division.  f = 0 keeps the whole column.
 template <int N>
 __device__ __forceinline__ float trmean_sorted(const float (&s)[N], const int f) {
   const int R = N - 2 * f;
   const int hi = N - f;
   float acc0 = 0.f;
-  if (N - 2 <= 16 || R <= 16) {
+  // N <= 17 keeps R <= 17 at every f; at R = 17 the cascade's s16 + S16 (S16 = s0 + ... + s15) is the sequential S16 + s16
+  if (N <= 17 || R <= 16) {
 #pragma unroll
     for (int k = 0; k < N; ++k)
       if (k >= f && k < hi) acc0 = __fadd_rn(acc0, s[k]);

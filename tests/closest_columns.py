@@ -33,11 +33,12 @@ def center(x, f, mode):
   return orc.trmean(x, f) if mode == "phocas" else orc.median(x)
 
 def k1_closest(x, f, mode, c=None):
-  """ K1's closest epilogue on the [n, d] rows x: (out fp32 [d], chosen bool [n, d] in the rows' order). """
+  """ K1's closest epilogue on the [n, d] rows x: (out fp32 [d], chosen bool [n, d] in the rows' order).
+  f = 0 (m = n) compares no pairs: the whole column summed in rank order. """
   x = np.asarray(x, dtype=F32)
   n, d = x.shape
   m = n - f
-  assert 1 <= f < m, (n, f)
+  assert 0 <= f < m, (n, f)
   c = center(x, f, mode) if c is None else np.asarray(c, dtype=F32)
   keys = to_key(x)
   order = np.argsort(keys, axis=0, kind="stable")
@@ -80,10 +81,10 @@ def sum_bound(values, exact):
   itself is fsum / m in fp64, off by 2^-52 of it). """
   v = np.asarray(values, dtype=np.float64)
   m = v.shape[0]
-  with np.errstate(invalid="ignore"):
-    mag = np.abs(v).sum(axis=0) / m
   g = (m - 1) * U / (1 - (m - 1) * U)
-  return (1 + U) * g * mag + (U + 2. ** -50) * np.abs(exact) + 2. ** -149
+  with np.errstate(invalid="ignore"):         # columns holding +-inf or NaN: the bound is NaN there
+    mag = np.abs(v).sum(axis=0) / m
+    return (1 + U) * g * mag + (U + 2. ** -50) * np.abs(exact) + 2. ** -149
 
 def check_restatement(x, f, mode, what=""):
   """ `k1_closest` against the exact reference on every column of x: a valid closest set of m values
@@ -114,12 +115,13 @@ def check_restatement(x, f, mode, what=""):
     parity.assert_in_hull(out, x, overflow, what + " [overflow]")
   return out, chosen, c
 
-def check_kernel(got, x, f, mode, what="", want=None):
+def check_kernel(got, x, f, mode, what="", want=None, c=None):
   """ A kernel's output against `k1_closest`, value for value (NaN == NaN) on every column, and, where the
-  chosen values are unique, against the oracle within the scaled bar of tests/parity.py. """
+  chosen values are unique, against the oracle within the scaled bar of tests/parity.py.  `c`: the centre,
+  when the caller has it already. """
   x = np.asarray(x, dtype=F32)
   n = x.shape[0]
-  c = center(x, f, mode)
+  c = center(x, f, mode) if c is None else np.asarray(c, dtype=F32)
   if want is None:
     want = k1_closest(x, f, mode, c)[0]
   parity.assert_bit_exact(np.asarray(got, dtype=F32), want, what + " [K1's closest epilogue]")

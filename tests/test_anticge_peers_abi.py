@@ -6,7 +6,9 @@ the exchange (`sharded.choose_anticge_exchange`) under gloo with two ranks.  No 
 
 `tests/golden/kernels_before_anticge_peers.json` records, for every kernel of the library as it was before these
 entry points, its registers, its stack and a digest of its SASS (`kernel_table`); it was written with
-`python tests/test_anticge_peers_abi.py --record byzantinemomentum_b200/libbyzagg.so` on that library."""
+`python tests/test_anticge_peers_abi.py --record byzantinemomentum_b200/libbyzagg.so` on that library.  The entries of
+`k1_sorted<18, 1, -1, -1>` and `k1_sorted<18, 4, -1, -1>` were recorded later, when the 18-row trimmed mean at f = 0
+began to sum in ATen's cascade order (`trmean_sorted` in k1_select.cuh)."""
 
 import ctypes
 import hashlib

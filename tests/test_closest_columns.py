@@ -99,6 +99,23 @@ def test_constructed_columns_get_their_outcomes(n):
       with np.errstate(all="ignore"):
         assert len(set(cc.abs_key(x[:, j] - c[j]).tolist())) <= n // 2 + 1
 
+@pytest.mark.parametrize("n", [1, 2, 3, 16, 17, 18, 40, 129])
+def test_f0_keeps_the_whole_column_in_rank_order(n):
+  """ f = 0 (m = n): no pairs; every entry chosen, summed from +0.0 in rank order, divided by n. """
+  x = random_columns(n, 2000, 19 * n)
+  s = cc.from_key(np.sort(cc.to_key(x), axis=0))
+  acc = np.zeros(x.shape[1], dtype=F32)
+  with np.errstate(all="ignore"):
+    for k in range(n):
+      acc = (acc + s[k]).astype(F32)
+    whole = (acc / F32(n)).astype(F32)
+  for mode in cc.MODES:
+    what = f"n={n} f=0 {mode}"
+    out, chosen, c = cc.check_restatement(x, 0, mode, what)
+    assert chosen.all(), what
+    assert parity.equal_values(out, np.where(np.isnan(c), np.nan, whole)).all(), what
+    cc.check_kernel(out, x, 0, mode, what)
+
 def test_exact_mean_is_exact():
   rng = np.random.default_rng(1)
   v = (rng.standard_normal((37, 5)) * 10. ** rng.integers(-30, 30, (37, 5))).astype(F32)

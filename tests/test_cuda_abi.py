@@ -53,7 +53,8 @@ def _call_coord(name, rows, f=None):
 
 @pytest.mark.parametrize("n", list(range(1, 65)))
 def test_median_trmean_every_n(n):
-  """ Sorting network of every size: median and trimmed means (all valid f) vs the oracle, bit-exact. """
+  """ Sorting network of every size: median and trimmed means (f = 1, (n - 1) // 4, (n - 1) // 2; every f in
+  test_cuda_every_f.py) vs the oracle, bit-exact. """
   d = 1000 + n
   x = _rand_rows(n, d, 1000 + n)
   rows = [x[i].to(DEV) for i in range(n)]

@@ -8,7 +8,8 @@ kernel of libbyzagg.so unchanged in resources and SASS, and the choice of `Shard
 `tests/golden/kernels_before_distance_peers.json` records, for every kernel of libbyzagg.so as it was before the
 second library, its registers, its stack and a digest of its SASS (`kernel_table` of test_anticge_peers_abi.py); it
 was written with `python tests/test_distance_peers_abi.py --record byzantinemomentum_b200/libbyzagg.so` on that
-library."""
+library.  The entries of `k1_sorted<18, 1, -1, -1>` and `k1_sorted<18, 4, -1, -1>` were recorded later, when the
+18-row trimmed mean at f = 0 began to sum in ATen's cascade order (`trmean_sorted` in k1_select.cuh)."""
 
 import ctypes
 import json
