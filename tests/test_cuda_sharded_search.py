@@ -128,15 +128,15 @@ def _shards(full, R, pitched):
       out.append([v[lo:hi] for v in full])
   return out
 
-def _emulate(gar, honest, f, avg, att, R, pitched, evals=16, negative=False, kind="identical"):
-  """ R ShardedLineSearch instances on one GPU driven through the stages; returns (instances, the
-  concatenated rule output of every evaluation). """
+def _emulate(gar, honest, f, avg, att, R, pitched, evals=16, negative=False, kind="identical", wide=False):
+  """ R ShardedLineSearch instances on one GPU driven through the stages (`wide`: as they take it); returns
+  (instances, the concatenated rule output of every evaluation). """
   from byzantinemomentum_b200 import sharded
   vectors = honest + [avg] + ([att] if att is not None else [])
   per_rank = _shards(vectors, R, pitched)
   nh = len(honest)
   inst = [sharded.ShardedLineSearch(gar, rows[:nh], f, f, rows[nh], rows[nh + 1] if att is not None else None, evals,
-                                    negative=negative, kind=kind) for rows in per_rank]
+                                    negative=negative, kind=kind, wide=wide) for rows in per_rank]
   outs = []
   for k in range(evals):
     parts = [s.evaluate(k) for s in inst]

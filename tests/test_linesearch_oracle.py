@@ -1,15 +1,18 @@
 # coding: utf-8
 """The restatement of `line_maximize` in tests/line_oracle.py against the reference's own
-`tools.line_maximize` (tools/misc.py:468-513) on synthetic scapes: the same x sequence, bit for bit, and the same result.  The GPU tests of the
+`tools.line_maximize` (tools/misc.py:468-513) on synthetic scapes and on the scripted scapes of
+tests/line_scapes.py: the same x sequence, bit for bit, and the same result.  The GPU tests of the
 device search compare against it, since they cannot read the reference.  Runs only when
 $BYZ_REFERENCE points at a reference checkout."""
 
 import math
 import sys
 
+import numpy as np
 import pytest
 
 import line_oracle
+import line_scapes
 from oracle import reference
 
 pytestmark = pytest.mark.skipif(reference.find_root() is None, reason="$BYZ_REFERENCE not set (live-reference test)")
@@ -48,3 +51,31 @@ def test_oracle_line_maximize_matches_the_reference(evals):
   xs = []
   line_oracle.line_maximize(lambda x: (xs.append(x), 1. if x == 0 else -x)[1], evals=16)
   assert min(xs) >= 0 and all(x >= 0 for x in xs)
+
+def _fl32(y):
+  with np.errstate(over="ignore"):
+    return float(np.float32(y))
+
+@pytest.mark.parametrize("rounded", [False, True])
+@pytest.mark.parametrize("evals", line_scapes.EVALS)
+def test_oracle_matches_the_reference_on_scripted_scapes(evals, rounded):
+  """ The scripted scapes of tests/line_scapes.py (ties, NaN, +-inf, -0.0, expansion to the end of the
+  budget, long halving runs), as doubles and rounded to fp32 as the device's scores are: the same x
+  sequence and the same result, bit for bit.  The device transition's tests feed these scapes. """
+  reference.load()
+  tools = sys.modules["tools"]
+  for name, scape in line_scapes.SCAPES:
+    seen = {"ref": [], "orc": []}
+    def traced(key):
+      def f(x):
+        k = len(seen[key])
+        seen[key].append(x)
+        y = scape(k, x, evals)
+        return _fl32(y) if rounded else y
+      return f
+    want = tools.line_maximize(traced("ref"), evals=evals)
+    got = line_oracle.line_maximize(traced("orc"), evals=evals)
+    assert len(seen["ref"]) == evals and len(seen["orc"]) == evals, name
+    assert [x.hex() for x in map(float, seen["orc"])] == [x.hex() for x in map(float, seen["ref"])], (name, evals)
+    assert float(got).hex() == float(want).hex(), (name, evals)
+    assert all(x >= 0 for x in seen["orc"]), (name, evals)
