@@ -311,6 +311,37 @@ def _run(device, fn, args):
   with _on(device):
     _call(fn, args)
 
+def _capture(prepared, device, issue, result, fx=None, exchanges=0):
+  """ The `graph()` of a prepared call.  On first use: one eager call `prepared()` (the warm-up), then a CUDA
+  graph of `issue(call)` on `device`, kept in `prepared._graph`, where every `call(fn, args)` is made on the
+  capture stream (a prepared call's last argument is its stream).  The first call that fails ends the issuing;
+  its error is raised once the capture has ended.  Returns `replay`: it launches the graph, advances the fused
+  exchange `fx` (if any) by the graph's `exchanges` and returns `result()`. """
+  if prepared._graph is None:
+    prepared()
+    failed = []
+    with _on(device):
+      torch.cuda.synchronize(device)
+      graph = torch.cuda.CUDAGraph()
+      with torch.cuda.graph(graph):
+        stream = torch.cuda.current_stream(device).cuda_stream
+        def call(fn, args):
+          if not failed:
+            code = fn(*(args[:-1] + (stream,)))
+            if code != 0:
+              failed.append((code, fn.__name__))
+        issue(call)
+    if failed:
+      _lib.check(*failed[0])
+    prepared._graph = graph
+  graph = prepared._graph
+  def replay():
+    graph.replay()
+    if fx is not None:
+      fx._reserve(exchanges)
+    return result()
+  return replay
+
 def _check_like_rows(vector, prep, what):
   if vector.dtype != torch.float32 or vector.shape != (prep.d,) or vector.device != prep.device or not vector.is_contiguous():
     raise ValueError(f"{what} must be a contiguous float32 vector like the rows")
@@ -673,21 +704,7 @@ class LineSearch:
     return self.byz
   def graph(self):
     """ Capture the search in a CUDA graph; returns `replay`, which launches it and returns `byz`. """
-    if self._graph is None:
-      with _on(self.device):
-        self()                                           # warm-up outside the capture
-        torch.cuda.synchronize(self.device)
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph):
-          code = self._fn(*(self._args[:-1] + (torch.cuda.current_stream(self.device).cuda_stream,)))
-        if code != 0:
-          _lib.check(code, self._fn.__name__)
-      self._graph = graph
-    graph, byz = self._graph, self.byz
-    def replay():
-      graph.replay()
-      return byz
-    return replay
+    return _capture(self, self.device, lambda call: call(self._fn, self._args), lambda: self.byz)
   def result(self):
     """ (factor, trace) from ONE device->host read: trace = [(x_k, y_k), ...].  With
     `config.strict_status`, a failed evaluation of Bulyan or brute raises what the plain call raises. """
@@ -743,34 +760,17 @@ class AntiCGE:
     self.byz = torch.empty(prep.d, dtype=torch.float32, device=prep.device)
     self._ws = torch.empty(int(_lib.lib().bz_anticge_workspace_bytes(prep.n)), dtype=torch.uint8, device=prep.device)
     self._fn = _lib.lib().bz_anticge
-    self._args = (prep.ptrs, prep.n, f_decl, f_real, prep.d, self.byz.data_ptr(), self._ws.data_ptr(), self._ws.numel())
+    self._args = (prep.ptrs, prep.n, f_decl, f_real, prep.d, self.byz.data_ptr(), self._ws.data_ptr(), self._ws.numel(),
+                  prep.stream)
     self._graph = None
-  def _issue(self):
-    return self._fn(*(self._args + (torch.cuda.current_stream(self.device).cuda_stream,)))
   def __call__(self):
     """ Enqueue the attack on the current stream of the rows' device; returns [byz] * f_real. """
     with _on(self.device):
-      code = self._issue()
-    if code != 0:
-      _lib.check(code, self._fn.__name__)
+      _call(self._fn, self._args[:-1] + (torch.cuda.current_stream(self.device).cuda_stream,))
     return [self.byz] * self.f_real
   def graph(self):
     """ Capture the call in a CUDA graph; returns `replay`, which launches it and returns [byz] * f_real. """
-    if self._graph is None:
-      with _on(self.device):
-        self()                                           # warm-up outside the capture
-        torch.cuda.synchronize(self.device)
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph):
-          code = self._issue()
-        if code != 0:
-          _lib.check(code, self._fn.__name__)
-      self._graph = graph
-    graph, byz, count = self._graph, self.byz, self.f_real
-    def replay():
-      graph.replay()
-      return [byz] * count
-    return replay
+    return _capture(self, self.device, lambda call: call(self._fn, self._args), lambda: [self.byz] * self.f_real)
 
 def anticge(grad_honests, f_decl, f_real):
   """ attacks/anticge.py's attack on the device (see `AntiCGE`): a new row, returned f_real times. """
@@ -1317,22 +1317,7 @@ class Plan:
     programmatic-dependent-launch edges) as ONE graph launch and returns `plan.out`.  Every launch
     of the library is capturable (it never synchronises and allocates nothing).  Worth it where
     launch latency shows: small d, or a host loop that cannot stay ahead of the GPU. """
-    if self._graph is None:
-      with _on(self.device):
-        self()                                           # warm-up outside the capture (module loading, attributes)
-        torch.cuda.synchronize(self.device)
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph):
-          stream = torch.cuda.current_stream(self.device).cuda_stream      # the capture stream
-          code = self._fn(*(self._args[:-1] + (stream,)))
-        if code != 0:                                    # raised after the capture has ended
-          _lib.check(code, self._fn.__name__)
-      self._graph = graph
-    graph, out = self._graph, self.out
-    def replay():
-      graph.replay()
-      return out
-    return replay
+    return _capture(self, self.device, lambda call: call(self._fn, self._args), lambda: self.out)
   def __call__(self):
     if torch.cuda.current_device() == self.device.index:
       code = self._fn(*self._args)

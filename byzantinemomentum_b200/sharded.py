@@ -22,6 +22,7 @@ multi-GPU form of its `aggregate(gradients, f, ...)`.
 phases raise.
 """
 
+import collections
 import ctypes
 import math
 
@@ -111,13 +112,16 @@ class FusedExchange:
   which copies the plan's staged phase-A block into the slot first): one exchange per call or replay either way,
   on the same condition of sharing.  So a buffer of n rows serves a `ShardedPlan`, a `ShardedAntiCGE` and a
   `ShardedLineSearch` of those n rows at any n, above MAX_N rows the search with `wide=True`.
-  `epoch` is the host's count of the exchanges issued so far; the flags hold the same count on the device
-  (this rank's own entry [rank] of its flag array, in the slot of its last epoch).  The eager calls pass
-  `epoch` by value.  A captured call (`ShardedPlan.graph()`, `ShardedLineSearch.graph()`) cannot: its
-  kernel takes the epoch from the flags instead (one past the later of the two own entries, wrap-aware; 1
-  on a zeroed buffer; the `bz_*_peers_next` calls), and each replay adds the graph's exchanges to `epoch`,
-  so that eager calls and replays can interleave on one buffer. """
+  The epoch rule, kept here alone: `epoch` is the host's count of the exchanges issued so far (unbounded; the
+  kernels see it modulo 2^32), and the flags hold the same count on the device (this rank's own entry [rank]
+  of its flag array, in the slot of its last epoch).  An eager call of k exchanges takes `epoch + 1` as its
+  first epoch, passes it by value with the tables of slot `epoch % 2` (`bz_anticge_peers`: of both slots),
+  and leaves `epoch` k higher (`_reserve`).  A captured call cannot pass it: its `bz_*_peers_next` twin takes
+  both slots' tables and the epoch from the flags (one past the later of the two own entries, wrap-aware; 1
+  on a zeroed buffer), and each replay reserves the graph's exchanges, so that eager calls and replays can
+  interleave on one buffer.  `_args` forms the arguments either way. """
   FLAG_WORDS = 16
+  _slot_tables = None                                          # (slot 0's, slot 1's, both()), built on first use
   def __init__(self, n, device, group=None):
     import torch.distributed._symmetric_memory as symm_mem
     self.n, self.device = n, device
@@ -153,31 +157,28 @@ class FusedExchange:
     pointers), slot 0's then slot 1's. """
     (b0, f0), (b1, f1) = self.tables(0), self.tables(1)
     return ((ctypes.c_void_p * (2 * self.world))(*b0, *b1), (ctypes.c_void_p * (2 * self.world))(*f0, *f1))
+  def _reserve(self, k):
+    """ The first epoch of a call of k exchanges; `epoch` is left k higher. """
+    first = self.epoch + 1
+    self.epoch += k
+    return first
+  def _args(self, exchanging, epoch):
+    """ (fn, args) of the `_Exchanging` call by value at `epoch`, or (None) of its `_next` twin. """
+    if self._slot_tables is None:
+      self._slot_tables = (self.tables(0), self.tables(1), self.both())
+    fn, fn_next, head, tail, both = exchanging
+    if epoch is None:
+      return fn_next, head + self._slot_tables[2] + tail
+    return fn, head + self._slot_tables[2 if both else epoch % 2] + (epoch % (1 << 32),) + tail
+
+# A call that exchanges over a `FusedExchange`: its by-value entry point, its `_next` twin, its arguments before the
+# slot tables (`head`) and after the epoch (`tail`); `both`: the by-value call takes both slots' tables.
+_Exchanging = collections.namedtuple("_Exchanging", "fn fn_next head tail both", defaults=(False,))
 
 _fused = {}
 
 def fused_exchange(n, device, group=None):
   return _registered(_fused, FusedExchange, n, device, group)
-
-def _capture(device, issue):
-  """ A CUDA graph of `issue(call)` on `device`: every `call(fn, args)` of a prepared call is made on the
-  capture stream (a prepared call's last argument is the stream current at construction).  The first call
-  that fails ends the issuing; its error is raised once the capture has ended. """
-  failed = []
-  with _engine._on(device):
-    torch.cuda.synchronize(device)
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph):
-      stream = torch.cuda.current_stream(device).cuda_stream
-      def call(fn, args):
-        if not failed:
-          code = fn(*(args[:-1] + (stream,)))
-          if code != 0:
-            failed.append((code, fn.__name__))
-      issue(call)
-  if failed:
-    _lib.check(*failed[0])
-  return graph
 
 def _capturable(exchange, world, what):
   """ Raise unless `what` can capture `exchange` on `world` ranks: "fused" anywhere, any exchange on one rank. """
@@ -379,12 +380,11 @@ class ShardedPlan:
     if exchange == "fused" and rule.pair and n <= _lib.MAX_N:
       fx = self._fx = fused_exchange(n, device, group)
       self.status = self._meta[n:]                          # krum too: a peer that never signals
-      self._fused_fn = getattr(_lib.lib(), f"bz_{gar}_peers")
-      self._next_fn = getattr(_lib.lib(), f"bz_{gar}_peers_next")
-      self._fused_head = (prep.ptrs, n) + rule.params + (prep.d, out, meta, status, fx.rank, fx.world)
-      self._fused_tail = (ws.data_ptr(), ws.numel(), prep.stream)
+      lib = _lib.lib()
+      self._exchanging = _Exchanging(getattr(lib, f"bz_{gar}_peers"), getattr(lib, f"bz_{gar}_peers_next"),
+                                     (prep.ptrs, n) + rule.params + (prep.d, out, meta, status, fx.rank, fx.world),
+                                     (ws.data_ptr(), ws.numel(), prep.stream))
       self._fused_around = ([], [])
-      self._fused_tables, self._next_tables = [fx.tables(0), fx.tables(1)], fx.both()
       return
     # aksel: the coordinate-wise median of the local shard is the center of phase A
     self._median = _engine.Plan("median", self.rows) if rule.center else None
@@ -418,24 +418,23 @@ class ShardedPlan:
     before = [(self._median._fn, self._median._args)] if self._median is not None else []
     if n <= _lib.MAX_N:
       lib = _lib.lib()
-      self._fused_fn, self._next_fn = lib.bz_rowdist_peers, lib.bz_rowdist_peers_next
-      self._fused_head = (code, prep.ptrs, n, rule.f, mode, center, prep.d, out, meta, status, fx.rank, fx.world)
-      self._fused_tail = (ws.data_ptr(), ws.numel(), prep.stream)
+      self._exchanging = _Exchanging(lib.bz_rowdist_peers, lib.bz_rowdist_peers_next,
+                                     (code, prep.ptrs, n, rule.f, mode, center, prep.d, out, meta, status, fx.rank, fx.world),
+                                     (ws.data_ptr(), ws.numel(), prep.stream))
       self._fused_around = (before, [])
     else:
       peers = _lib.peers_lib()
       self._part = torch.empty(n * n if rule.pair else n, dtype=torch.float64, device=device)
       a, _, c = rule.phase_entries(prep.ptrs, prep.d, center, self._part.data_ptr(), None, 1, out, meta, ws, prep.stream)
-      self._fused_fn, self._next_fn = peers.bz_distance_select_peers, peers.bz_distance_select_peers_next
-      self._fused_head = (code, self._part.data_ptr(), n, rule.f, m, mode, meta, status, fx.rank, fx.world)
-      self._fused_tail = (prep.stream,)
+      self._exchanging = _Exchanging(peers.bz_distance_select_peers, peers.bz_distance_select_peers_next,
+                                     (code, self._part.data_ptr(), n, rule.f, m, mode, meta, status, fx.rank, fx.world),
+                                     (prep.stream,))
       self._fused_around = (before + [a], [c])
-    self._fused_tables, self._next_tables = [fx.tables(0), fx.tables(1)], fx.both()
   def __call__(self):
     if self._local is not None:
       return self._local()
     with _engine._on(self.device):
-      self._issue(_engine._call)
+      self._issue()
     return self.out
   def graph(self):
     """ Capture a step in a CUDA graph (after one eager step, the warm-up) and return `replay`: a callable
@@ -443,28 +442,16 @@ class ShardedPlan:
     if self._local is not None:
       return self._local.graph()
     _capturable(self.exchange, self.world, "ShardedPlan")
-    if self._graph is None:
-      self()
-      self._graph = _capture(self.device, lambda call: self._issue(call, captured=True))
-    graph, out, fx = self._graph, self.out, self._fx if self.exchange == "fused" else None
-    def replay():
-      graph.replay()
-      if fx is not None:
-        fx.epoch += 1
-      return out
-    return replay
-  def _issue(self, call, captured=False):
+    fx = self._fx if self.exchange == "fused" else None
+    return _engine._capture(self, self.device, lambda call: self._issue(call, captured=True), lambda: self.out, fx, 1)
+  def _issue(self, call=_engine._call, captured=False):
     """ One step's calls through `call(fn, args)`; `captured`: the fused exchange takes its epoch from the buffer. """
     if self.exchange == "fused":
       before, after = self._fused_around
       for step in before:
         call(*step)
-      if captured:
-        call(self._next_fn, self._fused_head + self._next_tables + self._fused_tail)
-      else:
-        fx = self._fx
-        fx.epoch += 1
-        call(self._fused_fn, self._fused_head + self._fused_tables[fx.epoch % 2] + (fx.epoch,) + self._fused_tail)
+      fx = self._fx
+      call(*fx._args(self._exchanging, None if captured else fx._reserve(1)))
       for step in after:
         call(*step)
       return
@@ -730,7 +717,7 @@ class _SearchShard:
                         for which in (_lib.CANDIDATE_FIRST, _lib.CANDIDATE_NEXT, _lib.CANDIDATE_FINAL)]
     self._score = (lib.bz_search_score_partial, (out, avg, d, state, self.score.data_ptr(), ws.data_ptr(), ws.numel(), stream))
     self._stream = stream
-    self.call = _engine._call           # every stage's calls go through it (`ShardedLineSearch.graph()` swaps it)
+    self.call = _engine._call           # every stage's calls go through it (`ShardedLineSearch._issue` sets it)
     self.distance = gar in DISTANCE_BASED
     self.wide = self.distance and n > _lib.MAX_N
     eval_status = None
@@ -838,9 +825,8 @@ class _SearchShard:
     lib = _lib.lib()
     rows, ws, stream = self._rows, self._ws, self._stream
     n, d, state, out, record = rows.n, rows.d, self._state.data_ptr(), self.out.data_ptr(), self.record.data_ptr()
-    self._slots = [fx.tables(0), fx.tables(1)]
-    self._both = fx.both()
-    self._tail = (ws.data_ptr(), ws.numel(), stream)
+    self._fx = fx
+    tail = (ws.data_ptr(), ws.numel(), stream)
     peers = (fx.rank, fx.world)
     eval_status = None
     if self.distance:
@@ -851,28 +837,21 @@ class _SearchShard:
         # above MAX_N rows: phase A into the staging block `part`, then phase B's kernel copies it into the slot and
         # exchanges it (libbyzagg_peers), then phase C
         peers_lib, (m, mode) = _lib.peers_lib(), rule._m_mode()
-        self._rule_peers = (peers_lib.bz_distance_select_peers, peers_lib.bz_distance_select_peers_next,
-                            (code, self.part.data_ptr(), n, rule.f, m, mode, meta, eval_status) + peers)
+        self._rule_peers = _Exchanging(peers_lib.bz_distance_select_peers, peers_lib.bz_distance_select_peers_next,
+                                       (code, self.part.data_ptr(), n, rule.f, m, mode, meta, eval_status) + peers, (stream,))
       elif self._pair:
         head = (code, rows.ptrs, n, rule.f, rule.m, d, out, meta, eval_status)
-        self._rule_peers = [[(lib.bz_pairdist_reuse_peers, lib.bz_pairdist_reuse_peers_next, head + reuse + peers)
+        self._rule_peers = [[_Exchanging(lib.bz_pairdist_reuse_peers, lib.bz_pairdist_reuse_peers_next, head + reuse + peers, tail)
                              for reuse in self._reuse[s]] for s in (0, 1)]
       else:
         mode = _lib.AKSEL_MODES["mid"] if rule.center else 0
-        self._rule_peers = (lib.bz_rowdist_peers, lib.bz_rowdist_peers_next,
-                            (code, rows.ptrs, n, rule.f, mode, out if rule.center else None, d, out, meta, eval_status) + peers)
-    self._score_peers = [(lib.bz_search_score_peers, lib.bz_search_score_peers_next,
-                          (out, self._avg, d, state, record, eval_status, record + 8 * (2 * self.evals + 1), k, self.evals) + peers)
+        self._rule_peers = _Exchanging(lib.bz_rowdist_peers, lib.bz_rowdist_peers_next,
+                                       (code, rows.ptrs, n, rule.f, mode, out if rule.center else None, d, out, meta,
+                                        eval_status) + peers, tail)
+    self._score_peers = [_Exchanging(lib.bz_search_score_peers, lib.bz_search_score_peers_next,
+                                     (out, self._avg, d, state, record, eval_status, record + 8 * (2 * self.evals + 1), k,
+                                      self.evals) + peers, tail)
                          for k in range(self.evals)]
-  def _with_slot(self, fn, fn_next, head, epoch, tail=None):
-    """ An exchanging call: by value at `epoch`, or (None) its `_next` twin, which takes the epoch from the flags.
-    `tail`: the arguments after the epoch (default: the workspace and the stream). """
-    tail = self._tail if tail is None else tail
-    if epoch is None:
-      self.call(fn_next, head + self._both + tail)
-    else:
-      blocks, flags = self._slots[epoch % 2]
-      self.call(fn, head + (blocks, flags, epoch) + tail)
   def _phase_a_call(self, k):
     """ (fn, args) of evaluation k's phase A on the distance-rule paths that reuse pair distances or take no reuse. """
     if self.wide and self._rule.gar == "cge":
@@ -893,18 +872,18 @@ class _SearchShard:
         if self._median is not None:
           self.call(*self._median)
         self.call(*self._phase_a_call(k))
-        self._with_slot(*self._rule_peers, epoch, tail=(self._stream,))
+        self.call(*self._fx._args(self._rule_peers, epoch))
         self.call(*self._reduce)
       elif self._pair:
-        self._with_slot(*self._rule_peers[k % 2][int(k > 0 and self._mode.value >= 0)], epoch)
+        self.call(*self._fx._args(self._rule_peers[k % 2][int(k > 0 and self._mode.value >= 0)], epoch))
       else:
         if self._median is not None:
           self.call(*self._median)
-        self._with_slot(*self._rule_peers, epoch)
+        self.call(*self._fx._args(self._rule_peers, epoch))
   def score_fused(self, k, epoch):
     """ The score of evaluation k, its exchange at `epoch` (None: at the epoch the flags give) and the transition. """
     with _engine._on(self.device):
-      self._with_slot(*self._score_peers[k], epoch)
+      self.call(*self._fx._args(self._score_peers[k], epoch))
   def evaluate(self, k):
     call = self.call
     with _engine._on(self.device):
@@ -1038,10 +1017,6 @@ class ShardedLineSearch:
     if self.world > 1:
       dist.all_gather_into_tensor(gathered.view(-1), part, group=self.group)
     return gathered
-  def _epoch(self):
-    """ The epoch of the next exchange over the shared buffer. """
-    self._fx.epoch += 1
-    return self._fx.epoch
   def graph(self):
     """ Capture the whole search (every evaluation and the last candidate) in a CUDA graph, after one eager
     search (the warm-up), and return `replay`: a callable that launches it and returns `byz`.  With "fused",
@@ -1051,41 +1026,33 @@ class ShardedLineSearch:
       raise ValueError("ShardedLineSearch.graph() needs the CUDA engine, not a stand-in backend")
     _capturable(self.exchange, self.world, "ShardedLineSearch")
     shard = self._shard
-    if self._graph is None:
-      self()
-      def issue(call):
-        shard.call = call
-        try:
-          self._issue(captured=True)
-        finally:
-          shard.call = _engine._call
-      self._graph = _capture(shard.device, issue)
-    graph, byz = self._graph, self.byz
     fx = self._fx if self.exchange == "fused" else None
-    exchanges = (2 if shard.distance else 1) * self.evals
-    def replay():
-      graph.replay()
-      if fx is not None:
-        fx.epoch += exchanges
-      return byz
-    return replay
+    return _engine._capture(self, shard.device, lambda call: self._issue(call, captured=True), lambda: self.byz, fx,
+                            (2 if shard.distance else 1) * self.evals)
   def __call__(self):
     return self._issue()
-  def _issue(self, captured=False):
-    """ The search's stages and exchanges; `captured`: the fused exchanges take their epochs from the buffer. """
+  def _issue(self, call=_engine._call, captured=False):
+    """ The search's stages and exchanges, every C call of the CUDA engine's stages through `call(fn, args)`;
+    `captured`: the fused exchanges take their epochs from the buffer. """
     shard = self._shard
-    if self.exchange == "fused":
-      epoch = (lambda: None) if captured else self._epoch
+    shard.call = call
+    try:
+      if self.exchange == "fused":
+        fx = self._fx
+        def epoch():
+          return None if captured else fx._reserve(1)
+        for k in range(self.evals):
+          shard.evaluate_fused(k, epoch() if shard.distance else None)
+          shard.score_fused(k, epoch())
+        return self.finish()
       for k in range(self.evals):
-        shard.evaluate_fused(k, epoch() if shard.distance else None)
-        shard.score_fused(k, epoch())
+        part = self.evaluate(k)
+        if shard.distance:
+          part = self.conclude(self._exchange(shard.blocks, part))
+        self.step(k, self._exchange(shard.scores, part))
       return self.finish()
-    for k in range(self.evals):
-      part = self.evaluate(k)
-      if shard.distance:
-        part = self.conclude(self._exchange(shard.blocks, part))
-      self.step(k, self._exchange(shard.scores, part))
-    return self.finish()
+    finally:
+      shard.call = _engine._call
   def result(self):
     """ (factor, trace) from ONE device->host read, the same on every rank; with `engine.config.strict_status`,
     a failed evaluation of Bulyan or brute raises what the plain call raises. """
@@ -1166,12 +1133,11 @@ class ShardedAntiCGE:
       self._fuse(FusedExchange.local(prep.n, prep.device) if self.world == 1 else fused_exchange(prep.n, prep.device, group))
   def _fuse(self, fx):
     """ Run the fused exchanges over `fx`, a FusedExchange of n = nh. """
-    p = self._prep
+    p, lib = self._prep, _lib.lib()
     self._fx = fx
-    self._fused_head = (p.ptrs, p.n, self.f_decl, self.f_real, p.d, self.byz.data_ptr(), self.status.data_ptr(), fx.rank,
-                        fx.world) + fx.both()
-    self._fused_tail = (self._ws.data_ptr(), self._ws.numel())
-    self._exchanges = 0 if self.f_real > self.f_decl else 2
+    self._exchanging = _Exchanging(lib.bz_anticge_peers, lib.bz_anticge_peers_next,
+                                   (p.ptrs, p.n, self.f_decl, self.f_real, p.d, self.byz.data_ptr(), self.status.data_ptr(),
+                                    fx.rank, fx.world), (self._ws.data_ptr(), self._ws.numel()), both=True)
   def _stream(self):
     return torch.cuda.current_stream(self.device).cuda_stream
   def norms(self):
@@ -1202,38 +1168,22 @@ class ShardedAntiCGE:
     """ Capture a step in a CUDA graph (after one eager step, the warm-up) and return `replay`: a callable that
     launches it and returns [byz] * f_real.  With "fused", each replay advances the exchange's epoch by two. """
     _capturable(self.exchange, self.world, "ShardedAntiCGE")
-    if self._graph is None:
-      self()
-      with _engine._on(self.device):
-        torch.cuda.synchronize(self.device)
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph):
-          self._issue(captured=True)
-      self._graph = graph
-    graph, byz, count = self._graph, self.byz, self.f_real
-    fx, exchanges = (self._fx, self._exchanges) if self.exchange == "fused" else (None, 0)
-    def replay():
-      graph.replay()
-      if fx is not None:
-        fx.epoch += exchanges
-      return [byz] * count
-    return replay
-  def _issue(self, captured=False):
-    """ A step's calls; `captured`: the fused call takes its epoch from the buffer. """
-    lib = _lib.lib()
+    fx = self._fx if self.exchange == "fused" else None
+    return _engine._capture(self, self.device, lambda call: self._issue(call, captured=True), lambda: [self.byz] * self.f_real,
+                            fx, 0 if self.f_real > self.f_decl else 2)
+  def _issue(self, call=_engine._call, captured=False):
+    """ A step's calls, the fused one and the NaN fill's through `call(fn, args)`; `captured`: the fused call takes
+    its epoch from the buffer. """
     if self.exchange == "fused":
-      if captured:
-        _engine._call(lib.bz_anticge_peers_next, self._fused_head + self._fused_tail + (self._stream(),))
-        return
       fx = self._fx
-      epoch = (fx.epoch + 1) % (1 << 32)
-      fx.epoch += self._exchanges
-      _engine._call(lib.bz_anticge_peers, self._fused_head + (epoch,) + self._fused_tail + (self._stream(),))
+      # two exchanges, none for the NaN fill of f_real > f_decl
+      fn, args = fx._args(self._exchanging, None if captured else fx._reserve(0 if self.f_real > self.f_decl else 2))
+      call(fn, args + (self._stream(),))
       return
     if self.f_real > self.f_decl:
       p = self._prep
-      _engine._call(lib.bz_anticge, (p.ptrs, p.n, self.f_decl, self.f_real, p.d, self.byz.data_ptr(), self._ws.data_ptr(),
-                                     self._ws.numel(), self._stream()))
+      call(_lib.lib().bz_anticge, (p.ptrs, p.n, self.f_decl, self.f_real, p.d, self.byz.data_ptr(), self._ws.data_ptr(),
+                                   self._ws.numel(), self._stream()))
       return
     blocks = _gather(self.norms(), self.group)
     self.scale(_gather(self.sum(blocks), self.group).reshape(-1))
