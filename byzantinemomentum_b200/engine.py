@@ -24,7 +24,7 @@ from . import _lib, hostmem
 
 __all__ = ["average", "median", "trmean", "phocas", "meamed", "coordinate_many", "krum", "bulyan", "brute", "aksel", "cge",
            "pairdist_partial", "rowdist_partial", "select", "krum_select", "bulyan_select", "brute_select",
-           "rowdist_select", "average_selected", "bulyan_reduce", "avg_dev_max_async", "compute_avg_dev_max", "rowdots_async", "study_step",
+           "rowdist_select", "average_selected", "bulyan_reduce", "avg_dev_max_async", "avg_dev_max_many_async", "compute_avg_dev_max", "rowdots_async", "study_step",
            "StudyPartials", "study_partials", "study_finish",
            "wide_distance", "LineSearch", "line_search", "AntiCGE", "anticge", "config", "Plan", "pair_cache_stats", "GradientStack", "gradient_scatter", "momentum_rows", "host_path_report"]
 
@@ -660,18 +660,22 @@ class LineSearch:
   (kind "empire-strict": `grad_avg.mul(-x)`) against the rule `gar` with its defaults and f = f_decl,
   every evaluation, score and next factor computed on the device.  Against krum, bulyan, aksel and cge it takes
   up to MAX_N_DISTANCE rows (honest + f_real): above MAX_N through `bz_distance_line_search`, with a workspace
-  of its own, as `Plan` does.  Like `Plan`, `search()` only issues
+  of its own, as `Plan` does.  With `many`, against the coordinate-wise rules it takes up to MAX_N_MANY rows through
+  `bz_line_search_many` (libbyzagg_many_tools.so), which makes `bz_line_search`'s call up to MAX_N_COORDINATE rows; the
+  distance rules raise ValueError there.  Like `Plan`, `search()` only issues
   the call (no allocation, no synchronisation; `graph()` captures it) and holds what it reads and writes:
       byz     the candidate row; after the call the attack's Byzantine gradient for the chosen factor
       record  fp64 [2 * evals + 2]: (x_k, y_k) per evaluation, the chosen factor, then the status word
   `result()` reads `record` once and returns (factor, trace), raising where the plain rule raises. """
-  def __init__(self, gar, grad_honests, f_real, f_decl, grad_avg, grad_att, evals, negative=False, kind="identical"):
+  def __init__(self, gar, grad_honests, f_real, f_decl, grad_avg, grad_att, evals, negative=False, kind="identical", many=False):
     if gar not in _SEARCH_RULES:
       raise KeyError(f"unknown aggregation rule {gar!r}")
     if kind not in _SEARCH_KINDS:
       raise ValueError(f"unknown attack kind {kind!r}, expected one of {sorted(_SEARCH_KINDS)}")
+    if many and gar not in _RULE_CODES:
+      raise ValueError(f"many=True takes the coordinate-wise rules {sorted(_RULE_CODES)}, not {gar!r}")
     honest = list(grad_honests)
-    limit = _lib.MAX_N_DISTANCE if gar in WIDE_DISTANCE else search_max_rows(gar)
+    limit = _lib.MAX_N_MANY if many else _lib.MAX_N_DISTANCE if gar in WIDE_DISTANCE else search_max_rows(gar)
     prep = _prepare(honest, limit=limit)
     if prep.to_cpu:
       raise ValueError("the line search takes CUDA tensors")
@@ -686,7 +690,9 @@ class LineSearch:
     self._out = torch.empty(prep.d, dtype=torch.float32, device=prep.device)
     self.record = torch.empty(2 * max(self.evals, 0) + 2, dtype=torch.float64, device=prep.device)
     n = prep.n + int(f_real)
-    if n > _lib.MAX_N and gar in WIDE_DISTANCE:
+    if many:
+      self._fn, ws_bytes = _lib.many_tools_lib().bz_line_search_many, _lib.many_tools_lib().bz_line_search_many_workspace_bytes
+    elif n > _lib.MAX_N and gar in WIDE_DISTANCE:
       self._fn, ws_bytes = _lib.lib().bz_distance_line_search, _lib.lib().bz_distance_line_search_workspace_bytes
     else:
       self._fn, ws_bytes = _lib.lib().bz_line_search, _lib.lib().bz_line_search_workspace_bytes
@@ -720,11 +726,11 @@ def _search_outcome(record, evals):
   values = host.tolist()
   return values[2 * evals], [(values[2 * k], values[2 * k + 1]) for k in range(evals)]
 
-def line_search(gar, grad_honests, f_real, f_decl, grad_avg, grad_att, evals, negative=False, kind="identical"):
-  """ The attacks' factor search on the device (see `LineSearch`).  Returns (factor, byz): the factor
-  `tools.line_maximize` picks, a Python float, and the Byzantine gradient the attack returns for it, a
-  device tensor (the reference returns it `f_real` times, aliased). """
-  search = LineSearch(gar, grad_honests, f_real, f_decl, grad_avg, grad_att, evals, negative, kind)
+def line_search(gar, grad_honests, f_real, f_decl, grad_avg, grad_att, evals, negative=False, kind="identical", many=False):
+  """ The attacks' factor search on the device (see `LineSearch`, and its `many` for the coordinate-wise rules up to
+  MAX_N_MANY rows).  Returns (factor, byz): the factor `tools.line_maximize` picks, a Python float, and the Byzantine
+  gradient the attack returns for it, a device tensor (the reference returns it `f_real` times, aliased). """
+  search = LineSearch(gar, grad_honests, f_real, f_decl, grad_avg, grad_att, evals, negative, kind, many)
   byz = search()
   factor, _ = search.result()
   return factor, byz
@@ -791,6 +797,28 @@ def avg_dev_max_async(samples):
   _run(prep.device, _lib.lib().bz_avg_dev_max, (prep.ptrs, prep.n, prep.d, avg.data_ptr(), stats.data_ptr(), ws.data_ptr(), ws.numel(), prep.stream))
   return avg, stats
 
+_study_workspaces = {}
+
+def avg_dev_max_many_async(samples):
+  """ `avg_dev_max_async` for up to MAX_N_MANY rows (`bz_avg_dev_max_many`, libbyzagg_many_tools.so): up to
+  MAX_N_COORDINATE rows the call of `bz_avg_dev_max`, the same bits; above, K6-many.  Its workspace, one per
+  (device, stream), is its own.  No sync. """
+  prep = _prepare_device(samples, "the study metrics take CUDA tensors (tools.compute_avg_dev_max handles CPU samples)",
+                         limit=_lib.MAX_N_MANY)
+  avg = torch.empty(prep.d, dtype=torch.float32, device=prep.device)
+  stats = torch.empty(2 + prep.n, dtype=torch.float64, device=prep.device)
+  tools = _lib.many_tools_lib()
+  key = (prep.device.index, prep.stream)
+  ws = _study_workspaces.pop(key, None)
+  if ws is None:
+    ws = torch.empty(int(tools.bz_avg_dev_max_many_workspace_bytes(_lib.MAX_N_MANY)), dtype=torch.uint8, device=prep.device)
+    while len(_study_workspaces) >= _MAX_WORKSPACES:
+      _study_workspaces.pop(next(iter(_study_workspaces)))
+  _study_workspaces[key] = ws                                  # most recently used last
+  _run(prep.device, tools.bz_avg_dev_max_many, (prep.ptrs, prep.n, prep.d, avg.data_ptr(), stats.data_ptr(), ws.data_ptr(),
+                                                ws.numel(), prep.stream))
+  return avg, stats
+
 class _Memo:
   """ One result of a computation `what` with parameters `params`, valid only for the very tensor
   OBJECTS it was computed on (held through weak references, compared with `is`, like `_CallCache`),
@@ -827,10 +855,11 @@ class _Memo:
 # grad_sampleds[:nb_honests]`, attack.py:808): the second pass over n x d is saved.
 _study_memo = _Memo()
 
-def compute_avg_dev_max(samples):
+def compute_avg_dev_max(samples, many=False):
   """ Drop-in for `tools.compute_avg_dev_max(samples)` (tools/pytorch.py:97-125): returns
   (average gradient or None, norm of the average, norm standard deviation, max |coordinate| of the
-  average).  One device->host read of 2 + n doubles instead of the reference's n + 2 `.item()`s. """
+  average).  One device->host read of 2 + n doubles instead of the reference's n + 2 `.item()`s.
+  Up to MAX_N_COORDINATE samples; with `many`, up to MAX_N_MANY (`avg_dev_max_many_async`). """
   n = len(samples)
   if n == 0:
     return None, math.nan, math.nan, math.nan                 # :105-106
@@ -838,12 +867,12 @@ def compute_avg_dev_max(samples):
   if hit is not None:
     avg, a, b, c = hit
     return avg.clone(), a, b, c                               # callers own the average they get (grad_pasts keeps it)
-  result = _compute_avg_dev_max(samples, n)
+  result = _compute_avg_dev_max(samples, n, many)
   _study_memo.store("avg_dev_max", (), samples, (result[0].clone(),) + result[1:])
   return result
 
-def _compute_avg_dev_max(samples, n):
-  avg, stats = avg_dev_max_async(samples)
+def _compute_avg_dev_max(samples, n, many=False):
+  avg, stats = (avg_dev_max_many_async if many else avg_dev_max_async)(samples)
   return _study_tuple(avg, stats.tolist(), n)                 # the only synchronisation
 
 def _merge_ranks(parts, maxima):
@@ -914,7 +943,7 @@ class StudyPartials:
     ns, nh, na = self.counts
     return (1, 3 + ns) + ((5 + ns + nh,) if na else ()) + (self.vector.numel() - 1,)
 
-def study_partials(grad_sampleds, grad_honests, grad_attacks, grad_defense, pasts, backend=None):
+def study_partials(grad_sampleds, grad_honests, grad_attacks, grad_defense, pasts, backend=None, many=False):
   """ The device half of `study_step` on one shard of the columns (the whole vectors on one GPU):
   K6 over each list (the honest pass is skipped when `grad_honests` holds the very same tensors as
   `grad_sampleds`, attack.py:808 without momentum placement; none without attack gradients), three
@@ -922,10 +951,15 @@ def study_partials(grad_sampleds, grad_honests, grad_attacks, grad_defense, past
   Args:
     grad_sampleds, grad_honests, grad_attacks, grad_defense  As `study_step`, or this rank's columns of them
     pasts    Iterable of (gradient or its shard, norm of the WHOLE gradient), most recent first
-    backend  Provider of `avg_dev_max_async` and `rowdots_async` (default: this module)
+    backend  Provider of `avg_dev_max_async` and `rowdots_async` (default: this module), and of
+             `avg_dev_max_many_async` with `many`
+    many     K6 through `avg_dev_max_many_async`: lists of up to MAX_N_MANY gradients instead of MAX_N_COORDINATE
   Returns:
     StudyPartials """
-  avg_dev_max = avg_dev_max_async if backend is None else backend.avg_dev_max_async
+  if many:
+    avg_dev_max = avg_dev_max_many_async if backend is None else backend.avg_dev_max_many_async
+  else:
+    avg_dev_max = avg_dev_max_async if backend is None else backend.avg_dev_max_async
   rowdots = rowdots_async if backend is None else backend.rowdots_async
   pasts = list(pasts)
   ns, nh, na = len(grad_sampleds), len(grad_honests), len(grad_attacks)
@@ -1003,7 +1037,7 @@ def study_finish(partials, parts, momentum):
     out["curv_sampled"] = nan
   return out
 
-def study_step(grad_sampleds, grad_honests, grad_attacks, grad_defense, pasts, momentum):
+def study_step(grad_sampleds, grad_honests, grad_attacks, grad_defense, pasts, momentum, many=False):
   """ Everything attack.py:846-866 computes for one line of the study file, on the device:
     * the three `tools.compute_avg_dev_max` calls (K6, one pass each; a repeated list is computed once),
     * the norm and the largest |coordinate| of the defense gradient,
@@ -1017,9 +1051,10 @@ def study_step(grad_sampleds, grad_honests, grad_attacks, grad_defense, pasts, m
     grad_defense  The aggregated gradient
     pasts         Iterable of (gradient, norm) of the past sampled averages, most recent first
     momentum      args.momentum
+    many          Lists of up to MAX_N_MANY gradients (`avg_dev_max_many_async`) instead of MAX_N_COORDINATE
   Returns:
     dict with the reference's variable names (attack.py:846-866) """
-  partials = study_partials(grad_sampleds, grad_honests, grad_attacks, grad_defense, pasts)
+  partials = study_partials(grad_sampleds, grad_honests, grad_attacks, grad_defense, pasts, many=many)
   return study_finish(partials, [partials.vector.tolist()], momentum)            # the only synchronisation
 
 # ---------------------------------------------------------------------------- #

@@ -19,7 +19,8 @@ routes lead there without touching a reference file:
 (`engine.line_search`) when the rule they attack is one `install` registered, and, asked for by name, the
 attack against CGE run on the device (`engine.anticge`).  The search takes the rows the entry takes: up to
 128 against a wide entry, and against a default entry as many as `bz_line_search` takes
-(`engine.search_max_rows`).
+(`engine.search_max_rows`); with `install_attacks(..., many=True)`, up to 1024 against an entry of
+`install(..., many=True)`.
 """
 
 import math
@@ -32,6 +33,9 @@ __all__ = ["install", "install_tools", "install_attacks"]
 # rows the device search takes against it: the attacks replaced by `install_attacks` recognise the rule they
 # attack by identity.
 _installed = {}
+# The entries of `_installed` that `install` took from `gars.many_gars`: `install_attacks(..., many=True)` searches against
+# them up to MAX_N_MANY rows.
+_many_installed = set()
 
 def _record(aggregators, key, name, rule):
   from . import engine, _lib
@@ -39,6 +43,10 @@ def _record(aggregators, key, name, rule):
   if entry is not None and getattr(entry, "unchecked", None) is rule.unchecked:
     wide = wide_gars.get(name) is rule
     _installed[entry] = (name, _lib.MAX_N_DISTANCE if wide else engine.search_max_rows(name))
+    if many_gars.get(name) is rule:
+      _many_installed.add(entry)
+    else:
+      _many_installed.discard(entry)
 
 def install(aggregators, prefix="b200-", override=False, names=None, wide=False, many=False):
   """ Register the CUDA rules in the reference's `aggregators` module.
@@ -52,8 +60,9 @@ def install(aggregators, prefix="b200-", override=False, names=None, wide=False,
                  which stop at 64 gradients, as every earlier release did; the other six rules are the same
                  either way
     many         Register average, median, trmean, phocas and meamed from `gars.many_gars`: up to 1024 gradients.
-                 The attacks' device search against them keeps its 128 rows; above, the stock attack runs and calls
-                 the entry for each evaluation.  The default, False, keeps `gars`' entries, which stop at 128
+                 The attacks' device search against them keeps its 128 rows, unless `install_attacks(..., many=True)`
+                 takes it to 1024; above, the stock attack runs and calls the entry for each evaluation.  The default,
+                 False, keeps `gars`' entries, which stop at 128
   Returns:
     List of the registered names
   """
@@ -74,20 +83,22 @@ def install(aggregators, prefix="b200-", override=False, names=None, wide=False,
       done.append(target)
   return done
 
-def install_tools(tools):
+def install_tools(tools, many=False):
   """ Replace `tools.compute_avg_dev_max` (tools/pytorch.py:97, used by attack.py:846-848 for the
   study metrics) with the CUDA version when the samples live on a GPU.  CPU samples keep the
   reference's own function: this is a device kernel, not a CPU reimplementation.
   Args:
     tools  The imported reference `tools` package
+    many   Take up to 1024 CUDA samples on the device (`engine.compute_avg_dev_max(..., many=True)`) instead of 128
   Returns:
     The previous function
   """
   from . import engine, _lib
   stock = tools.compute_avg_dev_max
+  limit = _lib.MAX_N_MANY if many else _lib.MAX_N_COORDINATE
   def compute_avg_dev_max(samples):
-    if len(samples) > 0 and samples[0].is_cuda and len(samples) <= _lib.MAX_N_COORDINATE:
-      return engine.compute_avg_dev_max(samples)
+    if len(samples) > 0 and samples[0].is_cuda and len(samples) <= limit:
+      return engine.compute_avg_dev_max(samples, many=True) if many else engine.compute_avg_dev_max(samples)
     return stock(samples)
   compute_avg_dev_max.__doc__ = stock.__doc__
   tools.compute_avg_dev_max = compute_avg_dev_max
@@ -99,13 +110,14 @@ def install_tools(tools):
 def _is_cuda(tensors):
   return all(t.is_cuda for t in tensors)
 
-def _device_rule(defense, grad_honests, f_real, f_decl, model):
+def _device_rule(defense, grad_honests, f_real, f_decl, model, many=False):
   """ The name of the rule here that `defense` is, when the attack's search can run on the device:
   `defense` is an entry `install` registered, there are Byzantine rows to generate, every honest
   gradient is a float32 CUDA vector, the rule's input fits the search's row limit for that entry
-  (128 rows for a wide entry of `install(..., wide=True)`; otherwise `engine.search_max_rows`: 128 rows for
-  the coordinate-wise rules, 64 for the distance rules), and the rule accepts its parameters.  None
-  otherwise: the stock attack then runs (and fails, if it must, as it always did). """
+  (128 rows for a wide entry of `install(..., wide=True)`; with `many`, 1024 rows for an entry of
+  `install(..., many=True)`; otherwise `engine.search_max_rows`: 128 rows for the coordinate-wise rules, 64 for
+  the distance rules), and the rule accepts its parameters.  None otherwise: the stock attack then runs (and
+  fails, if it must, as it always did). """
   import torch
   try:
     installed = _installed.get(defense)
@@ -114,6 +126,9 @@ def _device_rule(defense, grad_honests, f_real, f_decl, model):
   if installed is None or not isinstance(f_real, int) or f_real < 1 or not isinstance(grad_honests, list) or not grad_honests:
     return None
   name, limit = installed
+  if many and defense in _many_installed:
+    from . import _lib
+    limit = _lib.MAX_N_MANY
   if len(grad_honests) + f_real > limit or not _is_cuda(grad_honests):
     return None
   if any(g.dtype != torch.float32 or g.dim() != 1 for g in grad_honests):
@@ -137,10 +152,18 @@ def _bulyan(grad_stck, grad_avg, target_idx=-1, **kwargs):
   grad_att[target_idx] = 1
   return grad_att
 
-def _identical(stock, direction, backend):
+def _search(backend, rule, grad_honests, f_real, *args, **kwargs):
+  """ `backend.line_search(rule, grad_honests, f_real, *args, **kwargs)`, with `many=True` above MAX_N_COORDINATE rows
+  (only an entry of `install(..., many=True)` gets there, through `install_attacks(..., many=True)`). """
+  from . import _lib
+  if len(grad_honests) + f_real > _lib.MAX_N_COORDINATE:
+    kwargs["many"] = True
+  return backend.line_search(rule, grad_honests, f_real, *args, **kwargs)
+
+def _identical(stock, direction, backend, many=False):
   """ attacks/identical.py:46-86 with the factor search on the device. """
   def attack(grad_honests, f_real, f_decl, defense, model, factor=-16, negative=False, **kwargs):
-    rule = _device_rule(defense, grad_honests, f_real, f_decl, model) if factor < 0 else None
+    rule = _device_rule(defense, grad_honests, f_real, f_decl, model, many) if factor < 0 else None
     if rule is None:
       return stock(grad_honests=grad_honests, f_real=f_real, f_decl=f_decl, defense=defense, model=model,
                    factor=factor, negative=negative, **kwargs)
@@ -148,15 +171,15 @@ def _identical(stock, direction, backend):
     grad_stck = torch.stack(grad_honests)
     grad_avg = grad_stck.mean(dim=0)
     grad_att = direction(grad_stck, grad_avg, **kwargs)
-    _, byz = backend.line_search(rule, grad_honests, f_real, f_decl, grad_avg, grad_att, math.ceil(-factor),
-                                 negative=negative, kind="identical")
+    _, byz = _search(backend, rule, grad_honests, f_real, f_decl, grad_avg, grad_att, math.ceil(-factor),
+                     negative=negative, kind="identical")
     return [byz] * f_real
   return attack
 
-def _empire_strict(stock, backend):
+def _empire_strict(stock, backend, many=False):
   """ attacks/empire.py:29-65 with the epsilon search on the device. """
   def attack(grad_honests, f_real, f_decl, defense, model, epsilon=1, **kwargs):
-    rule = _device_rule(defense, grad_honests, f_real, f_decl, model) if epsilon < 0 else None
+    rule = _device_rule(defense, grad_honests, f_real, f_decl, model, many) if epsilon < 0 else None
     if rule is None:
       return stock(grad_honests=grad_honests, f_real=f_real, f_decl=f_decl, defense=defense, model=model,
                    epsilon=epsilon, **kwargs)
@@ -164,7 +187,7 @@ def _empire_strict(stock, backend):
     for grad in grad_honests[1:]:
       grad_avg.add_(grad)
     grad_avg.div_(len(grad_honests))
-    _, byz = backend.line_search(rule, grad_honests, f_real, f_decl, grad_avg, None, math.ceil(-epsilon), kind="empire-strict")
+    _, byz = _search(backend, rule, grad_honests, f_real, f_decl, grad_avg, None, math.ceil(-epsilon), kind="empire-strict")
     return [byz] * f_real
   return attack
 
@@ -183,7 +206,7 @@ def _anticge(stock, backend):
 
 _ATTACK_NAMES = ("little", "empire", "bulyan", "empire-strict")
 
-def install_attacks(attacks, backend=None, names=None):
+def install_attacks(attacks, backend=None, names=None, many=False):
   """ Replace `little`, `empire`, `bulyan` and `empire-strict` in the reference's `attacks` registry
   (attacks/__init__.py: `attacks`, `register`) with versions that, when the factor (epsilon) is negative
   and `defense` is a rule `install` registered, run the whole `line_maximize` search on the device and
@@ -198,6 +221,8 @@ def install_attacks(attacks, backend=None, names=None):
     attacks  The imported reference `attacks` package
     backend  Provider of `line_search` and `anticge` (default: `engine`; tests substitute a stand-in)
     names    Attacks to replace (default: the four line-searching ones)
+    many     Against an entry of `install(..., many=True)`, search on the device up to 1024 rows, above 128 through
+             `backend.line_search(..., many=True)`.  The default, False, keeps the search at 128 rows there
   Returns:
     List of the replaced names """
   if backend is None:
@@ -211,9 +236,9 @@ def install_attacks(attacks, backend=None, names=None):
     if name == "anticge":
       attack = _anticge(stock.unchecked, backend)
     elif name == "empire-strict":
-      attack = _empire_strict(stock.unchecked, backend)
+      attack = _empire_strict(stock.unchecked, backend, many)
     elif name in directions:
-      attack = _identical(stock.unchecked, directions[name], backend)
+      attack = _identical(stock.unchecked, directions[name], backend, many)
     else:
       raise KeyError(f"no device version of the attack {name!r}")
     del attacks.attacks[name]                  # `register` refuses duplicates

@@ -474,12 +474,14 @@ class ShardedPlan:
 
 SEARCH_EXCHANGES = ("auto", "fused", "nccl")
 
-def search_rows(gar, wide=False):
+def search_rows(gar, wide=False, many=False):
   """ The most rows (honest + f_real) `ShardedLineSearch` takes against the rule `gar`: `engine.search_max_rows(gar)`,
-  and with `wide` MAX_N_DISTANCE for krum, bulyan, aksel and cge (brute stays at MAX_N, the coordinate-wise rules
-  at MAX_N_COORDINATE). """
+  with `wide` MAX_N_DISTANCE for krum, bulyan, aksel and cge (brute stays at MAX_N), and with `many` MAX_N_MANY for
+  the coordinate-wise rules (without it they stay at MAX_N_COORDINATE). """
   if wide and gar in _engine.WIDE_DISTANCE:
     return _lib.MAX_N_DISTANCE
+  if many and gar in COORDINATE_WISE:
+    return _lib.MAX_N_MANY
   return _engine.search_max_rows(gar)
 
 def choose_search_exchange(exchange, aligned, symmetric, engine, group=None):
@@ -685,11 +687,11 @@ class _SearchShard:
     blocks, part   [world, width] gathered partial blocks of the rule / this rank's block (blocks[0] on one rank)
     scores, score  [world] gathered score shares / this rank's share (scores[:1] on one rank)
   `fuse(fx)` prepares the stages of the fused exchange over the FusedExchange `fx` as well. """
-  def __init__(self, gar, grad_honests, f_real, f_decl, grad_avg, grad_att, evals, negative, kind, world, wide=False):
+  def __init__(self, gar, grad_honests, f_real, f_decl, grad_avg, grad_att, evals, negative, kind, world, wide=False, many=False):
     honest = list(grad_honests)
     f_real = int(f_real)
     n = len(honest) + f_real
-    limit = search_rows(gar, wide)
+    limit = search_rows(gar, wide, many)
     if f_real < 1 or n > limit:
       raise ValueError(f"f_real = {f_real} with {len(honest)} honest rows: expected f_real >= 1 and at most {limit} rows")
     prep = _engine._prepare_device(honest, "the line search takes CUDA tensors", limit=limit)
@@ -972,13 +974,20 @@ class ShardedLineSearch:
             the block in `bz_distance_select_peers` (libbyzagg_peers.so, rows of any alignment), 2 exchanges per
             evaluation; "auto" resolves to "nccl" there (`search_exchange`).  A stand-in backend gets
             `wide=True` as a keyword after its 10 arguments.
+  many:     False (default): the coordinate-wise rules up to MAX_N_COORDINATE rows, as before.  True: up to MAX_N_MANY
+            (`search_rows`); above MAX_N_COORDINATE rows the rule is `bz_coordinate_many` (`engine._coordinate_call`),
+            and the trace, the factor and `byz` on one rank are those of `engine.LineSearch(..., many=True)`.  The
+            fused exchange carries only the score's share for these rules, at any n.  The distance rules raise
+            ValueError.  A stand-in backend gets `many=True` as a keyword after its 10 arguments.
   `graph()` captures the whole search in a CUDA graph, as `engine.LineSearch.graph()` does: "fused" on any
   number of ranks, "nccl" on one rank (no collective).  Like a search, `graph()` and every replay are
   collective: every rank issues them at the same point of its stream order. """
   def __init__(self, gar, grad_honests, f_real, f_decl, grad_avg, grad_att, evals, negative=False, kind="identical",
-               group=None, backend=None, exchange="auto", wide=False):
+               group=None, backend=None, exchange="auto", wide=False, many=False):
     if gar not in _engine._SEARCH_RULES:
       raise KeyError(f"unknown aggregation rule {gar!r}")
+    if many and gar not in COORDINATE_WISE:
+      raise ValueError(f"many=True takes the coordinate-wise rules {list(COORDINATE_WISE)}, not {gar!r}")
     if kind not in _engine._SEARCH_KINDS:
       raise ValueError(f"unknown attack kind {kind!r}, expected one of {sorted(_engine._SEARCH_KINDS)}")
     if int(evals) < 1:
@@ -991,7 +1000,7 @@ class ShardedLineSearch:
                                     _symmetric_memory_importable(), backend is None, group, wide)
     make = _SearchShard if backend is None else backend.search_shard
     self._backend, self._graph = backend, None
-    extra = {"wide": True} if wide else {}
+    extra = dict({"wide": True} if wide else {}, **({"many": True} if many else {}))
     self._shard = make(gar, honest, f_real, f_decl, grad_avg, grad_att, self.evals, negative, kind, self.world, **extra)
     self.byz, self.record = self._shard.byz, self._shard.record
     if self.exchange == "fused":
@@ -1059,12 +1068,12 @@ class ShardedLineSearch:
     return _engine._search_outcome(self.record, self.evals)
 
 def line_search(gar, grad_honests, f_real, f_decl, grad_avg, grad_att, evals, negative=False, kind="identical", group=None,
-                exchange="auto", wide=False):
-  """ `engine.line_search` on a d-sharded trainer (see `ShardedLineSearch`, and its `wide` for krum, bulyan, aksel
-  and cge above MAX_N rows): returns (factor, this rank's shard of the Byzantine gradient), the factor the same
-  Python float on every rank. """
+                exchange="auto", wide=False, many=False):
+  """ `engine.line_search` on a d-sharded trainer (see `ShardedLineSearch`, its `wide` for krum, bulyan, aksel
+  and cge above MAX_N rows and its `many` for the coordinate-wise rules above MAX_N_COORDINATE rows): returns (factor,
+  this rank's shard of the Byzantine gradient), the factor the same Python float on every rank. """
   search = ShardedLineSearch(gar, grad_honests, f_real, f_decl, grad_avg, grad_att, evals, negative, kind, group,
-                             exchange=exchange, wide=wide)
+                             exchange=exchange, wide=wide, many=many)
   byz = search()
   factor, _ = search.result()
   return factor, byz
@@ -1216,12 +1225,12 @@ def aggregate(gar, gradients, f=None, m=None, mode="mid", group=None, backend=No
   out, sel = _phases(be, gar, gradients, f, m, mode, group, False)
   return (out, sel) if return_selection else out
 
-def compute_avg_dev_max(samples, group=None, backend=None):
+def compute_avg_dev_max(samples, group=None, backend=None, many=False):
   """ `tools.compute_avg_dev_max` (tools/pytorch.py:97-125) over d-sharded samples: every rank
   passes its columns of the n samples and gets its shard of the average plus the GLOBAL scalars.
   One pass over the local shard (`avg_dev_max_async`), then ONE all-gather of 2 + n doubles; the
   sums of squares are added in rank order and the maxima compared, so every rank returns
-  bitwise the same three numbers.
+  bitwise the same three numbers.  With `many`, up to MAX_N_MANY samples (`avg_dev_max_many_async`).
   Returns:
     (this rank's shard of the average or None, norm of the average, norm standard deviation,
      max |coordinate| of the average)
@@ -1230,11 +1239,11 @@ def compute_avg_dev_max(samples, group=None, backend=None):
   n = len(samples)
   if n == 0:
     return None, math.nan, math.nan, math.nan
-  avg, stats = be.avg_dev_max_async(samples)
+  avg, stats = be.avg_dev_max_many_async(samples) if many else be.avg_dev_max_async(samples)
   gathered = _gather(stats, group).tolist()            # [R][2 + n]; the only synchronisation
   return _engine._study_tuple(avg, _engine._merge_ranks(gathered, (1,)), n)      # fp32 overflow rule after the sums
 
-def study_step(grad_sampleds, grad_honests, grad_attacks, grad_defense, pasts, momentum, group=None, backend=None):
+def study_step(grad_sampleds, grad_honests, grad_attacks, grad_defense, pasts, momentum, group=None, backend=None, many=False):
   """ `engine.study_step` (attack.py:846-866) over d-sharded vectors: every rank passes its columns
   and gets its shards of the three averages plus the GLOBAL scalars, bitwise the same on every rank.
   One `engine.study_partials` pass over the local shard, then ONE all-gather of its fp64 vector
@@ -1250,11 +1259,13 @@ def study_step(grad_sampleds, grad_honests, grad_attacks, grad_defense, pasts, m
               first: (`sampled_grad_avg`, `sampled_norm_avg`) of an earlier call
     momentum  args.momentum
     group     Process group (default: the world)
-    backend   Provider of `avg_dev_max_async` and `rowdots_async` (default: the CUDA engine)
+    backend   Provider of `avg_dev_max_async` and `rowdots_async` (default: the CUDA engine), and of
+              `avg_dev_max_many_async` with `many`
+    many      Lists of up to MAX_N_MANY gradients (`avg_dev_max_many_async`) instead of MAX_N_COORDINATE
   Returns:
     dict with the reference's variable names
   """
-  partials = _engine.study_partials(grad_sampleds, grad_honests, grad_attacks, grad_defense, pasts, backend=backend)
+  partials = _engine.study_partials(grad_sampleds, grad_honests, grad_attacks, grad_defense, pasts, backend=backend, many=many)
   return _engine.study_finish(partials, _gather(partials.vector, group).tolist(), momentum)    # the only synchronisation
 
 def replicate(shard, group=None):
