@@ -18,8 +18,8 @@ its absence is an error (no CPU fallback).
 """
 
 from . import _lib, engine, gars as _gars, hostmem, plugin, sharded
-from .gars import gars, wide_gars, many_gars, make_gar, register, UserException, last_selection
+from .gars import gars, wide_gars, many_gars, many_distance_gars, make_gar, register, UserException, last_selection
 from .engine import config, Plan, compute_avg_dev_max, GradientStack
 
-__all__ = ["gars", "wide_gars", "many_gars", "make_gar", "register", "UserException", "last_selection", "config", "Plan", "GradientStack", "compute_avg_dev_max", "engine", "hostmem", "plugin", "sharded"]
+__all__ = ["gars", "wide_gars", "many_gars", "many_distance_gars", "make_gar", "register", "UserException", "last_selection", "config", "Plan", "GradientStack", "compute_avg_dev_max", "engine", "hostmem", "plugin", "sharded"]
 __version__ = "0.1.0"

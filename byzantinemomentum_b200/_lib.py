@@ -7,7 +7,9 @@
 second library `libbyzagg_peers.so` built next to it (C ABI: `include/byzagg_distance_peers.h`) and of the third,
 `libbyzagg_star.so` (C ABI: `include/byzagg_rowshare_star.h`), which the callers compose with the first through their
 C ABIs, of the fourth, `libbyzagg_many.so` (C ABI: `include/byzagg_coordinate_many.h`), which links against the first, and of
-the fifth, `libbyzagg_many_tools.so` (C ABI: `include/byzagg_many_tools.h`), which links against the first and the fourth.
+the fifth, `libbyzagg_many_tools.so` (C ABI: `include/byzagg_many_tools.h`), which links against the first and the fourth,
+and of the sixth, `libbyzagg_many_distance.so` (C ABI: `include/byzagg_distance_many.h`), which links against the first and
+the fourth.
 
 Each library is loaded lazily, on the first call that needs it, and the load FAILS LOUDLY:
 there is no CPU or PyTorch fallback anywhere in this package.  Build it in-tree with
@@ -19,8 +21,8 @@ import os
 import pathlib
 import threading
 
-__all__ = ["lib", "peers_lib", "star_lib", "many_lib", "many_tools_lib", "LibraryError", "library_path", "peers_library_path",
-           "star_library_path", "many_library_path", "many_tools_library_path", "check", "MAX_N", "MAX_N_COORDINATE", "MAX_N_MANY", "MAX_N_DISTANCE", "STATUS_MESSAGES",
+__all__ = ["lib", "peers_lib", "star_lib", "many_lib", "many_tools_lib", "many_distance_lib", "LibraryError", "library_path",
+           "peers_library_path", "star_library_path", "many_library_path", "many_tools_library_path", "many_distance_library_path", "check", "MAX_N", "MAX_N_COORDINATE", "MAX_N_MANY", "MAX_N_DISTANCE", "STATUS_MESSAGES",
            "AKSEL_MODES", "STATUS_NO_FINITE_SET", "STATUS_DEGENERATE"]
 
 MAX_N = 64
@@ -73,6 +75,13 @@ def many_tools_library_path():
   if override:
     return pathlib.Path(override)
   return library_path().parent / "libbyzagg_many_tools.so"
+
+def many_distance_library_path():
+  """ libbyzagg_many_distance.so: next to libbyzagg.so, or where BYZAGG_MANY_DISTANCE_LIBRARY says. """
+  override = os.environ.get("BYZAGG_MANY_DISTANCE_LIBRARY")
+  if override:
+    return pathlib.Path(override)
+  return library_path().parent / "libbyzagg_many_distance.so"
 
 _c_rows = ctypes.POINTER(ctypes.c_void_p)
 _vp, _i, _i64, _sz, _dbl = ctypes.c_void_p, ctypes.c_int, ctypes.c_int64, ctypes.c_size_t, ctypes.c_double
@@ -171,6 +180,13 @@ MANY_TOOLS_SIGNATURES = {
   "bz_line_search_many_workspace_bytes": (_sz, [_i]),
   "bz_line_search_many": (_i, [_i, _c_rows, _i, _i, _i, _i, _i, _vp, _vp, _i64, _i, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
 }
+# the same for include/byzagg_distance_many.h, the table of the sixth library (`many_distance_lib()`): Multi-Krum, Bulyan,
+# Aksel and CGE up to MAX_N_MANY rows
+MANY_DISTANCE_SIGNATURES = {
+  "bz_distance_many_last_error": (ctypes.c_char_p, []),
+  "bz_distance_many_workspace_bytes": (_sz, [_i]),
+  "bz_distance_many": (_i, [_i, _c_rows, _i, _i, _i, _i, _i64, _vp, _vp, _vp, _vp, _sz, _vp]),
+}
 # the same for include/byzagg_distance.h (Multi-Krum, Bulyan, Aksel and CGE up to MAX_N_DISTANCE rows)
 DISTANCE_SIGNATURES = {
   "bz_distance_workspace_bytes": (_sz, [_i]),
@@ -229,6 +245,7 @@ _peers_lib = None
 _star_lib = None
 _many_lib = None
 _many_tools_lib = None
+_many_distance_lib = None
 
 def _load(path, tables):
   """ The library at `path` with the signatures of `tables` bound; LibraryError when it is missing or stale. """
@@ -303,6 +320,17 @@ def many_tools_lib():
       _many_tools_lib = _load(many_tools_library_path(), (MANY_TOOLS_SIGNATURES,))
   return _many_tools_lib
 
+def many_distance_lib():
+  """ The sixth library, libbyzagg_many_distance.so (loads it on first use; no fallback when it is missing). """
+  global _many_distance_lib
+  if _many_distance_lib is not None:
+    return _many_distance_lib
+  many_lib()                     # libbyzagg.so and libbyzagg_many.so first: the sixth library links against both
+  with _lock:
+    if _many_distance_lib is None:
+      _many_distance_lib = _load(many_distance_library_path(), (MANY_DISTANCE_SIGNATURES,))
+  return _many_distance_lib
+
 def check(code, what):
   """ Raise on a non-zero return code of a bz_* call. """
   if code == 0:
@@ -316,6 +344,8 @@ def check(code, what):
     message = many_lib().bz_coordinate_many_last_error()
   elif what in MANY_TOOLS_SIGNATURES:
     message = many_tools_lib().bz_many_tools_last_error()
+  elif what in MANY_DISTANCE_SIGNATURES:
+    message = many_distance_lib().bz_distance_many_last_error()
   else:
     message = lib().bz_last_error()
   message = message.decode("utf-8", "replace") if message else ""

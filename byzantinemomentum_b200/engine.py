@@ -26,7 +26,7 @@ __all__ = ["average", "median", "trmean", "phocas", "meamed", "coordinate_many",
            "pairdist_partial", "rowdist_partial", "select", "krum_select", "bulyan_select", "brute_select",
            "rowdist_select", "average_selected", "bulyan_reduce", "avg_dev_max_async", "avg_dev_max_many_async", "compute_avg_dev_max", "rowdots_async", "study_step",
            "StudyPartials", "study_partials", "study_finish",
-           "wide_distance", "LineSearch", "line_search", "AntiCGE", "anticge", "config", "Plan", "pair_cache_stats", "GradientStack", "gradient_scatter", "momentum_rows", "host_path_report"]
+           "wide_distance", "distance_many", "LineSearch", "line_search", "AntiCGE", "anticge", "config", "Plan", "pair_cache_stats", "GradientStack", "gradient_scatter", "momentum_rows", "host_path_report"]
 
 class _Config:
   """ strict_status: after brute / bulyan, read the device status word (one 4-byte D2H copy,
@@ -51,21 +51,25 @@ class _Prepared:
 
 _workspaces = {}
 _wide_workspaces = {}
+_many_workspaces = {}
 _staging = {}
 
 _MAX_WORKSPACES = 16
 
-def _workspace(device, stream, wide=False):
+def _workspace(device, stream, wide=False, many=False):
   """ One scratch buffer per (device, stream), sized for MAX_N (~10 MB), or with `wide` for `bz_distance` up to
-  MAX_N_DISTANCE rows (~11 MB, kept apart).  At most `_MAX_WORKSPACES` of each are kept (least recently used
-  dropped; the caching allocator keeps a dropped buffer alive until the launches already queued on its stream
-  have run). """
-  cache = _wide_workspaces if wide else _workspaces
+  MAX_N_DISTANCE rows (~11 MB), or with `many` for `bz_distance_many` up to MAX_N_MANY rows (~21 MB), each kind kept
+  apart.  At most `_MAX_WORKSPACES` of each are kept (least recently used dropped; the caching allocator keeps a
+  dropped buffer alive until the launches already queued on its stream have run). """
+  cache = _many_workspaces if many else _wide_workspaces if wide else _workspaces
   key = (device.index, stream)
   ws = cache.pop(key, None)
   if ws is None:
     lib = _lib.lib()
-    nbytes = int(lib.bz_distance_workspace_bytes(_lib.MAX_N_DISTANCE) if wide else lib.bz_workspace_bytes(_lib.MAX_N))
+    if many:
+      nbytes = int(_lib.many_distance_lib().bz_distance_many_workspace_bytes(_lib.MAX_N_MANY))
+    else:
+      nbytes = int(lib.bz_distance_workspace_bytes(_lib.MAX_N_DISTANCE) if wide else lib.bz_workspace_bytes(_lib.MAX_N))
     ws = torch.empty(nbytes, dtype=torch.uint8, device=device)
     while len(cache) >= _MAX_WORKSPACES:
       cache.pop(next(iter(cache)))
@@ -522,7 +526,8 @@ def pair_cache_stats(device_index=None):
 # phases of the d-sharded path
 
 DISTANCE_BASED = ("krum", "bulyan", "brute", "aksel", "cge")
-WIDE_DISTANCE = ("krum", "bulyan", "aksel", "cge")        # `Plan` takes them up to MAX_N_DISTANCE rows (bz_distance)
+WIDE_DISTANCE = ("krum", "bulyan", "aksel", "cge")        # `Plan` takes them up to MAX_N_DISTANCE rows (bz_distance),
+                                                          # with `many` up to MAX_N_MANY (bz_distance_many)
 
 class _Rule:
   """ The facts of a distance-based rule for (gar, n, f, m, mode):
@@ -564,6 +569,11 @@ class _Rule:
     status = meta + 4 * self.n if self.status else None
     return _lib.lib().bz_distance, (_SEARCH_RULES[self.gar], ptrs, self.n, self.f, m, mode, d, out, meta, status,
                                     ws.data_ptr(), ws.numel(), stream)
+  def many_entry(self, ptrs, d, out, meta, ws, stream):
+    """ `wide_entry` through `bz_distance_many` (libbyzagg_many_distance.so), which takes krum, bulyan, aksel and cge
+    up to MAX_N_MANY rows and makes `bz_distance`'s call up to MAX_N_DISTANCE. """
+    _, args = self.wide_entry(ptrs, d, out, meta, ws, stream)
+    return _lib.many_distance_lib().bz_distance_many, args
   def phase_entries(self, ptrs, d, center, part, blocks, nparts, out, meta, ws, stream):
     """ The three (fn, args) of the d-sharded phases through `bz_distance_partial`, `bz_distance_select` and
     `bz_distance_reduce`, which take every rule up to MAX_N_DISTANCE rows (brute: MAX_N): phase A of this
@@ -622,6 +632,26 @@ def wide_distance(gar, gradients, f, m=None, mode="mid"):
   ws = _workspace(prep.device, prep.stream, wide=True)
   meta = torch.empty(prep.n + 1, dtype=torch.int32, device=prep.device)   # order[n] + status
   _run(prep.device, *rule.wide_entry(prep.ptrs, prep.d, out.data_ptr(), meta.data_ptr(), ws, prep.stream))
+  if rule.status and config.strict_status:
+    _raise_status(int(meta[prep.n].item()))
+  return _finish(prep, out), meta[:rule.length]
+
+def distance_many(gar, gradients, f, m=None, mode="mid"):
+  """ `wide_distance` for krum, bulyan, aksel and cge over 1 to MAX_N_MANY rows: up to MAX_N_DISTANCE exactly
+  `wide_distance`'s call, above it `bz_distance_many` (libbyzagg_many_distance.so) with a per-(device, stream)
+  workspace.  With `config.strict_status` Bulyan's status is raised as `wide_distance` raises it.  Host rows are
+  staged per row and give a host vector.  Returns (out, selection) as `wide_distance` does. """
+  if gar not in WIDE_DISTANCE:
+    raise KeyError(f"{gar!r} is not one of {WIDE_DISTANCE}")
+  n = len(gradients) if isinstance(gradients, (list, tuple)) else 0
+  if n <= _lib.MAX_N_DISTANCE:
+    return wide_distance(gar, gradients, f, m, mode)
+  rule = _rule(gar, n, f, m, mode)
+  prep = _prepare(gradients, limit=_lib.MAX_N_MANY)
+  out = torch.empty(prep.d, dtype=torch.float32, device=prep.device)
+  ws = _workspace(prep.device, prep.stream, many=True)
+  meta = torch.empty(prep.n + 1, dtype=torch.int32, device=prep.device)   # order[n] + status
+  _run(prep.device, *rule.many_entry(prep.ptrs, prep.d, out.data_ptr(), meta.data_ptr(), ws, prep.stream))
   if rule.status and config.strict_status:
     _raise_status(int(meta[prep.n].item()))
   return _finish(prep, out), meta[:rule.length]
@@ -1310,12 +1340,15 @@ class Plan:
       aggregated = plan()          # same tensor every time: plan.out
       plan.selection               # device int32 (distance-based rules)
   Up to MAX_N_MANY rows for the coordinate-wise rules (above MAX_N_COORDINATE through `bz_coordinate_many`), MAX_N_DISTANCE for krum, bulyan, aksel and cge
-  (above MAX_N through `bz_distance`, with a workspace of its own), MAX_N for brute.
+  (above MAX_N through `bz_distance`, with a workspace of its own), MAX_N for brute.  With `many`, krum, bulyan, aksel
+  and cge take up to MAX_N_MANY rows: above MAX_N_DISTANCE through `bz_distance_many`, with a workspace held by the
+  plan; up to MAX_N_DISTANCE, and for the other rules, `many` changes nothing.
   For brute / bulyan the device status word is NOT checked here (that would synchronise);
   read `plan.status` when needed: non-zero means the rule is undefined on this data and `out`
   is NaN. """
-  def __init__(self, gar, gradients, f=None, m=None, mode="mid", out=None):
-    limit = _lib.MAX_N_MANY if gar in _RULE_CODES else _lib.MAX_N_DISTANCE if gar in WIDE_DISTANCE else _lib.MAX_N
+  def __init__(self, gar, gradients, f=None, m=None, mode="mid", out=None, many=False):
+    many = many and gar in WIDE_DISTANCE
+    limit = _lib.MAX_N_MANY if gar in _RULE_CODES or many else _lib.MAX_N_DISTANCE if gar in WIDE_DISTANCE else _lib.MAX_N
     prep = _prepare(list(gradients), limit=limit)
     if prep.to_cpu:
       raise ValueError("Plan takes CUDA tensors (host tensors go through the plain call, which stages them)")
@@ -1337,7 +1370,12 @@ class Plan:
       self.selection = self._meta[:rule.length]
       if rule.status:
         self.status = self._meta[n:]
-      if n > _lib.MAX_N:
+      if n > _lib.MAX_N_DISTANCE:
+        # the tables and blocks of bz_distance_many, held by the plan
+        self._ws = torch.empty(int(_lib.many_distance_lib().bz_distance_many_workspace_bytes(n)), dtype=torch.uint8,
+                               device=prep.device)
+        fn, args = rule.many_entry(prep.ptrs, d, self.out.data_ptr(), self._meta.data_ptr(), self._ws, prep.stream)
+      elif n > _lib.MAX_N:
         # the pass tables of bz_distance, held by the plan: the per-stream workspace stays at its 64-row size
         self._ws = torch.empty(int(_lib.lib().bz_distance_workspace_bytes(n)), dtype=torch.uint8, device=prep.device)
         fn, args = rule.wide_entry(prep.ptrs, d, self.out.data_ptr(), self._meta.data_ptr(), self._ws, prep.stream)

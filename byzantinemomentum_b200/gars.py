@@ -11,6 +11,9 @@ names (average, median, trmean, phocas, meamed, krum, bulyan, brute, aksel, cge)
 `bz_distance`.  `plugin.install(..., wide=True)` registers them.  `many_gars` holds the five coordinate-wise
 rules again, for 1 to 1024 gradients (`BZ_MAX_N_MANY`): up to 128 they make exactly the call of their `gars`
 entry, above it they run `bz_coordinate_many`.  `plugin.install(..., many=True)` registers them.
+`many_distance_gars` holds krum, bulyan, aksel and cge once more, for 1 to 1024 gradients: up to 128 they make
+exactly the call of their `wide_gars` entry, above it they run `bz_distance_many`.
+`plugin.install(..., many_distance=True)` registers them.
 The arithmetic runs in `libbyzagg.so` (see `engine.py`); this module only holds the
 argument checks, the closed-form bounds and the selection bookkeeping for `influence`.
 
@@ -29,7 +32,7 @@ import math
 from . import _lib, engine
 from .engine import _Memo as _Selection, _rule
 
-__all__ = ["gars", "wide_gars", "many_gars", "make_gar", "register", "UserException", "last_selection"]
+__all__ = ["gars", "wide_gars", "many_gars", "many_distance_gars", "make_gar", "register", "UserException", "last_selection"]
 
 class UserException(RuntimeError):
   """ Raised by `checked` on invalid parameters (the reference raises tools.UserException). """
@@ -286,3 +289,31 @@ def _many(name):
   return make_gar(unchecked, narrow.check, upper_bound=narrow.upper_bound, influence=narrow.influence, name=name)
 
 many_gars = {name: _many(name) for name in ("average", "median", "trmean", "phocas", "meamed")}
+
+# ---------------------------------------------------------------------------- #
+# Multi-Krum, Bulyan, Aksel and CGE for up to 1024 gradients
+
+def _many_distance(name):
+  """ The `many_distance_gars` entry of `name`: the check, bound and influence of `gars[name]`; up to MAX_N_DISTANCE
+  gradients the call of `wide_gars[name]`, above it `engine.distance_many` (`bz_distance_many`), which stores the
+  selection for `influence` as `_wide` does. """
+  narrow, wide = gars[name], wide_gars[name]
+  def unchecked(gradients, f, m=None, mode="mid", **kwargs):
+    if not isinstance(gradients, list) or len(gradients) <= _lib.MAX_N_DISTANCE:
+      return wide.unchecked(gradients=gradients, f=f, m=m, mode=mode, **kwargs)
+    out, order = engine.distance_many(name, gradients, f, m if name in ("krum", "bulyan") else None,
+                                      mode if name == "aksel" else "mid")
+    if name != "bulyan":
+      _last.store(name, (f,) if name == "krum" else (), gradients, order)
+    return out
+  unchecked.__name__ = narrow.unchecked.__name__
+  influence = None
+  if narrow.influence is not None:
+    def influence(honests, attacks, f, m=None, mode="mid", **kwargs):
+      gradients = honests + attacks
+      if len(gradients) > _lib.MAX_N and _last.lookup(name, (f,) if name == "krum" else (), gradients) is None:
+        unchecked(gradients=gradients, f=f, m=m, mode=mode)
+      return narrow.influence(honests, attacks, f=f, m=m, mode=mode, **kwargs)
+  return make_gar(unchecked, narrow.check, upper_bound=narrow.upper_bound, influence=influence, name=name)
+
+many_distance_gars = {name: _many_distance(name) for name in engine.WIDE_DISTANCE}

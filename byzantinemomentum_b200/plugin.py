@@ -10,7 +10,8 @@ routes lead there without touching a reference file:
      `override=True` (`register` refuses duplicates, :82-84, so the entry is rebuilt with the
      reference's `make_gar`).  With `wide=True` it registers krum, bulyan, aksel and cge from
      `gars.wide_gars`, which take up to 128 gradients instead of 64; with `many=True`, average, median,
-     trmean, phocas and meamed from `gars.many_gars`, which take up to 1024 gradients instead of 128.
+     trmean, phocas and meamed from `gars.many_gars`, which take up to 1024 gradients instead of 128; with
+     `many_distance=True`, krum, bulyan, aksel and cge from `gars.many_distance_gars`, which take up to 1024.
   2. the top-level `native` package of this repository: the reference already looks for
      `native.{median,krum,bulyan,brute}.aggregate` and registers `native-<name>` when it finds
      them (median.py:80-87, krum.py:159-166, bulyan.py:137-144, brute.py:149-156).
@@ -25,7 +26,7 @@ attack against CGE run on the device (`engine.anticge`).  The search takes the r
 
 import math
 
-from .gars import gars, wide_gars, many_gars
+from .gars import gars, wide_gars, many_gars, many_distance_gars
 
 __all__ = ["install", "install_tools", "install_attacks"]
 
@@ -41,14 +42,15 @@ def _record(aggregators, key, name, rule):
   from . import engine, _lib
   entry = aggregators.gars.get(key)
   if entry is not None and getattr(entry, "unchecked", None) is rule.unchecked:
-    wide = wide_gars.get(name) is rule
+    # a many_distance entry is its wide entry up to 128 rows, where the device search stops against it
+    wide = wide_gars.get(name) is rule or many_distance_gars.get(name) is rule
     _installed[entry] = (name, _lib.MAX_N_DISTANCE if wide else engine.search_max_rows(name))
     if many_gars.get(name) is rule:
       _many_installed.add(entry)
     else:
       _many_installed.discard(entry)
 
-def install(aggregators, prefix="b200-", override=False, names=None, wide=False, many=False):
+def install(aggregators, prefix="b200-", override=False, names=None, wide=False, many=False, many_distance=False):
   """ Register the CUDA rules in the reference's `aggregators` module.
   Args:
     aggregators  The imported reference package (duck-typed: needs `gars`, `register`, `make_gar`)
@@ -63,12 +65,20 @@ def install(aggregators, prefix="b200-", override=False, names=None, wide=False,
                  The attacks' device search against them keeps its 128 rows, unless `install_attacks(..., many=True)`
                  takes it to 1024; above, the stock attack runs and calls the entry for each evaluation.  The default,
                  False, keeps `gars`' entries, which stop at 128
+    many_distance  Register krum, bulyan, aksel and cge from `gars.many_distance_gars`: up to 1024 gradients.  The
+                 attacks' device search against them stops at 128 rows, as against a wide entry; above, the stock
+                 attack runs and calls the entry for each evaluation.  Combines with `many`, not with `wide`
   Returns:
     List of the registered names
   """
+  if wide and many_distance:
+    raise ValueError("install takes wide=True or many_distance=True, not both: both register krum, bulyan, aksel and cge")
   done = []
   for name in (names or gars.keys()):
-    rule = wide_gars[name] if wide and name in wide_gars else many_gars[name] if many and name in many_gars else gars[name]
+    if many_distance and name in many_distance_gars:
+      rule = many_distance_gars[name]
+    else:
+      rule = wide_gars[name] if wide and name in wide_gars else many_gars[name] if many and name in many_gars else gars[name]
     if override:
       wrapped = aggregators.make_gar(rule.unchecked, rule.check, upper_bound=rule.upper_bound, influence=rule.influence)
       aggregators.gars[name] = wrapped
