@@ -8,8 +8,10 @@ second library `libbyzagg_peers.so` built next to it (C ABI: `include/byzagg_dis
 `libbyzagg_star.so` (C ABI: `include/byzagg_rowshare_star.h`), which the callers compose with the first through their
 C ABIs, of the fourth, `libbyzagg_many.so` (C ABI: `include/byzagg_coordinate_many.h`), which links against the first, and of
 the fifth, `libbyzagg_many_tools.so` (C ABI: `include/byzagg_many_tools.h`), which links against the first and the fourth,
-and of the sixth, `libbyzagg_many_distance.so` (C ABI: `include/byzagg_distance_many.h`), which links against the first and
-the fourth.
+of the sixth, `libbyzagg_many_distance.so` (C ABI: `include/byzagg_distance_many.h` and
+`include/byzagg_distance_many_table.h`), which links against the first and the fourth, and of the seventh,
+`libbyzagg_many_search.so` (C ABI: `include/byzagg_distance_search_many.h`), which links against the first, the fourth and
+the sixth.
 
 Each library is loaded lazily, on the first call that needs it, and the load FAILS LOUDLY:
 there is no CPU or PyTorch fallback anywhere in this package.  Build it in-tree with
@@ -21,8 +23,8 @@ import os
 import pathlib
 import threading
 
-__all__ = ["lib", "peers_lib", "star_lib", "many_lib", "many_tools_lib", "many_distance_lib", "LibraryError", "library_path",
-           "peers_library_path", "star_library_path", "many_library_path", "many_tools_library_path", "many_distance_library_path", "check", "MAX_N", "MAX_N_COORDINATE", "MAX_N_MANY", "MAX_N_DISTANCE", "STATUS_MESSAGES",
+__all__ = ["lib", "peers_lib", "star_lib", "many_lib", "many_tools_lib", "many_distance_lib", "many_search_lib", "LibraryError", "library_path",
+           "peers_library_path", "star_library_path", "many_library_path", "many_tools_library_path", "many_distance_library_path", "many_search_library_path", "check", "MAX_N", "MAX_N_COORDINATE", "MAX_N_MANY", "MAX_N_DISTANCE", "STATUS_MESSAGES",
            "AKSEL_MODES", "STATUS_NO_FINITE_SET", "STATUS_DEGENERATE"]
 
 MAX_N = 64
@@ -82,6 +84,13 @@ def many_distance_library_path():
   if override:
     return pathlib.Path(override)
   return library_path().parent / "libbyzagg_many_distance.so"
+
+def many_search_library_path():
+  """ libbyzagg_many_search.so: next to libbyzagg.so, or where BYZAGG_MANY_SEARCH_LIBRARY says. """
+  override = os.environ.get("BYZAGG_MANY_SEARCH_LIBRARY")
+  if override:
+    return pathlib.Path(override)
+  return library_path().parent / "libbyzagg_many_search.so"
 
 _c_rows = ctypes.POINTER(ctypes.c_void_p)
 _vp, _i, _i64, _sz, _dbl = ctypes.c_void_p, ctypes.c_int, ctypes.c_int64, ctypes.c_size_t, ctypes.c_double
@@ -187,6 +196,18 @@ MANY_DISTANCE_SIGNATURES = {
   "bz_distance_many_workspace_bytes": (_sz, [_i]),
   "bz_distance_many": (_i, [_i, _c_rows, _i, _i, _i, _i, _i64, _vp, _vp, _vp, _vp, _sz, _vp]),
 }
+# the same for include/byzagg_distance_many_table.h, also in the sixth library: the selection and reduce of Multi-Krum and
+# Bulyan from the distance table `bz_distance_many` leaves in its workspace
+MANY_DISTANCE_TABLE_SIGNATURES = {
+  "bz_distance_many_select": (_i, [_i, _c_rows, _i, _i, _i, _i64, _vp, _vp, _vp, _vp, _sz, _vp]),
+}
+# the same for include/byzagg_distance_search_many.h, the table of the seventh library (`many_search_lib()`): the line
+# search against Multi-Krum, Bulyan, Aksel and CGE up to MAX_N_MANY rows
+MANY_SEARCH_SIGNATURES = {
+  "bz_distance_line_search_many_last_error": (ctypes.c_char_p, []),
+  "bz_distance_line_search_many_workspace_bytes": (_sz, [_i]),
+  "bz_distance_line_search_many": (_i, [_i, _c_rows, _i, _i, _i, _i, _i, _vp, _vp, _i64, _i, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+}
 # the same for include/byzagg_distance.h (Multi-Krum, Bulyan, Aksel and CGE up to MAX_N_DISTANCE rows)
 DISTANCE_SIGNATURES = {
   "bz_distance_workspace_bytes": (_sz, [_i]),
@@ -246,6 +267,7 @@ _star_lib = None
 _many_lib = None
 _many_tools_lib = None
 _many_distance_lib = None
+_many_search_lib = None
 
 def _load(path, tables):
   """ The library at `path` with the signatures of `tables` bound; LibraryError when it is missing or stale. """
@@ -328,8 +350,19 @@ def many_distance_lib():
   many_lib()                     # libbyzagg.so and libbyzagg_many.so first: the sixth library links against both
   with _lock:
     if _many_distance_lib is None:
-      _many_distance_lib = _load(many_distance_library_path(), (MANY_DISTANCE_SIGNATURES,))
+      _many_distance_lib = _load(many_distance_library_path(), (MANY_DISTANCE_SIGNATURES, MANY_DISTANCE_TABLE_SIGNATURES))
   return _many_distance_lib
+
+def many_search_lib():
+  """ The seventh library, libbyzagg_many_search.so (loads it on first use; no fallback when it is missing). """
+  global _many_search_lib
+  if _many_search_lib is not None:
+    return _many_search_lib
+  many_distance_lib()            # the first, fourth and sixth libraries first: the seventh links against them
+  with _lock:
+    if _many_search_lib is None:
+      _many_search_lib = _load(many_search_library_path(), (MANY_SEARCH_SIGNATURES,))
+  return _many_search_lib
 
 def check(code, what):
   """ Raise on a non-zero return code of a bz_* call. """
@@ -344,8 +377,10 @@ def check(code, what):
     message = many_lib().bz_coordinate_many_last_error()
   elif what in MANY_TOOLS_SIGNATURES:
     message = many_tools_lib().bz_many_tools_last_error()
-  elif what in MANY_DISTANCE_SIGNATURES:
+  elif what in MANY_DISTANCE_SIGNATURES or what in MANY_DISTANCE_TABLE_SIGNATURES:
     message = many_distance_lib().bz_distance_many_last_error()
+  elif what in MANY_SEARCH_SIGNATURES:
+    message = many_search_lib().bz_distance_line_search_many_last_error()
   else:
     message = lib().bz_last_error()
   message = message.decode("utf-8", "replace") if message else ""

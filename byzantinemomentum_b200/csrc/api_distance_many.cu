@@ -8,6 +8,7 @@
 
 #include "distance_many.cuh"
 #include "../../include/byzagg_distance_many.h"
+#include "../../include/byzagg_distance_many_table.h"
 
 namespace bz {
 
@@ -61,6 +62,7 @@ constexpr size_t kOffOrder = 256;
 constexpr size_t kOffScores = kOffOrder + kMaxNMany * sizeof(int32_t);
 constexpr size_t kOffTable = kOffScores + kMaxNMany * sizeof(double);
 static_assert(kOffTable % 256 == 0, "the table starts 256-byte aligned");
+static_assert(kOffTable == BZ_DISTANCE_MANY_TABLE_OFFSET, "byzagg_distance_many_table.h states the table's offset");
 static_assert((size_t)kMaxRowParts * kMaxNMany <= (size_t)kMaxPairBlocks * kPairBlock, "K2'-many's blocks fit");
 
 static size_t many_distance_bytes(int n) {
@@ -125,45 +127,25 @@ static int cge_count(int n, int f) {
   return count;
 }
 
-// Unique rows by address, in order of first appearance (dedupe_rows' numbering), through an open-addressing table.
-static int dedupe_many(const float* const* rows, int n, const float** uniq, unsigned short* to_unique) {
-  constexpr int kSlots = 2 * kMaxNMany;
-  int slot[kSlots];
-  for (int s = 0; s < kSlots; ++s) slot[s] = -1;
-  int u = 0;
-  for (int i = 0; i < n; ++i) {
-    int h = (int)((((uintptr_t)rows[i] >> 2) * 0x9E3779B97F4A7C15ull) >> 53);     // 11 bits
-    while (slot[h] >= 0 && uniq[slot[h]] != rows[i]) h = (h + 1) & (kSlots - 1);
-    if (slot[h] < 0) {
-      slot[h] = u;
-      uniq[u++] = rows[i];
-    }
-    to_unique[i] = (unsigned short)slot[h];
-  }
+// The unique rows of the call (dedupe_many) and the map of the original rows to them.
+static int alias_map(const float* const* rows, int n, ManyRowTable& ut, ManyAliasMap& map) {
+  const float* uniq[kMaxNMany];
+  const int u = dedupe_many(rows, n, uniq, map.to_unique);
+  for (int i = n; i < kMaxNMany; ++i) map.to_unique[i] = 0;
+  for (int k = 0; k < kMaxNMany; ++k) ut.p[k] = uniq[k < u ? k : 0];
   return u;
 }
 
-// Multi-Krum or Bulyan above kMaxNDistance rows, after the checks: K2-many over the unique rows, K5-many, then the
-// average of the m selected rows or K4-many.
-static int run_pairwise(int rule, const float* const* rows, int n, int f, int m, int count, int64_t d, float* out,
-                        int32_t* order, int32_t* status, char* ws, cudaStream_t st) {
+// "Select" of Multi-Krum or Bulyan above kMaxNDistance rows: K5-many from the u x u table the workspace holds, then
+// the average of the m selected rows or K4-many.  The ticket is zero on entry.
+static int run_select(int rule, const float* const* rows, int n, int f, int m, int count, int64_t d, float* out,
+                      int32_t* order, int32_t* status, char* ws, const ManyAliasMap& map, int u, cudaStream_t st) {
   const bool bulyan = rule == BZ_RULE_BULYAN;
-  const float* uniq[kMaxNMany];
-  ManyAliasMap map;
-  const int u = dedupe_many(rows, n, uniq, map.to_unique);
-  for (int i = n; i < kMaxNMany; ++i) map.to_unique[i] = 0;
-  ManyRowTable ut;
-  for (int k = 0; k < kMaxNMany; ++k) ut.p[k] = uniq[k < u ? k : 0];
   unsigned* ticket = reinterpret_cast<unsigned*>(ws);
   int32_t* ord = order != nullptr ? order : reinterpret_cast<int32_t*>(ws + kOffOrder);
   int32_t* stat = !bulyan ? nullptr : status != nullptr ? status : reinterpret_cast<int32_t*>(ws + kOffStatus);
   double* scores = reinterpret_cast<double*>(ws + kOffScores);
-  double* table = reinterpret_cast<double*>(ws + kOffTable);
-  double* parts = reinterpret_cast<double*>(ws + round256(kOffTable + (size_t)n * n * sizeof(double)));   // 16-byte stores
-  cudaMemsetAsync(ticket, 0, sizeof(unsigned), st);
-  if (int rc = check_launch("memset")) return rc;
-  launch_pairdist_many(ut, u, d, pair_grid(u, d), parts, table, st);
-  if (int rc = check_launch("k2_pairdist_many")) return rc;
+  const double* table = reinterpret_cast<const double*>(ws + kOffTable);
   launch_select_many(table, map, n, u, count, scores, ord, stat, f, m, bulyan ? 1 : 0, ticket, st);
   if (int rc = check_launch("k5_select_many")) return rc;
   ManyRowTable t;
@@ -174,6 +156,23 @@ static int run_pairwise(int rule, const float* const* rows, int n, int f, int m,
   }
   launch_average_many(t, make_geom(rows, n, out, nullptr, d, 4), ord, m, 1, (float)m, out, st);
   return check_launch("k3_average_many");
+}
+
+// Multi-Krum or Bulyan above kMaxNDistance rows, after the checks: "pairs" (K2-many over the unique rows into the
+// table), then "select".
+static int run_pairwise(int rule, const float* const* rows, int n, int f, int m, int count, int64_t d, float* out,
+                        int32_t* order, int32_t* status, char* ws, cudaStream_t st) {
+  ManyRowTable ut;
+  ManyAliasMap map;
+  const int u = alias_map(rows, n, ut, map);
+  unsigned* ticket = reinterpret_cast<unsigned*>(ws);
+  double* table = reinterpret_cast<double*>(ws + kOffTable);
+  double* parts = reinterpret_cast<double*>(ws + round256(kOffTable + (size_t)n * n * sizeof(double)));   // 16-byte stores
+  cudaMemsetAsync(ticket, 0, sizeof(unsigned), st);
+  if (int rc = check_launch("memset")) return rc;
+  launch_pairdist_many(ut, u, d, pair_grid(u, d), parts, table, st);
+  if (int rc = check_launch("k2_pairdist_many")) return rc;
+  return run_select(rule, rows, n, f, m, count, d, out, order, status, ws, map, u, st);
 }
 
 // Aksel or CGE above kMaxNDistance rows, after the checks: Aksel's centre is bz_coordinate_many's median written into
@@ -227,6 +226,31 @@ int bz_distance_many(int rule, const float* const* rows, int n, int f, int m, in
   if (rule == BZ_RULE_KRUM || rule == BZ_RULE_BULYAN)
     return run_pairwise(rule, rows, n, f, m, count, d, out, order, status, base, st);
   return run_rowkeys(rule, rows, n, f, count, d, out, order, base, st);
+}
+
+int bz_distance_many_select(int rule, const float* const* rows, int n, int f, int m, int64_t d, float* out,
+                            int32_t* order, int32_t* status, void* ws, size_t ws_bytes, void* stream) {
+  static const char* who = "bz_distance_many_select";
+  if (rule != BZ_RULE_KRUM && rule != BZ_RULE_BULYAN)
+    return fail(BZ_EINVAL, "%s: rule %d, expected BZ_RULE_KRUM or BZ_RULE_BULYAN", who, rule);
+  if (int rc = check_call(rule, rows, n, d, out, who)) return rc;
+  if (n <= BZ_MAX_N_DISTANCE)
+    return fail(BZ_EUNSUPPORTED, "%s: n = %d, expected BZ_MAX_N_DISTANCE < n <= BZ_MAX_N_MANY", who, n);
+  int count;
+  if (int rc = check_rule(rule, n, f, m, BZ_AKSEL_MID, count, who)) return rc;
+  const size_t need = many_distance_bytes(n);
+  if (ws == nullptr || ((uintptr_t)ws % 8) != 0 || ws_bytes < need)
+    return fail(BZ_EWORKSPACE, "%s: workspace of %zu bytes at %p is too small or misaligned (need %zu, 8-byte aligned)",
+                who, ws_bytes, ws, need);
+  if (d == 0) return BZ_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  char* base = static_cast<char*>(ws);
+  ManyRowTable ut;
+  ManyAliasMap map;
+  const int u = alias_map(rows, n, ut, map);
+  cudaMemsetAsync(base, 0, sizeof(unsigned), st);
+  if (int rc = check_launch("memset")) return rc;
+  return run_select(rule, rows, n, f, m, count, d, out, order, status, base, map, u, st);
 }
 
 }  // extern "C"

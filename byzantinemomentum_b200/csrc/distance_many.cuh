@@ -25,15 +25,59 @@ constexpr int kPairTargetCtas = 396;                // three CTAs on each of the
 constexpr int kMaxPairTiles = kMaxNMany / kPairTile;
 constexpr int kMaxPairBlocks = kMaxPairTiles * (kMaxPairTiles + 1) / 2 > kPairTargetCtas
                                ? kMaxPairTiles * (kMaxPairTiles + 1) / 2 : kPairTargetCtas;
+constexpr int kPairChunk = 32;                      // columns per stage: every fp32 sum holds at most 32 squares
+constexpr int kMinSliceChunks = 8;                  // a slice keeps the ring busy for at least 8 chunks
 struct PairGrid {
   int tiles, npairs, slices;
   int64_t slice_chunks;                             // 32-column chunks per slice (the last may have fewer)
 };
-PairGrid pair_grid(int u, int64_t d);
+// The slices of K2-many over u unique rows: part of the bit contract (a pair's sum is added slice by slice), so that
+// every pass over these rows, K2-star-many's included, takes them from here.
+inline PairGrid pair_grid(int u, int64_t d) {
+  PairGrid g;
+  g.tiles = (u + kPairTile - 1) / kPairTile;
+  g.npairs = g.tiles * (g.tiles + 1) / 2;
+  const int64_t chunks = (d + kPairChunk - 1) / kPairChunk;
+  int64_t slices = kPairTargetCtas / g.npairs;
+  const int64_t most = (chunks + kMinSliceChunks - 1) / kMinSliceChunks;
+  if (slices > most) slices = most;
+  if (slices < 1) slices = 1;
+  g.slice_chunks = (chunks + slices - 1) / slices;
+  if (g.slice_chunks < 1) g.slice_chunks = 1;
+  g.slices = (int)((chunks + g.slice_chunks - 1) / g.slice_chunks);
+  if (g.slices < 1) g.slices = 1;
+  return g;
+}
+
+// Unique rows by address, in order of first appearance (dedupe_rows' numbering), through an open-addressing table.
+inline int dedupe_many(const float* const* rows, int n, const float** uniq, unsigned short* to_unique) {
+  constexpr int kSlots = 2 * kMaxNMany;
+  int slot[kSlots];
+  for (int s = 0; s < kSlots; ++s) slot[s] = -1;
+  int u = 0;
+  for (int i = 0; i < n; ++i) {
+    int h = (int)((((uintptr_t)rows[i] >> 2) * 0x9E3779B97F4A7C15ull) >> 53);     // 11 bits
+    while (slot[h] >= 0 && uniq[slot[h]] != rows[i]) h = (h + 1) & (kSlots - 1);
+    if (slot[h] < 0) {
+      slot[h] = u;
+      uniq[u++] = rows[i];
+    }
+    to_unique[i] = (unsigned short)slot[h];
+  }
+  return u;
+}
 // K2-many, then the sum of each pair's slices in slice order into table[a * u + b] (a <= b, the diagonal is the
 // self distance: 0, or NaN for a row holding NaN / inf).
 void launch_pairdist_many(const ManyRowTable& uniq, int u, int64_t d, const PairGrid& g, double* parts, double* table,
                           cudaStream_t st);
+
+// ---- K2-star-many (k2_star_many.cu, in libbyzagg_many_search.so) --------------------------------------------
+// Column c = u - 1 of the table over the same u unique rows, the candidate last: table[a * u + c] for a <= c, with
+// the bits launch_pairdist_many writes there (the slices of pair_grid(u, d), each slice's chunk sums added in chunk
+// order, the slices in slice order).  `blocks` takes one fp64 sum per (slice, row): g.slices * u <= kStarBlocks.
+constexpr int kStarBlocks = kPairTargetCtas * kPairTile;
+void launch_star_many(const ManyRowTable& uniq, int u, int64_t d, const PairGrid& g, double* blocks, double* table,
+                      cudaStream_t st);
 
 // ---- K2'-many (k2_many.cu): one fp64 sum per row over the 1024-pointer table --------------------------------
 // Aksel (center != NULL): sum_k (x_i[k] - center[k])^2; CGE: sum_k x_i[k]^2.  Per-CTA blocks of n sums in `parts`

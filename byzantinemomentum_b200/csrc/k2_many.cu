@@ -28,13 +28,11 @@
 namespace bz {
 
 constexpr int kPairThreads = 256;
-constexpr int kPairChunk = 32;                      // columns per stage: every fp32 sum holds at most 32 squares
 constexpr int kPairStages = 3;
 constexpr int kPairLd = kPairTile + 4;              // floats per staged column: float4 reads stay aligned
 constexpr int kPairTileFloats = kPairChunk * kPairLd;
 constexpr int kPairStageFloats = 2 * kPairTileFloats;
 constexpr size_t kPairSmem = (size_t)kPairStages * kPairStageFloats * sizeof(float);
-constexpr int kMinSliceChunks = 8;                  // a slice keeps the ring busy for at least 8 chunks
 
 __global__ void __launch_bounds__(kPairThreads, 3)
 k2_pairdist_many(const __grid_constant__ ManyRowTable uniq, const int u, const int64_t d, const int tiles,
@@ -137,22 +135,6 @@ k2_pairsum_many(const double* __restrict__ parts, const int u, const int tiles, 
     for (int s = 1; s < slices; ++s) v += __ldcg(src + (size_t)s * npairs * kPairBlock);
     table[e] = v;
   }
-}
-
-PairGrid pair_grid(int u, int64_t d) {
-  PairGrid g;
-  g.tiles = (u + kPairTile - 1) / kPairTile;
-  g.npairs = g.tiles * (g.tiles + 1) / 2;
-  const int64_t chunks = (d + kPairChunk - 1) / kPairChunk;
-  int64_t slices = kPairTargetCtas / g.npairs;
-  const int64_t most = (chunks + kMinSliceChunks - 1) / kMinSliceChunks;
-  if (slices > most) slices = most;
-  if (slices < 1) slices = 1;
-  g.slice_chunks = (chunks + slices - 1) / slices;
-  if (g.slice_chunks < 1) g.slice_chunks = 1;
-  g.slices = (int)((chunks + g.slice_chunks - 1) / g.slice_chunks);
-  if (g.slices < 1) g.slices = 1;
-  return g;
 }
 
 void launch_pairdist_many(const ManyRowTable& uniq, int u, int64_t d, const PairGrid& g, double* parts, double* table,

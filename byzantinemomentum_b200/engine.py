@@ -692,20 +692,27 @@ class LineSearch:
   up to MAX_N_DISTANCE rows (honest + f_real): above MAX_N through `bz_distance_line_search`, with a workspace
   of its own, as `Plan` does.  With `many`, against the coordinate-wise rules it takes up to MAX_N_MANY rows through
   `bz_line_search_many` (libbyzagg_many_tools.so), which makes `bz_line_search`'s call up to MAX_N_COORDINATE rows; the
-  distance rules raise ValueError there.  Like `Plan`, `search()` only issues
+  distance rules raise ValueError there.  With `many_distance`, against krum, bulyan, aksel and cge it takes up to
+  MAX_N_MANY rows through `bz_distance_line_search_many` (libbyzagg_many_search.so), which makes
+  `bz_distance_line_search`'s call up to MAX_N_DISTANCE rows and, above, keeps the honest rows' distances of krum and
+  bulyan from one evaluation to the next; the other rules raise ValueError there.  Like `Plan`, `search()` only issues
   the call (no allocation, no synchronisation; `graph()` captures it) and holds what it reads and writes:
       byz     the candidate row; after the call the attack's Byzantine gradient for the chosen factor
       record  fp64 [2 * evals + 2]: (x_k, y_k) per evaluation, the chosen factor, then the status word
   `result()` reads `record` once and returns (factor, trace), raising where the plain rule raises. """
-  def __init__(self, gar, grad_honests, f_real, f_decl, grad_avg, grad_att, evals, negative=False, kind="identical", many=False):
+  def __init__(self, gar, grad_honests, f_real, f_decl, grad_avg, grad_att, evals, negative=False, kind="identical", many=False,
+               many_distance=False):
     if gar not in _SEARCH_RULES:
       raise KeyError(f"unknown aggregation rule {gar!r}")
     if kind not in _SEARCH_KINDS:
       raise ValueError(f"unknown attack kind {kind!r}, expected one of {sorted(_SEARCH_KINDS)}")
     if many and gar not in _RULE_CODES:
       raise ValueError(f"many=True takes the coordinate-wise rules {sorted(_RULE_CODES)}, not {gar!r}")
+    if many_distance and gar not in WIDE_DISTANCE:
+      raise ValueError(f"many_distance=True takes the distance rules {sorted(WIDE_DISTANCE)}, not {gar!r}")
     honest = list(grad_honests)
-    limit = _lib.MAX_N_MANY if many else _lib.MAX_N_DISTANCE if gar in WIDE_DISTANCE else search_max_rows(gar)
+    limit = (_lib.MAX_N_MANY if many or many_distance else _lib.MAX_N_DISTANCE if gar in WIDE_DISTANCE
+             else search_max_rows(gar))
     prep = _prepare(honest, limit=limit)
     if prep.to_cpu:
       raise ValueError("the line search takes CUDA tensors")
@@ -722,6 +729,9 @@ class LineSearch:
     n = prep.n + int(f_real)
     if many:
       self._fn, ws_bytes = _lib.many_tools_lib().bz_line_search_many, _lib.many_tools_lib().bz_line_search_many_workspace_bytes
+    elif many_distance:
+      search_lib = _lib.many_search_lib()
+      self._fn, ws_bytes = search_lib.bz_distance_line_search_many, search_lib.bz_distance_line_search_many_workspace_bytes
     elif n > _lib.MAX_N and gar in WIDE_DISTANCE:
       self._fn, ws_bytes = _lib.lib().bz_distance_line_search, _lib.lib().bz_distance_line_search_workspace_bytes
     else:
@@ -756,11 +766,12 @@ def _search_outcome(record, evals):
   values = host.tolist()
   return values[2 * evals], [(values[2 * k], values[2 * k + 1]) for k in range(evals)]
 
-def line_search(gar, grad_honests, f_real, f_decl, grad_avg, grad_att, evals, negative=False, kind="identical", many=False):
-  """ The attacks' factor search on the device (see `LineSearch`, and its `many` for the coordinate-wise rules up to
-  MAX_N_MANY rows).  Returns (factor, byz): the factor `tools.line_maximize` picks, a Python float, and the Byzantine
+def line_search(gar, grad_honests, f_real, f_decl, grad_avg, grad_att, evals, negative=False, kind="identical", many=False,
+                many_distance=False):
+  """ The attacks' factor search on the device (see `LineSearch`, its `many` for the coordinate-wise rules and its
+  `many_distance` for krum, bulyan, aksel and cge up to MAX_N_MANY rows).  Returns (factor, byz): the factor `tools.line_maximize` picks, a Python float, and the Byzantine
   gradient the attack returns for it, a device tensor (the reference returns it `f_real` times, aliased). """
-  search = LineSearch(gar, grad_honests, f_real, f_decl, grad_avg, grad_att, evals, negative, kind, many)
+  search = LineSearch(gar, grad_honests, f_real, f_decl, grad_avg, grad_att, evals, negative, kind, many, many_distance)
   byz = search()
   factor, _ = search.result()
   return factor, byz

@@ -21,7 +21,8 @@ routes lead there without touching a reference file:
 attack against CGE run on the device (`engine.anticge`).  The search takes the rows the entry takes: up to
 128 against a wide entry, and against a default entry as many as `bz_line_search` takes
 (`engine.search_max_rows`); with `install_attacks(..., many=True)`, up to 1024 against an entry of
-`install(..., many=True)`.
+`install(..., many=True)`, and with `install_attacks(..., many_distance=True)`, up to 1024 against an entry of
+`install(..., many_distance=True)`.
 """
 
 import math
@@ -37,6 +38,9 @@ _installed = {}
 # The entries of `_installed` that `install` took from `gars.many_gars`: `install_attacks(..., many=True)` searches against
 # them up to MAX_N_MANY rows.
 _many_installed = set()
+# The entries of `_installed` that `install` took from `gars.many_distance_gars`: `install_attacks(..., many_distance=True)`
+# searches against them up to MAX_N_MANY rows.
+_many_distance_installed = set()
 
 def _record(aggregators, key, name, rule):
   from . import engine, _lib
@@ -49,6 +53,10 @@ def _record(aggregators, key, name, rule):
       _many_installed.add(entry)
     else:
       _many_installed.discard(entry)
+    if many_distance_gars.get(name) is rule:
+      _many_distance_installed.add(entry)
+    else:
+      _many_distance_installed.discard(entry)
 
 def install(aggregators, prefix="b200-", override=False, names=None, wide=False, many=False, many_distance=False):
   """ Register the CUDA rules in the reference's `aggregators` module.
@@ -66,8 +74,9 @@ def install(aggregators, prefix="b200-", override=False, names=None, wide=False,
                  takes it to 1024; above, the stock attack runs and calls the entry for each evaluation.  The default,
                  False, keeps `gars`' entries, which stop at 128
     many_distance  Register krum, bulyan, aksel and cge from `gars.many_distance_gars`: up to 1024 gradients.  The
-                 attacks' device search against them stops at 128 rows, as against a wide entry; above, the stock
-                 attack runs and calls the entry for each evaluation.  Combines with `many`, not with `wide`
+                 attacks' device search against them keeps its 128 rows, as against a wide entry, unless
+                 `install_attacks(..., many_distance=True)` takes it to 1024; above, the stock attack runs and calls
+                 the entry for each evaluation.  Combines with `many`, not with `wide`
   Returns:
     List of the registered names
   """
@@ -120,12 +129,12 @@ def install_tools(tools, many=False):
 def _is_cuda(tensors):
   return all(t.is_cuda for t in tensors)
 
-def _device_rule(defense, grad_honests, f_real, f_decl, model, many=False):
+def _device_rule(defense, grad_honests, f_real, f_decl, model, many=False, many_distance=False):
   """ The name of the rule here that `defense` is, when the attack's search can run on the device:
   `defense` is an entry `install` registered, there are Byzantine rows to generate, every honest
   gradient is a float32 CUDA vector, the rule's input fits the search's row limit for that entry
   (128 rows for a wide entry of `install(..., wide=True)`; with `many`, 1024 rows for an entry of
-  `install(..., many=True)`; otherwise `engine.search_max_rows`: 128 rows for the coordinate-wise rules, 64 for
+  `install(..., many=True)`; with `many_distance`, 1024 rows for an entry of `install(..., many_distance=True)`; otherwise `engine.search_max_rows`: 128 rows for the coordinate-wise rules, 64 for
   the distance rules), and the rule accepts its parameters.  None otherwise: the stock attack then runs (and
   fails, if it must, as it always did). """
   import torch
@@ -136,7 +145,7 @@ def _device_rule(defense, grad_honests, f_real, f_decl, model, many=False):
   if installed is None or not isinstance(f_real, int) or f_real < 1 or not isinstance(grad_honests, list) or not grad_honests:
     return None
   name, limit = installed
-  if many and defense in _many_installed:
+  if (many and defense in _many_installed) or (many_distance and defense in _many_distance_installed):
     from . import _lib
     limit = _lib.MAX_N_MANY
   if len(grad_honests) + f_real > limit or not _is_cuda(grad_honests):
@@ -163,17 +172,19 @@ def _bulyan(grad_stck, grad_avg, target_idx=-1, **kwargs):
   return grad_att
 
 def _search(backend, rule, grad_honests, f_real, *args, **kwargs):
-  """ `backend.line_search(rule, grad_honests, f_real, *args, **kwargs)`, with `many=True` above MAX_N_COORDINATE rows
-  (only an entry of `install(..., many=True)` gets there, through `install_attacks(..., many=True)`). """
+  """ `backend.line_search(rule, grad_honests, f_real, *args, **kwargs)`, above MAX_N_COORDINATE rows with `many=True`
+  for a coordinate-wise rule (only an entry of `install(..., many=True)` gets there, through
+  `install_attacks(..., many=True)`) and `many_distance=True` for krum, bulyan, aksel and cge (only an entry of
+  `install(..., many_distance=True)` gets there, through `install_attacks(..., many_distance=True)`). """
   from . import _lib
   if len(grad_honests) + f_real > _lib.MAX_N_COORDINATE:
-    kwargs["many"] = True
+    kwargs["many_distance" if rule in many_distance_gars else "many"] = True
   return backend.line_search(rule, grad_honests, f_real, *args, **kwargs)
 
-def _identical(stock, direction, backend, many=False):
+def _identical(stock, direction, backend, many=False, many_distance=False):
   """ attacks/identical.py:46-86 with the factor search on the device. """
   def attack(grad_honests, f_real, f_decl, defense, model, factor=-16, negative=False, **kwargs):
-    rule = _device_rule(defense, grad_honests, f_real, f_decl, model, many) if factor < 0 else None
+    rule = _device_rule(defense, grad_honests, f_real, f_decl, model, many, many_distance) if factor < 0 else None
     if rule is None:
       return stock(grad_honests=grad_honests, f_real=f_real, f_decl=f_decl, defense=defense, model=model,
                    factor=factor, negative=negative, **kwargs)
@@ -186,10 +197,10 @@ def _identical(stock, direction, backend, many=False):
     return [byz] * f_real
   return attack
 
-def _empire_strict(stock, backend, many=False):
+def _empire_strict(stock, backend, many=False, many_distance=False):
   """ attacks/empire.py:29-65 with the epsilon search on the device. """
   def attack(grad_honests, f_real, f_decl, defense, model, epsilon=1, **kwargs):
-    rule = _device_rule(defense, grad_honests, f_real, f_decl, model, many) if epsilon < 0 else None
+    rule = _device_rule(defense, grad_honests, f_real, f_decl, model, many, many_distance) if epsilon < 0 else None
     if rule is None:
       return stock(grad_honests=grad_honests, f_real=f_real, f_decl=f_decl, defense=defense, model=model,
                    epsilon=epsilon, **kwargs)
@@ -216,7 +227,7 @@ def _anticge(stock, backend):
 
 _ATTACK_NAMES = ("little", "empire", "bulyan", "empire-strict")
 
-def install_attacks(attacks, backend=None, names=None, many=False):
+def install_attacks(attacks, backend=None, names=None, many=False, many_distance=False):
   """ Replace `little`, `empire`, `bulyan` and `empire-strict` in the reference's `attacks` registry
   (attacks/__init__.py: `attacks`, `register`) with versions that, when the factor (epsilon) is negative
   and `defense` is a rule `install` registered, run the whole `line_maximize` search on the device and
@@ -233,6 +244,9 @@ def install_attacks(attacks, backend=None, names=None, many=False):
     names    Attacks to replace (default: the four line-searching ones)
     many     Against an entry of `install(..., many=True)`, search on the device up to 1024 rows, above 128 through
              `backend.line_search(..., many=True)`.  The default, False, keeps the search at 128 rows there
+    many_distance  Against an entry of `install(..., many_distance=True)`, search on the device up to 1024 rows, above
+             128 through `backend.line_search(..., many_distance=True)`.  The default, False, keeps the search at
+             128 rows there.  Combines with `many`
   Returns:
     List of the replaced names """
   if backend is None:
@@ -246,9 +260,9 @@ def install_attacks(attacks, backend=None, names=None, many=False):
     if name == "anticge":
       attack = _anticge(stock.unchecked, backend)
     elif name == "empire-strict":
-      attack = _empire_strict(stock.unchecked, backend, many)
+      attack = _empire_strict(stock.unchecked, backend, many, many_distance)
     elif name in directions:
-      attack = _identical(stock.unchecked, directions[name], backend, many)
+      attack = _identical(stock.unchecked, directions[name], backend, many, many_distance)
     else:
       raise KeyError(f"no device version of the attack {name!r}")
     del attacks.attacks[name]                  # `register` refuses duplicates
